@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- SD1.5 LoRA-r4 512px training step (BASELINE.json configs[1]) on N x B200.
+"""bench.py -- SD1.5 LoRA-r4 512px training step (BASELINE.json configs[1]) on N x H100.
 
   python bench.py --gpus N --steps K --warmup W            (N > 1: launched under torchrun)
   python bench.py --impl reference ...                     (the reference's CPU path, oracle port)
@@ -12,7 +12,7 @@ random-initialised SD1.5-shaped weights (no datasets or checkpoints offline).
 
 Prints ONE JSON line (rank 0). `value` = images/s with inputs resident in HBM; `e2e` = the same
 through the public step_host() call with pinned-host inputs (H2D) and a D2H loss read per step;
-`roofline` = the fused tcgen05 LoRA-linear kernel (all 384 fwd + dX launches of one step, real
+`roofline` = the fused wgmma LoRA-linear kernel (all 384 fwd + dX launches of one step, real
 site shapes) timed live with CUDA events: algorithmic bytes / time vs the measured HBM peak;
 `cpu_baseline` = the oracle port of the reference's step on the host cores (rank 0, N = 1).
 """
@@ -52,7 +52,7 @@ def bench_config(args, world, lora_sites=None, lora_params=None):
         wl = WORKLOAD
     return {"workload": wl, "extended": bool(args.extended), "resolution": args.res, "rank": args.rank,
             "global_batch": world, "parallelism": f"dp{world}",
-            "l2": "working set per step (>=1.7 GB frozen weights + activations) exceeds the 126 MB L2; no explicit flush"}
+            "l2": "working set per step (>=1.7 GB frozen weights + activations) exceeds the 50 MB L2; no explicit flush"}
 
 
 def load_peaks():
@@ -60,8 +60,8 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as fh:
             d = json.load(fh)
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -156,7 +156,7 @@ def site_shapes(model, tokens_by_module):
 
 
 def fused_linear_bytes(M, K, N, r, bias, e=2):
-    """SURVEY.md 8(d): algorithmic bytes of one fused LoRA-linear launch (16-bit operands):
+    """Algorithmic bytes of one fused LoRA-linear launch (16-bit operands):
     X + W + down + up + Y (+ bias fp32) (+ T fp32 [M,16] side output)."""
     return e * (M * K + N * K + r * K + M * N) + 4 * N * r + (4 * N if bias else 0) + 4 * M * 16
 
@@ -255,7 +255,7 @@ def roofline_sweep(trainer, families, iters=10, eager_once=False):
 
 
 def conv_bytes(n, cin, cout, k, H, W, r, e=2):
-    """SURVEY.md 8(d): a conv site counts the activation ONCE (not im2col-expanded): X + W + down + Y
+    """A conv site counts the activation ONCE (not im2col-expanded): X + W + down + Y
     (16-bit) + up (fp32) + bias (fp32) + T [pixels,16] fp32."""
     P, taps = n * H * W, k * k
     return e * (P * cin + cout * taps * cin + r * taps * cin + P * cout) + 4 * cout * r + 4 * cout + 4 * P * 16
@@ -372,7 +372,7 @@ def run_native(args):
         L.inject_trainable_lora(unet, r=args.rank)
     L.inject_trainable_lora(text, target_replace_module={"CLIPAttention"}, r=args.rank)
     # reference init has up = 0 (lora.py:51); give the up factors small non-zero values so the
-    # LoRA branch and all three gradients are numerically exercised (SURVEY.md 8d)
+    # LoRA branch and all three gradients are numerically exercised
     g = torch.Generator(device=dev).manual_seed(1)
     for m in list(unet.modules()) + list(text.modules()):
         if type(m).__name__ in ("LoraInjectedLinear", "LoraInjectedConv2d"):
@@ -443,6 +443,8 @@ def run_native(args):
     ms_dev = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
     loss_dev = float(trainer.loss.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, trainer)
 
     # ---------------- end-to-end timing (public step_host API, pinned host inputs, D2H loss)
     for i in range(3):
@@ -469,11 +471,6 @@ def run_native(args):
         hbm_peak, peak_src = load_peaks()
         rb, rms, n_l = roofline_sweep(trainer, fams)
         achieved = rb / (rms * 1e-3) / 1e9
-        traffic = None   # DRAM bytes of the same 384 launches, from the committed ncu capture
-        tpath = os.path.join(ROOT, "profiles", "fused_linear_dram_traffic.json")
-        if os.path.exists(tpath) and not args.tiny and not args.extended and args.res == 512 and args.rank == 4:
-            with open(tpath) as fh:
-                traffic = json.load(fh).get("dram_bytes_per_sweep")
         value = world * args.steps / (ms_dev * 1e-3)
         conv_roof = None
         if args.extended and conv_seen:
@@ -504,10 +501,10 @@ def run_native(args):
             "gpu_launches": int(launches_per_step * args.steps * 2),
             "gpu_launches_per_step": int(launches_per_step),
             "clocks": clocks,
-            "roofline": {"bound": "hbm", "kernel": "fused_lora_kernel / fused_lora_grouped_kernel / fused_lora_persistent_kernel: every forward + dX launch of the fused LoRA-linear path in one step (families grouped as in the step)",
+            "roofline": {"bound": "hbm", "kernel": "fused_lora_kernel / fused_lora_grouped_kernel: every forward + dX launch of the fused LoRA-linear path in one step (families grouped as in the step)",
                          "sites": 2 * len(shapes),
                          "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
-                         "frac": achieved / hbm_peak, "traffic": traffic,
+                         "frac": achieved / hbm_peak,
                          "launches": n_l, "algorithmic_bytes": rb, "ms_per_sweep": rms,
                          "avg_launch_us": rms * 1e3 / n_l,
                          "share_of_step": rms / (ms_dev / args.steps), "peak_source": peak_src},
@@ -529,6 +526,22 @@ def run_native(args):
         dist.barrier()
         dist.destroy_process_group()
     return out
+
+
+def dump_outputs(out_dir, trainer, max_bytes=64 << 20):
+    """Write what the last timed step computed as DIR/<name>.npy (float32): its loss, the gradient
+    norm it clipped with, and the LoRA factors AdamW left in the arena. An array too large for its
+    share of `max_bytes` is cut to a fixed, seeded sample of its elements, the same in every run."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": trainer.loss, "grad_norm": trainer.arena.gnorm, "lora_params": trainer.arena.p}
+    cap = max_bytes // (4 * len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().reshape(-1).cpu()
+        if a.numel() > cap:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:cap].sort().values
+            a = a[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.numpy())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -574,7 +587,7 @@ def cpu_reference(res, rank_r, budget_s=30.0, max_steps=None, warmup=1, tiny=Fal
 
 
 def cuda_reference(dev, args, steps, warmup):
-    """The reference's LoRA path on the SAME B200: its operator modules (oracle/ref_modules.py, the
+    """The reference's LoRA path on the SAME GPU: its operator modules (oracle/ref_modules.py, the
     three-GEMM + elementwise torch formulation of lora.py:53-58,130-135) injected into the same host
     models, its step (oracle/ref_step.py: torch.optim.AdamW + clip_grad_norm_), torch eager -- the
     stock way the reference runs on a GPU. Also timed as ONE CUDA-graph replay per step (something
@@ -725,6 +738,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-cuda-baseline", action="store_true", help="skip the reference-on-this-GPU block")
     ap.add_argument("--cpu-budget", type=float, default=25.0, help="seconds of CPU-baseline work")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss, gradient norm and LoRA factors as DIR/<name>.npy")
     args = ap.parse_args()
     out = (run_reference(args) if args.impl == "reference" else
            run_reference_cuda(args) if args.impl == "reference-cuda" else run_native(args))

@@ -1,4 +1,4 @@
-/* lora_b200 C-ABI: the drop-in boundary for the LoRA hot path of cloneofsimo/lora on B200 (sm_100a).
+/* lora_b200 C-ABI: the drop-in boundary for the LoRA hot path of cloneofsimo/lora on H100 (sm_90a).
  *
  * Plain C: raw device pointers, sizes, dtype enums and a cudaStream_t passed as void*. No torch
  * or ATen types cross this boundary. Every entry point enqueues work on `stream` and returns an
@@ -38,14 +38,13 @@ enum lb_dtype { LB_BF16 = 0, LB_F16 = 1, LB_F32 = 2 };
  * entry) is NOT row-major [N, K] but the 64 x 64-block layout written by lb_tile_weight -- block
  * (n64, kb) occupies rows [(n64 * ceil(K/64) + kb) * 64, +64) of a [rows, 64] 16-bit tensor, zero padded
  * -- so that every TMA box of the weight stream is one contiguous 8 KB run of HBM (a row-major box is
- * 64-192 rows of 128 bytes a whole K apart). Optional: measured on B200 against row-major on every
- * SD1.5 site shape it is neither faster nor slower (profiles/r2h_site_table_tiled_vs_rowmajor.md). */
+ * 64-192 rows of 128 bytes a whole K apart). Optional; off by default. */
 #define LB_W_TILED 0x100
 
 /* ABI version of this header (bumped on any signature change). */
 int lb_abi_version(void);
 
-/* Fused frozen linear + LoRA forward (tcgen05/TMEM/TMA), one launch:
+/* Fused frozen linear + LoRA forward (wgmma/TMA), one launch:
  *     Y[M,N] = X[M,K] . W[N,K]^T (+ bias[N]) + ((X . down16^T) * (scale * diag)) . up^T
  * up element (n, j) is read from the fp32 master at up[n*up_rs + j*up_cs]; diag is the optional
  * selector diagonal [r] (NULL = identity); T_out (NULL = skip) receives X . down16^T (unscaled);
@@ -67,7 +66,7 @@ int lb_lora_linear_fwd(const void* X, const void* W, const float* bias, const vo
  * training mode, p > 0 -- the state of every site built by inject_trainable_lora_extended and the
  * monkeypatch_* loaders), still ONE launch:
  *     Y = X . W^T (+ bias) + keep(m,n)/(1-p) * (((X . down16^T) * (scale * diag)) . up^T)[m,n]
- * The LoRA product keeps its own TMEM columns and the keep-mask (csrc/dropmask.cuh: a counter hash
+ * The LoRA product keeps its own accumulator and the keep-mask (csrc/dropmask.cuh: a counter hash
  * of (*seed_dev, m*N + n); seed_dev points to one uint64 in DEVICE memory so that a captured graph
  * draws a new mask per replay) is applied while the tile is drained. Backward recomputes the same
  * mask: lb_lora_dropout_dt, lb_lora_wgrad_masked / lb_lora_wgrad_pair(drop_p). */
@@ -82,8 +81,9 @@ int lb_lora_linear_fwd_dropout(const void* X, const void* W, const float* bias, 
  * with gY [M, N_out], Wt = W^T [K_in, N_out] (pre-transposed frozen weight), upT16 = B^T padded [16, N_out],
  * `down` = A read transposed (element (k, j) at down[k*down_rs + j*down_cs]: down_rs = 1, down_cs = K_in).
  * The mask (same counter hash as the forward, element index m*N_out + n) is applied to a shared-memory
- * copy of every gY tile by the otherwise idle epilogue warps and feeds only the rank-r MMA -- no
- * separate pass over gY (round 1: lb_lora_dropout_dt + T_in). dA then is lb_lora_wgrad(X, T_out) with
+ * copy of every gY tile by the consumer warpgroups inside the MMA loop (one named barrier per K
+ * block) and feeds only the rank-r MMA -- no separate pass over gY (the alternative is
+ * lb_lora_dropout_dt + T_in). dA then is lb_lora_wgrad(X, T_out) with
  * scale / (1-p); dB the masked reduction. */
 int lb_lora_linear_dx_dropout(const void* gY, const void* Wt, const void* upT16, const float* down,
                               long long down_rs, long long down_cs, const float* diag, float scale,
@@ -92,7 +92,7 @@ int lb_lora_linear_dx_dropout(const void* gY, const void* Wt, const void* upT16,
 
 /* Up to 4 independent lb_lora_linear_fwd problems of the same operand/output dtype in ONE launch
  * (sites that share an input -- q/k/v of a self-attention, k/v of a cross-attention, CLIP's k/v/q --
- * each under-fill 148 SMs on their own). All array arguments are HOST arrays of length n; per-problem
+ * each under-fill 132 SMs on their own). All array arguments are HOST arrays of length n; per-problem
  * semantics are exactly lb_lora_linear_fwd's (T_in unsupported). */
 int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W,
                                const float* const* bias, const void* const* down16,
@@ -103,17 +103,16 @@ int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W
 
 /* Benchmark/profiling knob: tile schedule of lb_lora_linear_fwd.
  *   mode = schedule + 4 * block_n + 16 * split
- *   schedule: 0 = auto (default), 1 = one tile per CTA, 2 = persistent CTAs with double-buffered
- *             TMEM accumulators, 3 = EXPERIMENTAL cluster split-K (csrc/fused_splitk.cuh; never
- *             chosen by `auto`)
- *   block_n:  0 = auto, 1 = 64, 2 = 128
- *   split:    (schedule 3 only) 0 = auto (4), 1..3 = 2..4 CTAs of one cluster share a tile's K loop */
+ *   schedule: 0 = auto (default), 1 and 2 = one tile per CTA, 3 = split-K with the partials
+ *             reduced at L2 (never chosen by `auto` for these shapes)
+ *   block_n:  0 = auto, 1 = 64, 2 = 128, 3 = 192 (16-bit outputs)
+ *   split:    (schedule 3 only) 0 = auto (4), 1..3 = 2..4 CTAs share a tile's K loop */
 int lb_debug_set_linear_mode(int mode);
 /* Profiling knob: device buffer (16 x uint64) receiving %globaltimer phase stamps of CTA (0,0) of
  * subsequent lb_lora_linear_fwd launches; NULL switches it off. */
 int lb_debug_set_stamp_buffer(void* dev_buf);
 /* Programmatic dependent launch for the fused kernels (cudaLaunchAttributeProgrammaticStream-
- * Serialization): the prologue of a launch (barrier init, TMEM allocation, descriptor prefetch)
+ * Serialization): the prologue of a launch (barrier init, descriptor prefetch)
  * overlaps the tail of the previous kernel in the stream. 0 = off, 1 = on; initial value from the
  * environment variable LB_PDL. */
 int lb_debug_set_pdl(int on);
@@ -203,7 +202,7 @@ int lb_lora_wgrad_conv(const void* S, const float* V, const float* diag, float s
                        int C, int r, int H, int W, int kh, int kw, int pad_h, int pad_w, int in_dtype,
                        void* stream);
 
-/* Fused frozen Conv2d + LoRA (NHWC implicit GEMM on tcgen05; stride 1, dilation 1, groups 1,
+/* Fused frozen Conv2d + LoRA (NHWC implicit GEMM on wgmma; stride 1, dilation 1, groups 1,
  * 1x1 or 3x3 "same" padding -- the ResnetBlock2D sites of SD1.5):
  *     Y[n,h,w,:] = sum_tap X[n,h+ty-pad,w+tx-pad,:] . W[:, tap, :]^T (+ bias)
  *                  + ((sum_tap X[..] . down16[:, tap, :]^T) * (scale*diag)) . up^T
@@ -357,7 +356,7 @@ int lb_refresh_shadows(const float* p, const long long* table, int n_entries, in
  * matrices. Tall-skinny operands are fp32 row-major [batch, rows, 32]. See lora_b200/svd.py for
  * the driver (probe -> power iterations with CholeskyQR2 -> 32x32 Jacobi -> factors). */
 /* SVD distillation of cli_svd.py:24-92 (`overwrite_base`) for ALL sites of a model in one call,
- * ragged over shapes (SURVEY.md 8b `lora_svd_truncated_batched`): for b < batch,
+ * ragged over shapes: for b < batch,
  *   dW = Wt[b] - Wb[b]  ([N[b], K[b]] row-major, w_dtype in {LB_F32, LB_BF16, LB_F16}; Wb NULL or
  *   Wb[b] ignored when the array is NULL: dW = Wt[b]) -> top-`rank` singular triplets by a
  *   randomized range finder (32 probes, `power_iters` power iterations = 2*power_iters+2 streaming

@@ -30,11 +30,11 @@ def _load():
         except Exception as e:  # nvcc missing or compile error: there is nothing to fall back to
             raise LoraB200Error(
                 f"{LIB_PATH} is missing and building it failed ({e}); run `python -m lora_b200.build` "
-                "(nvcc, sm_100a). lora_b200 has no fallback path.") from e
+                "(nvcc, sm_90a). lora_b200 has no fallback path.") from e
     if not os.path.exists(LIB_PATH):
         raise LoraB200Error(
             f"{LIB_PATH} is missing: build it with `python -m lora_b200.build` "
-            "(nvcc, sm_100a). lora_b200 has no fallback path."
+            "(nvcc, sm_90a). lora_b200 has no fallback path."
         )
     lib = ctypes.CDLL(LIB_PATH)
     vp, ll, i32, f32 = ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_float

@@ -1,5 +1,5 @@
-"""lora_b200 -- Blackwell-native (sm_100a) LoRA fine-tuning hot path behind the API of
-cloneofsimo/lora (`lora_diffusion`). See DESIGN.md / INTEGRATION.md."""
+"""lora_b200 -- Hopper-native (sm_90a) LoRA fine-tuning hot path behind the API of
+cloneofsimo/lora (`lora_diffusion`). See INTEGRATION.md."""
 from .lora import *  # noqa: F401,F403
 from .lora import (_find_children, _find_modules, _find_modules_v2, _text_lora_path,  # noqa: F401
                    _ti_lora_path)

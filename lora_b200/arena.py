@@ -1,6 +1,6 @@
 """Flat LoRA-parameter arena + fused clip/AdamW step + data-parallel gradient exchange.
 
-B200-first replacement for what the reference gets from torch.optim.AdamW over 288-448 tiny
+GPU-first replacement for what the reference gets from torch.optim.AdamW over 288-448 tiny
 tensors, clip_grad_norm_ and DDP's bucketed allreduce
 (training_scripts/train_lora_dreambooth.py:651-676, 744-757, 877-888;
 lora_diffusion/cli_lora_pti.py:997, 606-609):
@@ -12,7 +12,7 @@ lora_diffusion/cli_lora_pti.py:997, 606-609):
   * data parallel: ONE NCCL all-reduce(sum) over `g` per step; the 1/world average, the
     global-norm clip coefficient, AdamW, gradient zeroing are one fused pass
     (lb_adamw_clip_step), followed by one batched refresh of the 16-bit operand copies the
-    tcgen05 kernels read (lb_refresh_shadows);
+    wgmma kernels read (lb_refresh_shadows);
   * nothing here synchronises the host, so a whole training step can be captured in a CUDA graph
     (learning rates and the step counter live in device memory).
 """

@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI library (nvcc, sm_100a only). No torch headers are involved.
+"""In-tree build of the C-ABI library (nvcc, sm_90a only). No torch headers are involved.
 
 `python -m lora_b200.build` or `__graft_entry__.build()`; output: lora_b200/liblora_b200.so
 (git-ignored, travels to the GPU box with the gpurun snapshot).
@@ -20,7 +20,7 @@ HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [
     os.path.join(ROOT, "include", "lora_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
     "-I", os.path.join(ROOT, "include"), "-I", CSRC,

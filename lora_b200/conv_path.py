@@ -21,7 +21,7 @@ def _geometry(conv):
     if not ok:
         raise LoraB200Error(
             f"LoraInjectedConv2d: unsupported geometry kernel={conv.kernel_size} stride={conv.stride} "
-            f"padding={conv.padding} dilation={conv.dilation} groups={conv.groups}; the sm_100a "
+            f"padding={conv.padding} dilation={conv.dilation} groups={conv.groups}; the sm_90a "
             "kernel covers stride-1 'same' 1x1/3x3 convs (the SD1.5 ResnetBlock2D sites)")
     return kh, kw, ph, pw
 

@@ -6,7 +6,7 @@
 // warps drain a 128 x BLOCK_N tile, pays 8 integer operations per element instead of a 64-bit
 // splitmix per element. The stream differs from ATen's Philox, so parity with the reference under
 // dropout is statistical (keep probability 1-p to 8e-6, survivors scaled by 1/(1-p), identical
-// mask in forward and backward), see DESIGN.md.
+// mask in forward and backward).
 #pragma once
 #include <stdint.h>
 

@@ -38,15 +38,16 @@ static int launch_conv(const void* X, const void* W, const void* Dn, void* Y, co
              ? LB_OK : LB_ERR_CUDA;
 }
 
-// Split-K plan for one conv problem (same cost model as the linear planner, fused_linear.cu: ~92
-// GB/s operand ingest per SM; K = taps x Cin runs to 23040 on the SD1.5 ResnetBlock2D sites while
+// Split-K plan for one conv problem (same cost model as the linear planner, fused_linear.cu; K = taps x
+// Cin runs to 23040 on the SD1.5 ResnetBlock2D sites while
 // the 8x8 / 16x16 levels have only 10-40 output tiles). g = T groups (1 forward, taps for dX).
 struct ConvPlan { int block_n, split; };
 static ConvPlan plan_conv_split(long long m_tiles, int num_kb, int N, int g, int n_sms) {
   if (!splitk_enabled() || n_sms <= 0) return {0, 1};
   ConvPlan best = {0, 1};
   double best_t = 1e30, base_t = 1e30;
-  for (int bn = 64; bn <= 128; bn += 64) {
+  {
+    const int bn = 64;   // split plans use BLOCK_N 64 (see plan_split in fused_linear.cu)
     const long long tiles = m_tiles * ((N + bn - 1) / bn);
     const double per_kb = (128.0 + bn + 16.0) * 128.0 / 92e3;
     const double waves = static_cast<double>((tiles + n_sms - 1) / n_sms);
@@ -125,11 +126,11 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
 #define LB_CONVMS(BN, ST, OT, GG) launch_conv<BN, ST, OT, GG, false, true, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, sp.split)
     if (sp.split > 1) {
       if (groups) {
-        if (out_dtype == LB_F32) return sp.block_n == 64 ? LB_CONVMS(64, 3, float, 9) : LB_CONVMS(128, 2, float, 9);
-        return sp.block_n == 64 ? LB_CONVMS(64, 3, uint16_t, 9) : LB_CONVMS(128, 3, uint16_t, 9);
+        if (out_dtype == LB_F32) return LB_CONVMS(64, 3, float, 9);
+        return LB_CONVMS(64, 3, uint16_t, 9);
       }
-      if (out_dtype == LB_F32) return sp.block_n == 64 ? LB_CONVMS(64, 4, float, 1) : LB_CONVMS(128, 3, float, 1);
-      return sp.block_n == 64 ? LB_CONVMS(64, 4, uint16_t, 1) : LB_CONVMS(128, 3, uint16_t, 1);
+      if (out_dtype == LB_F32) return LB_CONVMS(64, 4, float, 1);
+      return LB_CONVMS(64, 4, uint16_t, 1);
     }
     if (groups) {
       if (out_dtype == LB_F32) return narrow ? LB_CONVM(64, 3, float, 9) : LB_CONVM(128, 2, float, 9);
@@ -144,8 +145,8 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
 #define LB_CONVD(BN, OT) launch_conv<BN, 4, OT, 1, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
 #define LB_CONVDS(BN, OT) launch_conv<BN, 4, OT, 1, true, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, sp.split)
     if (sp.split > 1) {
-      if (out_dtype == LB_F32) return sp.block_n == 64 ? LB_CONVDS(64, float) : LB_CONVDS(128, float);
-      return sp.block_n == 64 ? LB_CONVDS(64, uint16_t) : LB_CONVDS(128, uint16_t);
+      if (out_dtype == LB_F32) return LB_CONVDS(64, float);
+      return LB_CONVDS(64, uint16_t);
     }
     if (out_dtype == LB_F32) return narrow ? LB_CONVD(64, float) : LB_CONVD(128, float);
     return narrow ? LB_CONVD(64, uint16_t) : LB_CONVD(128, uint16_t);
@@ -156,11 +157,11 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
     if (sp.split > 1) {
 #define LB_CONVS(BN, ST, OT, GG) launch_conv<BN, ST, OT, GG, false, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, sp.split)
       if (groups) {
-        if (out_dtype == LB_F32) return sp.block_n == 64 ? LB_CONVS(64, 4, float, 9) : LB_CONVS(128, 3, float, 9);
-        return sp.block_n == 64 ? LB_CONVS(64, 4, uint16_t, 9) : LB_CONVS(128, 4, uint16_t, 9);
+        if (out_dtype == LB_F32) return LB_CONVS(64, 4, float, 9);
+        return LB_CONVS(64, 4, uint16_t, 9);
       }
-      if (out_dtype == LB_F32) return sp.block_n == 64 ? LB_CONVS(64, 4, float, 1) : LB_CONVS(128, 4, float, 1);
-      return sp.block_n == 64 ? LB_CONVS(64, 4, uint16_t, 1) : LB_CONVS(128, 4, uint16_t, 1);
+      if (out_dtype == LB_F32) return LB_CONVS(64, 4, float, 1);
+      return LB_CONVS(64, 4, uint16_t, 1);
 #undef LB_CONVS
     }
   }

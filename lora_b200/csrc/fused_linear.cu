@@ -1,10 +1,8 @@
 // C-ABI entry point for the fused LoRA linear (forward and, on transposed operands, dX).
-// Replaces LoraInjectedLinear.forward (/root/reference/lora_diffusion/lora.py:53-58) and the dX
+// Replaces LoraInjectedLinear.forward (lora_diffusion/lora.py:53-58 of cloneofsimo/lora) and the dX
 // part of its autograd backward. Kernel: fused_core.cuh.
 #include <stdlib.h>
 #include "fused_core.cuh"
-#include "fused_persistent.cuh"
-#include "fused_splitk.cuh"
 #include "lora_b200.h"
 #include "tmap.h"
 
@@ -19,11 +17,11 @@ static bool tmap_weight(CUtensorMap* tm, const void* W, CUtensorMapDataType dt, 
 }
 
 template <int BLOCK_N, int STAGES, typename OutT, int MIN_CTAS, bool DROP = false, bool SPLITK = false,
-          bool BMASK = false>
+          bool BMASK = false, int CL = 1, bool INLINE_TMA = false>
 static int launch_linear(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p_in,
                          int out_dtype, cudaStream_t stream, int split = 1) {
-  using S = Smem<BLOCK_N, STAGES, OutT, 1, DROP, BMASK>;
-  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, false, 1, MIN_CTAS, DROP, SPLITK, BMASK>;
+  using S = Smem<BLOCK_N, STAGES, OutT, 1, DROP, BMASK, CL>;
+  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, false, 1, MIN_CTAS, DROP, SPLITK, BMASK, CL, INLINE_TMA>;
   FusedParams p = p_in;
   p.split = 1;
   if constexpr (SPLITK) {
@@ -33,7 +31,7 @@ static int launch_linear(const void* X, const void* W, const void* Dn, void* Y, 
                           static_cast<unsigned int>(tiles), &p.ws, &p.counters))
       return LB_ERR_CUDA;
   }
-  static_assert(MIN_CTAS * (S::DYN_BYTES + 1024) <= 233472 && MIN_CTAS * S::TMEM_COLS <= 512, "occupancy target does not fit");
+  static_assert(MIN_CTAS * (S::DYN_BYTES + 1024) <= 233472, "occupancy target does not fit");
   static unsigned long long attr_mask = 0;
   if (!ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::DYN_BYTES, attr_mask)) return LB_ERR_CUDA;
   const CUtensorMapDataType in_dt = p.fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
@@ -43,29 +41,30 @@ static int launch_linear(const void* X, const void* W, const void* Dn, void* Y, 
   if (!tmap_weight(&tmW, W, in_dt, p.N, p.K, BLOCK_N, p.w_tiled)) return LB_ERR_TMAP;
   if (!tmap_2d(&tmD, Dn, in_dt, 2, p.K, R_PAD, BLOCK_K, R_PAD, true)) return LB_ERR_TMAP;
   if (!tmap_2d(&tmY, Y, out_dt, sizeof(OutT), p.N, p.M, S::BOX_COLS, BLOCK_M, true)) return LB_ERR_TMAP;
-  dim3 grid((p.N + BLOCK_N - 1) / BLOCK_N, (p.M + BLOCK_M - 1) / BLOCK_M, SPLITK ? split : 1);
-  return launch_ex(kern, dim3(grid), dim3(NUM_THREADS), S::DYN_BYTES, stream, 1, tmX, tmW, tmD, tmY, p) == cudaSuccess
+  dim3 grid((p.N + BLOCK_N - 1) / BLOCK_N, (p.M + BLOCK_M - 1) / BLOCK_M, SPLITK ? split : CL);
+  return launch_ex(kern, dim3(grid), dim3(kernel_threads<INLINE_TMA>()), S::DYN_BYTES, stream, CL, tmX, tmW, tmD, tmY,
+                   p) == cudaSuccess
              ? LB_OK : LB_ERR_CUDA;
 }
 
-// Split-K plan for one linear problem (fused_core.cuh, SPLITK): the per-SM operand ingest (~92 GB/s
-// measured, DESIGN.md) makes a lone CTA's K loop cost ~0.29 us (BLOCK_N 64) / ~0.38 us (128) per
-// 64-wide K block, so sites with few tiles and long K leave most SMs idle while a handful stream.
-// Cost model in microseconds: fixed 2.0 (prologue + tail) + blocks x ingest; a split adds ~3.0
-// (L2 reductions of the partials, election, one burst read of the reduced row), independent of the
-// split factor. Only single-wave plans (tiles x split <= SMs), and a split must win by > 25 %.
+// Split-K plan for one linear problem (fused_core.cuh, SPLITK): a lone CTA streams its operands at a
+// bounded per-SM rate, so sites with few tiles and long K leave most SMs idle while a handful stream.
+// Cost model in microseconds (a planning heuristic, its parameters are not H100 measurements): fixed
+// 2.0 (prologue + tail) + K blocks x per-SM ingest at 92 GB/s; a split adds 3.0 (L2 reductions of the
+// partials, election, one burst read of the reduced row), independent of the split factor. Only
+// single-wave plans (tiles x split <= SMs), and a split must win by > 25 %. Split plans use BLOCK_N 64:
+// a 128-wide tile's reduced row and accumulator do not fit the registers together.
 struct SplitPlan { int block_n, split; };
 static SplitPlan plan_split(int M, int K, int N, int n_sms) {
   if (!splitk_enabled() || n_sms <= 0) return {0, 1};
   const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
   const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-  {  // profiling knob: LB_SPLIT_FORCE=<s> [LB_SPLIT_BN=64|128] forces a split wherever it fits in one wave
-    static int force = -1, force_bn = 64;
+  {  // profiling knob: LB_SPLIT_FORCE=<s> forces a split wherever it fits in one wave
+    static int force = -1;
+    const int force_bn = 64;
     if (force < 0) {
       const char* e = getenv("LB_SPLIT_FORCE");
       force = e ? atoi(e) : 0;
-      const char* b = getenv("LB_SPLIT_BN");
-      if (b && atoi(b) == 128) force_bn = 128;
     }
     if (force > 1) {
       const long long tiles = static_cast<long long>(m_tiles) * ((N + force_bn - 1) / force_bn);
@@ -76,7 +75,8 @@ static SplitPlan plan_split(int M, int K, int N, int n_sms) {
   }
   SplitPlan best = {0, 1};
   double best_t = 1e30, base_t = 1e30;
-  for (int bn = 64; bn <= 128; bn += 64) {
+  {
+    const int bn = 64;
     const long long tiles = static_cast<long long>(m_tiles) * ((N + bn - 1) / bn);
     const double per_kb = (128.0 + bn + 16.0) * 128.0 / 92e3;
     const double waves = static_cast<double>((tiles + n_sms - 1) / n_sms);
@@ -92,33 +92,12 @@ static SplitPlan plan_split(int M, int K, int N, int n_sms) {
   return {0, 1};
 }
 
-template <int BLOCK_N, int STAGES, typename OutT>
-static int launch_persistent(const void* X, const void* W, const void* Dn, void* Y,
-                             const FusedParams& p, int out_dtype, cudaStream_t stream) {
-  using S = PSmem<BLOCK_N, STAGES, OutT>;
-  auto kern = fused_lora_persistent_kernel<BLOCK_N, STAGES, OutT>;
-  static unsigned long long attr_mask = 0;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::DYN_BYTES, attr_mask)) return LB_ERR_CUDA;
-  const int num_sms = sm_count();
-  if (num_sms <= 0) return LB_ERR_CUDA;
-  const CUtensorMapDataType in_dt = p.fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const CUtensorMapDataType out_dt = out_dtype == LB_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : in_dt;
-  CUtensorMap tmX, tmW, tmD, tmY;
-  if (!tmap_2d(&tmX, X, in_dt, 2, p.K, p.M, BLOCK_K, BLOCK_M, true)) return LB_ERR_TMAP;
-  if (!tmap_weight(&tmW, W, in_dt, p.N, p.K, BLOCK_N, p.w_tiled)) return LB_ERR_TMAP;
-  if (!tmap_2d(&tmD, Dn, in_dt, 2, p.K, R_PAD, BLOCK_K, R_PAD, true)) return LB_ERR_TMAP;
-  if (!tmap_2d(&tmY, Y, out_dt, sizeof(OutT), p.N, p.M, S::BOX_COLS, BLOCK_M, true)) return LB_ERR_TMAP;
-  const long long total = static_cast<long long>((p.N + BLOCK_N - 1) / BLOCK_N) * ((p.M + BLOCK_M - 1) / BLOCK_M);
-  const int grid = static_cast<int>(total < num_sms ? total : num_sms);
-  return launch_ex(kern, dim3(grid), dim3(NUM_THREADS), S::DYN_BYTES, stream, 1, tmX, tmW, tmD, tmY, p) == cudaSuccess
-             ? LB_OK : LB_ERR_CUDA;
-}
-
-template <int BLOCK_N, int STAGES, typename OutT, int MIN_CTAS>
+template <int BLOCK_N, int STAGES, typename OutT, int MIN_CTAS, bool INLINE_TMA = false>
 static int launch_grouped(GroupedArgs& a, const void* const* X, const void* const* W,
                           const void* const* Dn, void* const* Y, int out_dtype, cudaStream_t stream) {
   using S = Smem<BLOCK_N, STAGES, OutT, 1>;
-  auto kern = fused_lora_grouped_kernel<BLOCK_N, STAGES, OutT, MIN_CTAS>;
+  static_assert(MIN_CTAS * (S::DYN_BYTES + 1024) <= 233472, "occupancy target does not fit");
+  auto kern = fused_lora_grouped_kernel<BLOCK_N, STAGES, OutT, MIN_CTAS, INLINE_TMA>;
   static unsigned long long attr_mask = 0;
   if (!ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::DYN_BYTES, attr_mask)) return LB_ERR_CUDA;
   const int fmt = a.p[0].fmt;
@@ -136,38 +115,20 @@ static int launch_grouped(GroupedArgs& a, const void* const* X, const void* cons
     total += a.n_tiles_n[i] * ((p.M + BLOCK_M - 1) / BLOCK_M);
   }
   for (int i = a.n_problems; i <= MAX_GROUP; ++i) a.tile_start[i] = total;
-  return launch_ex(kern, dim3(total), dim3(NUM_THREADS), S::DYN_BYTES, stream, 1, a) == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
-
-// EXPERIMENTAL cluster split-K schedule (fused_splitk.cuh): SPLIT CTAs of one cluster per output tile.
-template <int BLOCK_N, int STAGES, typename OutT, int SPLIT>
-static int launch_splitk(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p,
-                         int out_dtype, cudaStream_t stream) {
-  using S = SplitSmem<BLOCK_N, STAGES, OutT, SPLIT>;
-  auto kern = fused_lora_splitk_kernel<BLOCK_N, STAGES, OutT, SPLIT>;
-  static unsigned long long attr_mask = 0;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(kern), S::DYN_BYTES, attr_mask)) return LB_ERR_CUDA;
-  const CUtensorMapDataType in_dt = p.fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const CUtensorMapDataType out_dt = out_dtype == LB_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : in_dt;
-  CUtensorMap tmX, tmW, tmD, tmY;
-  if (!tmap_2d(&tmX, X, in_dt, 2, p.K, p.M, BLOCK_K, BLOCK_M, true)) return LB_ERR_TMAP;
-  if (!tmap_weight(&tmW, W, in_dt, p.N, p.K, BLOCK_N, p.w_tiled)) return LB_ERR_TMAP;
-  if (!tmap_2d(&tmD, Dn, in_dt, 2, p.K, R_PAD, BLOCK_K, R_PAD, true)) return LB_ERR_TMAP;
-  if (!tmap_2d(&tmY, Y, out_dt, sizeof(OutT), p.N, p.M, S::BOX_COLS, BLOCK_M, true)) return LB_ERR_TMAP;
-  const dim3 grid((p.N + BLOCK_N - 1) / BLOCK_N, (p.M + BLOCK_M - 1) / BLOCK_M, SPLIT);
-  return launch_ex(kern, grid, dim3(NUM_THREADS), S::DYN_BYTES, stream, SPLIT, tmX, tmW, tmD, tmY, p) == cudaSuccess
+  return launch_ex(kern, dim3(total), dim3(kernel_threads<INLINE_TMA>()), S::DYN_BYTES, stream, 1, a) == cudaSuccess
              ? LB_OK : LB_ERR_CUDA;
 }
 
+
 static int g_linear_mode = 0;
-static unsigned long long* g_dbg = nullptr;  // profiling: device buffer of 16 timestamps  // 0 = auto, 1 = one tile per CTA (2-3 CTAs/SM), 2 = persistent
+static unsigned long long* g_dbg = nullptr;  // profiling: device buffer of 16 timestamps
 
 }  // namespace lb
 
 // Tuning knob (benchmarks / profiling only): force the tile schedule of lb_lora_linear_fwd.
 extern "C" int lb_debug_set_linear_mode(int mode) {
-  // schedule (0 auto, 1 one tile per CTA, 2 persistent, 3 EXPERIMENTAL cluster split-K)
+  // schedule (0 auto, 1 one tile per CTA, 2 one tile per CTA and one CTA per SM, 3 cluster split-K
+  // over 2..4 CTAs per tile)
   // + 4 * block_n choice (0 auto, 1: 64, 2: 128) + 16 * split-K factor choice (0: auto, 1..3: 2..4 CTAs)
   if (mode < 0 || mode > 63) return LB_ERR_SHAPE;          // block_n choice 3 = 192 (16-bit outputs, one tile per CTA)
   lb::g_linear_mode = mode;
@@ -220,15 +181,13 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
   p.seed = reinterpret_cast<const unsigned long long*>(seed_dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (mask_input) {
-    // Dropout BACKWARD (dX): X = gY, and the T path must see mask o gY -- the epilogue warps write a
+    // Dropout BACKWARD (dX): X = gY, and the T path must see mask o gY -- the consumer warps write a
     // masked copy of every A tile for the T MMA (fused_core.cuh, BMASK); mask index = row * K + k.
     const SplitPlan spm = plan_split(M, K, N, sm_count());
     if (spm.split > 1) {
       if (out_dtype == LB_F32)
-        return spm.block_n == 64 ? launch_linear<64, 4, float, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split)
-                                 : launch_linear<128, 3, float, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split);
-      return spm.block_n == 64 ? launch_linear<64, 4, uint16_t, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split)
-                               : launch_linear<128, 3, uint16_t, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split);
+        return launch_linear<64, 4, float, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split);
+      return launch_linear<64, 4, uint16_t, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split);
     }
     const long long t128 = static_cast<long long>((M + 127) / 128) * ((N + 127) / 128);
     const bool nar = t128 < 90 && !(K >= 2048 && t128 >= 64);
@@ -239,16 +198,14 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
                : launch_linear<128, 3, uint16_t, 1, false, false, true>(X, W, down16, Y, p, out_dtype, st);
   }
   if (drop_p > 0.f) {
-    // Dropout on the branch: the LoRA product keeps its own TMEM columns and is masked in the
-    // drain (fused_core.cuh, DROP). One tile per CTA; BLOCK_N 64 (256 TMEM columns, 2 CTAs/SM)
-    // unless the site has plenty of 128-wide tiles.
+    // Dropout on the branch: the LoRA product keeps its own accumulator and is masked in the
+    // drain (fused_core.cuh, DROP). One tile per CTA; BLOCK_N 64 (2 CTAs/SM) unless the site has
+    // plenty of 128-wide tiles.
     const SplitPlan spd = plan_split(M, K, N, sm_count());
     if (spd.split > 1) {
       if (out_dtype == LB_F32)
-        return spd.block_n == 64 ? launch_linear<64, 4, float, 1, true, true>(X, W, down16, Y, p, out_dtype, st, spd.split)
-                                 : launch_linear<128, 4, float, 1, true, true>(X, W, down16, Y, p, out_dtype, st, spd.split);
-      return spd.block_n == 64 ? launch_linear<64, 5, uint16_t, 1, true, true>(X, W, down16, Y, p, out_dtype, st, spd.split)
-                               : launch_linear<128, 4, uint16_t, 1, true, true>(X, W, down16, Y, p, out_dtype, st, spd.split);
+        return launch_linear<64, 4, float, 1, true, true>(X, W, down16, Y, p, out_dtype, st, spd.split);
+      return launch_linear<64, 5, uint16_t, 1, true, true>(X, W, down16, Y, p, out_dtype, st, spd.split);
     }
     const long long t128 = static_cast<long long>((M + 127) / 128) * ((N + 127) / 128);
     const bool nar = t128 < 120 && !(K >= 2048 && t128 >= 64);
@@ -263,10 +220,8 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
     const SplitPlan sp = plan_split(M, K, N, sm_count());
     if (sp.split > 1) {
       if (out_dtype == LB_F32)
-        return sp.block_n == 64 ? launch_linear<64, 5, float, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split)
-                                : launch_linear<128, 4, float, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split);
-      return sp.block_n == 64 ? launch_linear<64, 6, uint16_t, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split)
-                              : launch_linear<128, 4, uint16_t, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split);
+        return launch_linear<64, 5, float, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split);
+      return launch_linear<64, 6, uint16_t, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split);
     }
   }
   const int sched = g_linear_mode & 3, bn_choice = (g_linear_mode >> 2) & 3, split_choice = g_linear_mode >> 4;
@@ -275,73 +230,61 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
   const long long tiles64 = m_tiles * ((N + 63) / 64);
   const int n_sms = sm_count();
   if (g_linear_mode == 0 && T_in == nullptr && splitk_enabled() && n_sms > 0) {
-    // Cluster split-K (fused_splitk.cuh): few tiles and a K loop of >= 10 blocks -- the attention
-    // projections of the 16x16 / 8x8 levels, the 77-token k/v sites, CLIP. Two CTAs of a cluster halve
-    // the K loop and merge through distributed shared memory (one bulk copy, no global round trip:
-    // the L2-reduction split above costs 4-5 us and only pays for K >= 5120). Measured per site
-    // (profiles/r2g_site_table_cluster_splitk.md): 256x1280->1280 11.0 -> 9.6 us, 64x1280->1280 10.8 -> 9.0,
-    // 77x768->768 8.35 -> 7.9; K = 320 sites lose (6.7 -> 7.3) and stay unsplit.
+    // Cluster split-K: few tiles and a K loop of >= 10 blocks -- the attention projections of the
+    // 16x16 / 8x8 levels, the 77-token k/v sites, CLIP. Two CTAs of a cluster halve the K loop and
+    // merge through distributed shared memory (one bulk copy, no global round trip).
     if (K >= 640 && tiles64 * 2 <= n_sms) {
-      if (out_dtype == LB_F32) return launch_splitk<64, 4, float, 2>(X, W, down16, Y, p, out_dtype, st);
-      return launch_splitk<64, 6, uint16_t, 2>(X, W, down16, Y, p, out_dtype, st);
+      if (out_dtype == LB_F32) return launch_linear<64, 4, float, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      return launch_linear<64, 6, uint16_t, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
     }
     // One balanced wave of 192-wide tiles instead of 1.1 waves of 128-wide ones (256x1280->10240:
-    // 160 -> 108 CTAs, 18.7 -> 13.9 us)
+    // 160 tiles of 128, 80 of 192)
     if (out_dtype != LB_F32 && tiles128 > n_sms && m_tiles * ((N + 191) / 192) <= n_sms && K >= 640)
       return launch_linear<192, 4, uint16_t, 1>(X, W, down16, Y, p, out_dtype, st);
   }
   // not enough tiles to fill the SMs with 128-wide ones: halve BLOCK_N -- as long as the 64-wide tiles
-  // still fit ONE wave (64x1280->10240: 80 tiles of 128 on 80 SMs take 12.9 us, 160 tiles of 64 at
-  // 3 CTAs/SM 16.6; 4096x320->320: 96 vs 160 tiles, 11.1 vs 12.3 us)
-  bool narrow = tiles64 <= n_sms;
+  // still fit ONE wave (at 2 CTAs per SM for short K and many row tiles: 4096x320->320 on an H100,
+  // 96 tiles of 128 at one CTA per SM ~37-40 us, 160 tiles of 64 at two per SM ~21 us)
+  bool narrow = tiles64 <= n_sms || (tiles64 <= 2LL * n_sms && K < 2048 && m_tiles >= 8);
   if (K >= 2048 && tiles128 >= 64) narrow = false;  // long K: per-tile work is large, keep W reuse
   if (bn_choice == 1) narrow = true;
   if (bn_choice == 2) narrow = false;
-  // More tiles than SMs: persistent CTAs with a double-buffered TMEM accumulator (epilogue of
-  // tile i overlaps the main loop of tile i+1). Otherwise one tile per CTA.
   const long long tiles_n = narrow ? tiles64 : tiles128;
   if (sched == 3 && T_in == nullptr) {
-    // EXPERIMENTAL, opt-in only: split the K loop of every tile across a cluster of 2..4 CTAs
+    // opt-in: split the K loop of every tile across a cluster of 2..4 CTAs (as the auto rule above)
     const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
     int split = split_choice ? split_choice + 1 : 4;
     if (split > num_kb) split = num_kb;
     if (bn_choice == 2 && split > 2) split = 2;        // 128-wide partials: one peer slot fits
     if (split >= 2) {
       if (out_dtype == LB_F32) {
-        if (split == 2) return launch_splitk<64, 4, float, 2>(X, W, down16, Y, p, out_dtype, st);
-        if (split == 3) return launch_splitk<64, 3, float, 3>(X, W, down16, Y, p, out_dtype, st);
-        return launch_splitk<64, 2, float, 4>(X, W, down16, Y, p, out_dtype, st);
+        if (split == 2) return launch_linear<64, 4, float, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+        if (split == 3) return launch_linear<64, 3, float, 1, false, false, false, 3>(X, W, down16, Y, p, out_dtype, st);
+        return launch_linear<64, 2, float, 1, false, false, false, 4>(X, W, down16, Y, p, out_dtype, st);
       }
-      if (bn_choice == 2) return launch_splitk<128, 3, uint16_t, 2>(X, W, down16, Y, p, out_dtype, st);
-      if (split == 2) return launch_splitk<64, 6, uint16_t, 2>(X, W, down16, Y, p, out_dtype, st);
-      if (split == 3) return launch_splitk<64, 4, uint16_t, 3>(X, W, down16, Y, p, out_dtype, st);
-      return launch_splitk<64, 3, uint16_t, 4>(X, W, down16, Y, p, out_dtype, st);
+      if (bn_choice == 2) return launch_linear<128, 3, uint16_t, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      if (split == 2) return launch_linear<64, 6, uint16_t, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      if (split == 3) return launch_linear<64, 4, uint16_t, 1, false, false, false, 3>(X, W, down16, Y, p, out_dtype, st);
+      return launch_linear<64, 2, uint16_t, 1, false, false, false, 4>(X, W, down16, Y, p, out_dtype, st);
     }
   }
   if (bn_choice == 3 && out_dtype != LB_F32)
     return launch_linear<192, 4, uint16_t, 1>(X, W, down16, Y, p, out_dtype, st);
-  const bool persistent = sched == 2 || (sched == 0 && tiles_n >= 3 * 148);
-  if (persistent) {
-    if (out_dtype == LB_F32) {
-      return narrow ? launch_persistent<64, 4, float>(X, W, down16, Y, p, out_dtype, st)
-                    : launch_persistent<128, 4, float>(X, W, down16, Y, p, out_dtype, st);
-    }
-    return narrow ? launch_persistent<64, 6, uint16_t>(X, W, down16, Y, p, out_dtype, st)
-                  : launch_persistent<128, 4, uint16_t>(X, W, down16, Y, p, out_dtype, st);
-  }
-  // One tile per CTA. More tiles than SMs: 2 (BLOCK_N = 128) or 3 (BLOCK_N = 64) CTAs per SM with
-  // a short smem ring, so one CTA's drain overlaps its neighbours' loads. Fewer tiles than SMs
-  // (small-M / long-K sites): one CTA per SM with a DEEP ring (7 x 26 KB or 4 x 34 KB in flight),
-  // because a lone CTA streaming K = 768..10240 is bound by load latency, not bandwidth.
-  const bool crowded = tiles_n > 148;
+  // One tile per CTA. More tiles than SMs: 2 CTAs per SM with a short smem ring, so one CTA's
+  // park / LoRA MMA / drain / store overlaps its neighbour's loads and MMAs (16-bit 128-wide tiles:
+  // the 256-thread inline-TMA kernel, see fused_core.cuh). Fewer tiles than SMs (small-M / long-K
+  // sites): one CTA per SM with a DEEP ring (7 x 26 KB or 4 x 34 KB in flight), because a lone CTA
+  // streaming K = 768..10240 is bound by load latency, not bandwidth. Schedule 2 forces one CTA per
+  // SM (deep ring) everywhere, to measure the overlap against.
+  const bool crowded = tiles_n > n_sms && sched != 2;
   if (out_dtype == LB_F32) {
     return narrow ? launch_linear<64, 3, float, 2>(X, W, down16, Y, p, out_dtype, st)
                   : launch_linear<128, 4, float, 1>(X, W, down16, Y, p, out_dtype, st);
   }
   if (narrow)
-    return crowded ? launch_linear<64, 2, uint16_t, 3>(X, W, down16, Y, p, out_dtype, st)
+    return crowded ? launch_linear<64, 2, uint16_t, 2>(X, W, down16, Y, p, out_dtype, st)
                    : launch_linear<64, 7, uint16_t, 1>(X, W, down16, Y, p, out_dtype, st);
-  return crowded ? launch_linear<128, 2, uint16_t, 2>(X, W, down16, Y, p, out_dtype, st)
+  return crowded ? launch_linear<128, 2, uint16_t, 2, false, false, false, 1, true>(X, W, down16, Y, p, out_dtype, st)
                  : launch_linear<128, 4, uint16_t, 1>(X, W, down16, Y, p, out_dtype, st);
 }
 
@@ -408,13 +351,13 @@ extern "C" int lb_lora_linear_fwd_grouped(int n, const void* const* X, const voi
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bool narrow = tiles128 < 120;
-  const bool crowded = (narrow ? tiles64 : tiles128) > 148;
+  const bool crowded = (narrow ? tiles64 : tiles128) > sm_count();
   if (out_dtype == LB_F32)
     return narrow ? launch_grouped<64, 3, float, 2>(a, X, W, down16, Y, out_dtype, st)
                   : launch_grouped<128, 4, float, 1>(a, X, W, down16, Y, out_dtype, st);
   if (narrow)
-    return crowded ? launch_grouped<64, 2, uint16_t, 3>(a, X, W, down16, Y, out_dtype, st)
+    return crowded ? launch_grouped<64, 2, uint16_t, 2>(a, X, W, down16, Y, out_dtype, st)
                    : launch_grouped<64, 7, uint16_t, 1>(a, X, W, down16, Y, out_dtype, st);
-  return crowded ? launch_grouped<128, 2, uint16_t, 2>(a, X, W, down16, Y, out_dtype, st)
+  return crowded ? launch_grouped<128, 2, uint16_t, 2, true>(a, X, W, down16, Y, out_dtype, st)
                  : launch_grouped<128, 4, uint16_t, 1>(a, X, W, down16, Y, out_dtype, st);
 }

@@ -1,4 +1,4 @@
-// HBM-bound helper kernels around the fused tcgen05 path:
+// HBM-bound helper kernels around the fused wgmma path:
 //   - skinny weight-gradient reduction (dA, dB)        lora.py:53-58 autograd backward
 //   - 16-bit shadow / frozen-weight casts + transposes
 //   - global-norm clip + AdamW over the flat LoRA arena  train_lora_dreambooth.py:878-888
@@ -11,6 +11,7 @@
 
 #include "dropmask.cuh"
 #include "lora_b200.h"
+#include "tmap.h"
 
 namespace lb {
 
@@ -548,7 +549,7 @@ adamw_update_kernel(float* __restrict__ p, float* __restrict__ g, float* __restr
 //   phase 1  per-block partial sum of g^2 (fixed order => deterministic)          -- grid barrier --
 //   phase 2  every block re-reduces the partials, forms coef, updates its slice of p/m/v, zeroes g
 //                                                                                  -- grid barrier --
-//   phase 3  re-casts every LoRA factor into the zero-padded 16-bit [16, C] operands the tcgen05
+//   phase 3  re-casts every LoRA factor into the zero-padded 16-bit [16, C] operands the wgmma
 //            kernels read (table walk, same rows as lb_refresh_shadows)
 // The grid is launched with cudaLaunchAttributeCooperative (co-residency guaranteed) and at most
 // one CTA per SM; the barrier is a generation counter in `bar` (2 x uint32, zero-initialised).
@@ -1225,7 +1226,8 @@ extern "C" int lb_adamw_clip_step(float* p, float* g, float* m, float* v, long l
   int nblk = static_cast<int>(want < 1 ? 1 : (want > OPT_MAX_PARTIALS ? OPT_MAX_PARTIALS : want));
   sqnorm_partial_kernel<<<nblk, OPT_THREADS, 0, st>>>(g, n, partials, step_dev);
   long long want2 = (n + OPT_THREADS - 1) / OPT_THREADS;
-  int nblk2 = static_cast<int>(want2 > 148 * 8 ? 148 * 8 : want2);
+  const int cap2 = 8 * (sm_count() > 0 ? sm_count() : 132);
+  int nblk2 = static_cast<int>(want2 > cap2 ? cap2 : want2);
   adamw_update_kernel<<<nblk2, OPT_THREADS, 0, st>>>(p, g, m, v, n, groups, lr_dev, beta1, beta2,
                                                      eps, weight_decay, max_norm, inv_world,
                                                      step_dev, partials, nblk, gnorm_out);

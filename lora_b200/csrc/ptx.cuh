@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the LoRA kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), proxy fences.
+// Thin inline-PTX wrappers for the sm_90a features the LoRA kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (descriptors, fence / commit / wait), proxy fences.
 // Everything here is device-only and header-only.
 #pragma once
 #include <cuda.h>
@@ -41,7 +41,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug traps (CUDA error on the host) instead of hanging the GPU box.
 #ifndef LB_WAIT_TIMEOUT_CYCLES
-#define LB_WAIT_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.9 GHz
+#define LB_WAIT_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.98 GHz
 #endif
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
@@ -51,15 +51,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// ---------------------------------------------------------------- proxy / tcgen05 fences
+// ---------------------------------------------------------------- proxy fence
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -102,88 +96,38 @@ __device__ __forceinline__ void tma_store_wait_read0() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-// ---------------------------------------------------------------- TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32-bit, 16 consecutive columns -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32"
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA (tcgen05.mma)
-// Shared-memory matrix descriptor (sm_100 "version 1").
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+// Shared-memory matrix descriptor (sm_90):
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1
-//   bits [61,64) layout: 0 = no swizzle (interleaved core matrices), 2 = 128B swizzle
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes, uint32_t layout) {
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout: 0 = no swizzle (interleaved core
+//   matrices), 1 = 128B swizzle. K-major operands: LBO = next core matrix along K, SBO = next 8-row group.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+                                               uint32_t layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout & 7) << 61;
+  d |= static_cast<uint64_t>(layout & 3) << 62;
   return d;
 }
-// Instruction descriptor for kind::f16 with fp32 accumulate, both operands K-major.
-//   fmt: 0 = fp16, 1 = bf16
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// Orders this thread's register accumulator accesses before the warpgroup's next wgmma.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory");
 }
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
+// Keeps the compiler from moving accesses of an accumulator register across wgmma issue / wait.
+template <int NREG>
+__device__ __forceinline__ void reg_fence(float* r) {
+#pragma unroll
+  for (int i = 0; i < NREG; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while its
-// predecessor in the stream is still draining: everything before pdl_wait() (barrier init, TMEM
-// allocation, descriptor prefetch) overlaps the predecessor's tail; pdl_wait() returns once the
+// predecessor in the stream is still draining: everything before pdl_wait() (barrier init,
+// descriptor prefetch) overlaps the predecessor's tail; pdl_wait() returns once the
 // predecessor grid has completed and its writes are visible. Both are no-ops in a normal launch.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() {

@@ -1,4 +1,4 @@
-// The two ends of a training step, either side of the UNet call (SURVEY.md 8f rank 3):
+// The two ends of a training step, either side of the UNet call:
 //   lb_step_prologue      scheduler.add_noise + cast + NCHW -> NHWC (+ the inpainting concat)
 //                         cli_lora_pti.py:295-313, train_lora_dreambooth.py:822-840
 //   lb_masked_mse_fwd_bwd the (mask-weighted) MSE of cli_lora_pti.py:340-370 /

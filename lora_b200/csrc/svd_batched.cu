@@ -1,6 +1,6 @@
 // lb_svd_truncated_batched: the whole SVD distillation of /root/reference/lora_diffusion/cli_svd.py:24-92
 // (`overwrite_base`: per site  dW = W_tuned - W_base -> SVD -> U_r diag(S_r), Vh_r -> quantile clamp)
-// for ALL sites of a model in one C call, ragged over shapes (SURVEY.md 8b).
+// for ALL sites of a model in one C call, ragged over shapes.
 //
 // Algorithm (per matrix, all matrices in flight together): randomized range finder with L = 32
 // Rademacher probes and q power iterations, then the exact SVD of the projected 32 x K problem:
@@ -13,11 +13,11 @@
 //
 // Kernels:
 //   mul_right / mul_left   the passes. HBM-bound: AI = 2*32 flop per 4 bytes = 16 flop/B, i.e.
-//       ~105 TFLOP/s at the 6.6 TB/s roofline -- beyond the fp32 CUDA cores (72 TFLOP/s), so the
-//       contraction runs on the tensor cores: the fp32 delta tile is split in registers into
+//       ~54 TFLOP/s at the H100's 3.35 TB/s data-sheet bandwidth -- near the fp32 CUDA cores' 67
+//       TFLOP/s data-sheet peak, so the contraction runs on the tensor cores: the fp32 delta tile is split in registers into
 //       bf16 hi + lo, the tall-skinny operand likewise, and hi.hi + lo.hi + hi.lo are accumulated
-//       in fp32 with mma.sync.m16n8k16 (2^-16 relative per product: fp32-faithful; tcgen05 would
-//       need the operands staged in UMMA shared-memory layouts and buys nothing on a memory-bound
+//       in fp32 with mma.sync.m16n8k16 (2^-16 relative per product: fp32-faithful; wgmma would
+//       need the operands staged in its shared-memory layouts and buys nothing on a memory-bound
 //       pass). Weights come in through 16-byte vector loads, one tile ahead in registers.
 //   mul_right also accumulates the Gram matrix of its output tile (no separate pass over Y).
 //   tall_transform         Y <- Y V diag(1/s) (+ Gram of the result), or Gram only
@@ -545,8 +545,8 @@ tall_transform_kernel(const MatDesc* __restrict__ mats, const TItem* __restrict_
 // rows, l = tid % 16 its columns), so a step is: read (block + the column rotation's pivots) ->
 // barrier -> write -> barrier. Every lane derives the rotation of its column pair and fetches the
 // row pair's from a lane of its own warp (no serial 16-thread phase); the round-robin pairing is
-// tabulated once (no permutation array to maintain): 2 barriers per step instead of 5 (round 2a:
-// 130-240 us per solve, latency-bound on the barriers).
+// tabulated once (no permutation array to maintain): 2 barriers per step instead of 5 (a solve is
+// latency-bound on the barriers).
 // Outputs eigenvectors (columns, descending eigenvalue) and sqrt(max(eig, 0)).
 __device__ __forceinline__ int rr_elem(int pos, int step) {   // element at tournament position `pos` after `step` rotations
   if (pos == 0) return 0;

@@ -1,6 +1,6 @@
 """Data-parallel plumbing for the LoRA step (one process per GPU, torch.distributed).
 
-The path shards by data only (SURVEY.md 8e): every rank holds a full replica, processes its own
+The path shards by data only: every rank holds a full replica, processes its own
 image(s) and the single exchange is a SUM all-reduce of the flat LoRA-gradient buffer; the 1/world
 average is folded into the fused clip+AdamW kernel. Replaces what the reference gets from
 accelerate -> DDP (training_scripts/train_lora_dreambooth.py:744-757, 877)."""

@@ -6,10 +6,10 @@ state of every operator built by inject_trainable_lora_extended and by the monke
 
 The mask sits between the up-projection and the sum, so the branch cannot be accumulated into the
 base accumulator -- but it still never leaves the SM: the fused kernel gives the LoRA product
-T'.U^T its own TMEM columns and applies keep(m,n)/(1-p) while the tile is drained
+T'.U^T its own accumulator and applies keep(m,n)/(1-p) while the tile is drained
 (lb_lora_linear_fwd_dropout / lb_lora_conv2d_fwd_dropout; csrc/fused_core.cuh, DROP): ONE launch,
 no extra pass over Y. Backward recomputes the same counter-based mask INSIDE the dX kernel
-(lb_lora_linear_dx_dropout / lb_lora_conv2d_dx_dropout: the epilogue warps, idle during the K loop,
+(lb_lora_linear_dx_dropout / lb_lora_conv2d_dx_dropout: the consumer warpgroups, inside the MMA loop,
 write a masked copy of each gY tile that feeds only the rank-r MMA -- dT = (mask o gY) . B without a
 separate pass over gY); dB uses the masked reduction (lb_lora_wgrad_masked).
 
@@ -27,9 +27,8 @@ from .modules import _LOW, _SiteState, _compute_dtype, _fp32_master, _out_dtype
 
 # Backward formulation. "twopass" (default): lb_lora_dropout_dt (one masked pass over gY) + the plain dX
 # kernel with T_in. "fused": the mask applied inside the dX kernel (lb_lora_*_dx_dropout, one launch, no
-# extra pass). Same results (tests/test_dropout_gpu.py runs both); measured on the same box the fused
-# form is SLOWER on the extended step (26.3 vs 23.7 ms, profiles/r2g_*): hashing 8192 mask decisions per
-# K block on four warps costs more than the streaming pass it deletes.
+# extra pass). Same results (tests/test_dropout_gpu.py runs both); the fused form hashes 8192 mask
+# decisions per K block inside the MMA loop, where the separate streaming pass costs one read of gY.
 _TWO_PASS = os.environ.get("LB_DROPOUT_BWD", "twopass") != "fused"
 
 

@@ -1,7 +1,7 @@
 """Grouped launches for LoRA linear sites that share an input (q/k/v of a self-attention, k/v of a
 cross-attention, CLIP's k/v/q projections).
 
-At bs = 1 those sites are 12-40 output tiles each: alone they leave most of the 148 SMs idle, and
+At bs = 1 those sites are 12-40 output tiles each: alone they leave most of the 132 SMs idle, and
 the host model calls them back to back on the same tensor. With `lora_b200.set_grouping(True)`
 the first site of such a family to be called launches ONE kernel (`lb_lora_linear_fwd_grouped`)
 that computes the outputs of the whole family; the siblings' outputs are parked on the parent

@@ -1,5 +1,5 @@
 """Rank-concatenation of LoRA files ("join") and the small manager object that drives a joined
-model -- the host-side file arithmetic next to `collapse_lora` (SURVEY.md 8(f) rank 2).
+model -- the host-side file arithmetic next to `collapse_lora`.
 
 Behaviour follows the reference's `lora_diffusion/lora_manager.py` (`lora_join` :13-71,
 `DummySafeTensorObject` :74-86, `LoRAManager` :89-144); tests/test_formats_cpu.py runs both side

@@ -1,6 +1,6 @@
 """`lora_add`: arithmetic on LoRA files and merging a LoRA into a pipeline's frozen weights.
 
-Mirrors `lora_diffusion/cli_lora_add.py:24-183` of the reference (SURVEY.md 8(f) rank 2), modes
+Mirrors `lora_diffusion/cli_lora_add.py:24-183` of the reference, modes
   lpl          LoRA (+) LoRA: alpha_1 * factors_1 + alpha_2 * factors_2, `.pt` pair lists or safetensors
   ljl          join: rank-concatenate two safetensors LoRAs (`join.lora_join`)
   upl          pipeline (+) LoRA: W += alpha_1 * B·A on every site, LoRA removed, pipeline saved

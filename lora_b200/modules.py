@@ -1,4 +1,4 @@
-"""LoRA operator modules whose forward/backward run in liblora_b200.so (sm_100a).
+"""LoRA operator modules whose forward/backward run in liblora_b200.so (sm_90a).
 
 Drop-in for the two operator classes of the reference (same class NAMES -- three reference call
 sites match on ``__class__.__name__``, lora_diffusion/lora.py:879,885,1030 -- same constructor
@@ -8,7 +8,7 @@ signatures, same child names ``linear|conv``, ``lora_down``, ``dropout``, ``lora
     LoraInjectedLinear   <- /root/reference/lora_diffusion/lora.py:32-70
     LoraInjectedConv2d   <- /root/reference/lora_diffusion/lora.py:73-156
 
-What differs is only *how* ``forward`` is computed: one fused tcgen05 kernel
+What differs is only *how* ``forward`` is computed: one fused wgmma kernel
 (include/lora_b200.h: lb_lora_linear_fwd / lb_lora_conv2d_fwd) instead of three library GEMMs
 and four elementwise passes; backward = the same fused kernel on the pre-transposed frozen weight
 plus one skinny reduction per LoRA factor. The children stay ordinary nn.Linear / nn.Conv2d
@@ -137,7 +137,7 @@ class _SiteState:
 
     def frozen(self, weight2d: torch.Tensor, dtype, need_t: bool, tiled: Optional[bool] = None):
         """16-bit copies of the frozen weight: (W [N,K], W^T [K,N] or None), row-major tensors -- or, with
-        ops.TILED_WEIGHTS (opt-in, LB_TILED_W=1; measured: no gain), ops.TiledWeight in contiguous
+        ops.TILED_WEIGHTS (opt-in, LB_TILED_W=1), ops.TiledWeight in contiguous
         64 x 64 blocks. tiled=False forces row-major (row slicing: the rank > 16 chunks)."""
         tiled = ops.TILED_WEIGHTS if tiled is None else tiled
         k = _key(weight2d)

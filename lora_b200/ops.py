@@ -159,9 +159,8 @@ def cast_weight(w: torch.Tensor, dtype, want_plain: bool, want_t: bool):
 
 LB_W_TILED = 0x100
 # LB_TILED_W=1: the module layer (modules._SiteState.frozen) keeps its frozen-weight copies in the
-# 64x64-block layout. OFF by default: measured per site against row-major on the same box
-# (profiles/r2h_site_table_tiled_vs_rowmajor.md) it changes nothing -- DRAM page locality of the weight
-# stream is not what limits these kernels -- and it costs a second copy of every 16-bit frozen weight.
+# 64x64-block layout. OFF by default: it costs a second copy of every 16-bit frozen weight, and DRAM
+# page locality of the weight stream is not what limits these kernels.
 TILED_WEIGHTS = os.environ.get("LB_TILED_W", "0") == "1"
 
 class TiledWeight:

@@ -1,5 +1,5 @@
 """Pack `.pt` LoRA pair lists and textual-inversion `.pt` dicts into ONE `.safetensors` file
-(SURVEY.md 8(f) rank 4; behaviour of the reference's `cli_pt_to_safetensors.convert`, :19-77).
+(behaviour of the reference's `cli_pt_to_safetensors.convert`, :19-77).
 
 File kinds are told apart by what unpickles: a dict is a {token: embedding} table, anything else
 is the flat list [up_0, down_0, up_1, down_1, ...] that `save_lora_weight` writes. The model a

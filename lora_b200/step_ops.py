@@ -1,4 +1,4 @@
-"""The two ends of a training step as single kernels (csrc/step_glue.cu; SURVEY.md 8f rank 3):
+"""The two ends of a training step as single kernels (csrc/step_glue.cu):
 
   step_prologue     scheduler.add_noise + cast to the model dtype + NCHW -> channels_last
                     (+ the 9-channel inpainting concat)   cli_lora_pti.py:295-313

@@ -13,7 +13,7 @@ eigen-solve, exact quantile clamp): the only passes over the weights are 2(q+1) 
 (3-term split-bf16, fp32-faithful).
 
 Singular vectors are unique up to a per-component sign, and the reference's clamp threshold is a
-quantile over SIGNED values, so elementwise equality with LAPACK is not defined (SURVEY.md 7);
+quantile over SIGNED values, so elementwise equality with LAPACK is not defined;
 parity is stated on singular values, on the rank-r product before clamping and on the clamp rule
 (tests/test_svd_gpu.py).
 """
@@ -110,7 +110,7 @@ def overwrite_base(base_model: nn.Module, tuned_model: nn.Module, rank: int, cla
     """cli_svd.py:24-92 on two LoRA-injected models with identical site structure: the factors of
     `base_model`'s sites are overwritten with the rank-`rank` distillation of (tuned - base).
 
-    shard=(rank, world) (SURVEY.md 8e, config C5 on several GPUs): the weight deltas are
+    shard=(rank, world) (svd distillation on several GPUs): the weight deltas are
     independent, so this process distils only sites i = rank (mod world) in traversal order -- no
     collective on the compute path -- and the factors are then exchanged with ONE SUM all-reduce
     over a zero-initialised flat fp32 buffer in which every rank has filled only its own slots

@@ -1,4 +1,4 @@
-"""Pivotal-tuning phase 1: textual inversion of a few placeholder tokens (SURVEY.md 8f, rank 1).
+"""Pivotal-tuning phase 1: textual inversion of a few placeholder tokens.
 
 Restates what `train_inversion` does to the embedding table each step
 (lora_diffusion/cli_lora_pti.py:373-542: AdamW over the input-embedding table, the norm "decay" of

@@ -1,6 +1,6 @@
 """Export a saved diffusers pipeline directory as one CompVis / A1111 `.ckpt` file.
 
-Mirrors `lora_diffusion/to_ckpt_v2.py:91-232` of the reference (SURVEY.md 8(f) rank 4): the same
+Mirrors `lora_diffusion/to_ckpt_v2.py:91-232` of the reference: the same
 key names come out for the SD1.x topology (4 levels, 2 down / 3 up resnets per level), but the
 renaming is done by parsing each key into (block, index, rest) rather than by a table of string
 replacements. Keys that are not part of that topology pass through unchanged, as they do there.

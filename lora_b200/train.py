@@ -6,7 +6,7 @@ Restates (diffusers / accelerate are not installed, so the scripts themselves ca
       add_noise, text encoder, UNet, MSE, backward, clip_grad_norm_(1.0), AdamW, zero_grad)
   lora_diffusion/cli_lora_pti.py:260-370, 585-617     -- PTI LoRA-tuning phase (same step with
       t_mutliplier and mean([1,2,3]).mean() reduction)
-Differences by design (DESIGN.md): LoRA factors/grads/moments live in a LoraArena, the
+Differences by design: LoRA factors/grads/moments live in a LoraArena, the
 DDP all-reduce + clip + AdamW + zero_grad are one NCCL call and two kernels, and steady-state
 steps are CUDA-graph replays (no Python, no launch gaps, no host sync).
 """
@@ -43,8 +43,7 @@ class StepConfig:
     # EXPERIMENTAL (not yet run on hardware): capture the NCCL all-reduce INSIDE one step graph,
     # with capture_error_mode="thread_local" so that the NCCL watchdog thread's event queries do
     # not collide with the capture (the suspected cause of the round-1 dead-lock with a globally
-    # scoped capture). Saves the host gap between the two replays (~1 ms/step measured at N=8).
-    # Try it at N=2 under `timeout` first.
+    # scoped capture). Saves the host gap between the two replays.
     capture_collective: bool = False
     # accelerate-style mixed precision (fp32 frozen weights + torch.autocast), the reference's
     # own configuration (train_lora_dreambooth.py:489-494). None: run in the models' own dtype.

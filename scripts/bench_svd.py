@@ -1,5 +1,5 @@
 """BASELINE.json configs[4]: cli_svd distill full-finetune -> rank 8 over all SD1.5 attention/GEGLU
-weight deltas + CLIP attention, on 1 x B200. Synthetic fp16 weight pairs (SURVEY.md 8d C5:
+weight deltas + CLIP attention, on 1 x H100. Synthetic fp16 weight pairs (
 dW = lowrank(8)*0.02 + noise*1e-3). Prints matrices/s and algorithmic GB/s (ONE read of both
 fp16 models = 2*2*sum(N*K) bytes) against the measured HBM peak, and the reference's way
 (serial torch.linalg.svd, full_matrices default, cli_svd.py:35) timed on a subset."""

@@ -1,11 +1,10 @@
-"""Round-2 opener: time the EXPERIMENTAL cluster split-K schedule (csrc/fused_splitk.cuh) against
-the default schedule on the small-M / long-K SD1.5 sites.
+"""Time the cluster split-K schedule (lb_debug_set_linear_mode schedule 3, csrc/fused_core.cuh with
+CL > 1) against the other schedules on the small-M / long-K SD1.5 sites.
 
 Launches are enqueued back to back (REPS per measurement, one CUDA-event pair around the batch,
-rotating over enough operand sets to exceed the 126 MB L2 when COLD=1), so the GPU never waits for
+rotating over enough operand sets to exceed the 50 MB L2 when COLD=1), so the GPU never waits for
 Python -- scripts/prof_site.py's per-launch event pairs measure CPU launch latency for kernels this
-short. Run the parity test first (LB_EXPERIMENTAL=1 pytest tests/test_zz_splitk_experimental_gpu.py):
-a protocol bug in the kernel traps.
+short. Run the parity test first (pytest tests/test_zz_splitk_experimental_gpu.py).
     python scripts/prof_splitk.py            # -> gpurun_out/splitk_times.json
 """
 import json

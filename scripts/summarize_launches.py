@@ -24,7 +24,7 @@ else:
 
 def family(name):
     n = name
-    for pat, fam in [(r"fused_lora", "OURS fused_lora (tcgen05 fwd/dX)"), (r"wgrad_kernel", "OURS wgrad (dA/dB)"),
+    for pat, fam in [(r"fused_lora", "OURS fused_lora (wgmma fwd/dX)"), (r"wgrad_kernel", "OURS wgrad (dA/dB)"),
                      (r"adamw_update|sqnorm_partial|optim_step_", "OURS clip+AdamW (one launch)"), (r"prologue_kernel|masked_mse_kernel", "OURS step prologue / loss"), (r"refresh_shadows|cast_rows|cast_weight|cast_conv", "OURS casts/shadows"),
                      (r"up_dropout|dropout_dt", "OURS dropout branch"),
                      (r"fmha|flash|attention|sdp", "attention (SDPA)"), (r"cudnn|conv|implicit_gemm|xmma|cutlass.*conv|sm\d+_xmma|wgrad|dgrad", "cuDNN conv"),

@@ -22,7 +22,7 @@ def _sites(model):
 
 
 def test_constructor_consumes_rng_like_the_reference():
-    """Seed parity (SURVEY.md 7): after manual_seed(0) the down factor and the NEXT random draw
+    """Seed parity: after manual_seed(0) the down factor and the NEXT random draw
     equal the reference's (it burns three kaiming inits before normal_, lora.py:43-50)."""
     g = torch.load(f"{GOLD}/ctor_rng.pt")
     torch.manual_seed(0)
@@ -225,7 +225,7 @@ def test_collapse_add_scale_diag_inspect():
 
 
 def test_fixture_manifest_layout():
-    """The ten fixture files of the reference pin the on-disk layout (SURVEY.md 4). The manifest
+    """The ten fixture files of the reference pin the on-disk layout. The manifest
     (keys, shapes, dtypes, metadata, what the reference's own parse_safeloras returned) travels
     with the repo; where the files themselves are mounted, our parser is run on them too."""
     man = json.load(open(f"{GOLD}/example_loras_manifest.json"))

@@ -1,4 +1,4 @@
-"""GPU parity of the fused LoRA Conv2d path (NHWC implicit GEMM on tcgen05) against the oracle
+"""GPU parity of the fused LoRA Conv2d path (NHWC implicit GEMM on wgmma) against the oracle
 (oracle/lora_ops.py: lora_conv2d_forward / lora_conv2d_backward, float64), through the module API.
 
 Tolerances: 16-bit operands, fp32 accumulate. Outputs are compared with the oracle evaluated on the

@@ -127,7 +127,7 @@ def _svd_worker(rank, world, port, out_dir):
 
 
 def test_sharded_svd_distill_equals_single_process(tmp_path):
-    """SURVEY.md 8(e), config C5 on several GPUs: weight deltas are sharded round-robin over the
+    """SVD distillation on several GPUs: weight deltas are sharded round-robin over the
     ranks (no collective on the compute path), factors exchanged by one all-reduce over a
     zero-padded flat buffer; every rank must end with exactly the single-process result."""
     import lora_b200.svd as svd

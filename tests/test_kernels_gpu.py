@@ -53,7 +53,7 @@ def run_fused(x, W, A, B, b, d, scale, out_dtype, want_t=True):
 
 
 SHAPES = [
-    # (M, K, N, r)  -- SD1.5 site census (SURVEY.md Appendix A) + ragged edges
+    # (M, K, N, r)  -- SD1.5 site census + ragged edges
     (4096, 320, 320, 4),
     (4096, 320, 2560, 4),
     (1024, 640, 640, 4),
@@ -156,7 +156,7 @@ def test_backward_kernels_match_oracle(M, K, N, r):
 
 @pytest.mark.parametrize("M,K,N,r", [(256, 1280, 2304, 4), (64, 640, 1000, 8), (300, 320, 192, 4)])
 def test_block_n_192_schedule_matches_default(M, K, N, r):
-    """The 192-wide tile (13 TMEM-resident n8 groups, 3 store boxes; 16-bit outputs) is the same math."""
+    """The 192-wide tile (208-column accumulator incl. T, 3 store boxes; 16-bit outputs) is the same math."""
     from lora_b200 import _C
     x, W, A, B, b, d = make_case(M, K, N, r, torch.bfloat16, seed=M + N + r, diag=True)
     try:
@@ -172,8 +172,10 @@ def test_block_n_192_schedule_matches_default(M, K, N, r):
 @pytest.mark.parametrize("mode", [1 + 4, 1 + 8, 2 + 4, 2 + 8])
 @pytest.mark.parametrize("M,K,N,r", SHAPES)
 def test_every_tile_schedule_gives_the_same_result(M, K, N, r, mode):
-    """One-tile-per-CTA vs persistent (double-buffered TMEM), BLOCK_N 64 vs 128: same math, results
-    equal to fp32-accumulation noise (1e-5) between schedules and vs the oracle."""
+    """Forced schedules 1 (one tile per CTA; 2 CTAs per SM on crowded sites) and 2 (one CTA per SM)
+    at BLOCK_N 64 and 128 vs the auto schedule: same math, results equal to fp32-accumulation noise
+    (1e-5) between schedules and vs the oracle. The cluster split-K schedule is
+    tests/test_zz_splitk_experimental_gpu.py."""
     from lora_b200 import _C
     x, W, A, B, b, d = make_case(M, K, N, r, torch.bfloat16, seed=M * 3 + N + r, diag=True)
     try:

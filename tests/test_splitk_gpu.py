@@ -19,7 +19,7 @@ def rel(a, b):
     return float((a - b).norm() / (b.norm() + 1e-30))
 
 
-# (M, K, N, r): shapes for which plan_split() chooses split > 1 on a 148-SM part
+# (M, K, N, r): shapes for which plan_split() chooses split > 1 on a 132-SM H100
 LONG_K = [(256, 10240, 1280, 4), (1024, 5120, 640, 8), (64, 10240, 1280, 16), (256, 5120, 1280, 4),
           (77, 2560, 768, 12), (1, 5120, 320, 8), (200, 2560, 136, 3)]
 

@@ -1,7 +1,7 @@
 """GPU parity of the batched truncated SVD (csrc/svd.cu, lora_b200/svd.py) against the oracle's
 exact SVD (oracle/svd_ref.py, restating cli_svd.py:24-92), on the sign-invariant quantities:
 singular values, the rank-r product before clamping, orthonormality of the right factor, and the
-clamp rule. Inputs follow SURVEY.md 8(d) C5: dW = lowrank(8) * 0.02 + noise * 1e-3, fp16 weights."""
+clamp rule. Inputs: dW = lowrank(8) * 0.02 + noise * 1e-3, fp16 weights."""
 import pytest
 import torch
 
@@ -99,7 +99,7 @@ def test_overwrite_base_matches_oracle_on_tiny_models():
         assert a.lora_up.weight.dtype == torch.float16
         ours = a.lora_up.weight.data.float().flatten(1).cpu() @ a.lora_down.weight.data.float().flatten(1).cpu()
         # The reference's threshold `hi` is a quantile over SIGNED factor entries, hence depends on the
-        # (arbitrary) sign of each singular pair (SURVEY.md 7). Sign-invariant statement: clamping the
+        # (arbitrary) sign of each singular pair. Sign-invariant statement: clamping the
         # exact factors at OUR threshold reproduces our clamped product.
         u2, d2, hi_ours = svd_ref.clamp_rule(a.lora_up.weight.data.float().cpu(), a.lora_down.weight.data.float().cpu(), 0.99)
         hi_eff = float(max(a.lora_up.weight.data.abs().max(), a.lora_down.weight.data.abs().max()))

@@ -1,4 +1,4 @@
-"""SURVEY.md 8(f) ranks 3/4 on the GPU: the PTI step variants either side of the UNet call --
+"""On the GPU: the PTI step variants either side of the UNet call --
 masked loss (cli_lora_pti.py:340-368), t_mutliplier (:298-304), the inpainting input
 (:279-313, 9-channel UNet) -- through lora_b200.train.LoraTrainStep (fused LoRA kernels, arena
 optimizer) against the oracle step (oracle/ref_step.py, itself pinned to the reference's

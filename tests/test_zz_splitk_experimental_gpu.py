@@ -1,9 +1,13 @@
-"""EXPERIMENTAL cluster split-K schedule of the fused LoRA linear kernel (csrc/fused_splitk.cuh).
+"""Cluster split-K schedule of the fused LoRA linear kernel (lb_debug_set_linear_mode schedule 3:
+2..4 CTAs of a thread-block cluster share each tile's K loop and merge through distributed shared
+memory; the auto planner uses the 2-CTA form on few-tile, K >= 640 sites).
 
-Opt-in: runs only with LB_EXPERIMENTAL=1 in the environment. The kernel was written after round
-1's GPU budget was spent (compiled and SASS-inspected, never executed); a protocol bug in it would
-`__trap` and poison the CUDA context of the whole pytest process, so it must not run by default.
-    LB_EXPERIMENTAL=1 python -m pytest tests/test_zz_splitk_experimental_gpu.py -x -q
+Every case runs by default except the schedule FORCED onto K = 10240 with 2 CTAs per tile (and the
+128-wide case on the same shape), which is opt-in (LB_EXPERIMENTAL=1). There T differs from the
+default schedule's T -- the L2-reduction split-K the planner picks for that site -- by 3.3-3.4e-6
+(relative) on an H100, above the 3e-6 bound: two fp32 tensor-core reductions over 5120-long K
+halves in different orders. The auto planner never sends such long-K sites to the cluster form.
+    LB_EXPERIMENTAL=1 python -m pytest tests/test_zz_splitk_experimental_gpu.py -q
 Same acceptance as tests/test_kernels_gpu.py::test_every_tile_schedule_gives_the_same_result."""
 import os
 
@@ -12,9 +16,13 @@ import torch
 
 from oracle import lora_ops as O
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(os.environ.get("LB_EXPERIMENTAL") != "1",
-                                 reason="experimental kernel: set LB_EXPERIMENTAL=1 to run")]
+pytestmark = pytest.mark.gpu
+
+
+def _skip_forced_long_k(K, split):
+    if K == 10240 and split == 2 and os.environ.get("LB_EXPERIMENTAL") != "1":
+        pytest.skip("opt-in: forced 2-way cluster split at K = 10240 differs from the L2 split-K's T by "
+                    "3.3e-6 > 3e-6 (see module docstring)")
 
 SHAPES = [(77, 768, 768, 4), (77, 768, 320, 4), (256, 1280, 1280, 4), (64, 1280, 1280, 8),
           (1024, 640, 640, 4), (256, 10240, 1280, 4), (300, 200, 136, 16), (128, 64, 64, 1)]
@@ -24,6 +32,7 @@ SHAPES = [(77, 768, 768, 4), (77, 768, 320, 4), (256, 1280, 1280, 4), (64, 1280,
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
 @pytest.mark.parametrize("M,K,N,r", SHAPES)
 def test_cluster_splitk_matches_default_schedule(M, K, N, r, split, out_dtype):
+    _skip_forced_long_k(K, split)
     from lora_b200 import _C
     from test_kernels_gpu import make_case, rel_err, run_fused     # tests/ is on sys.path under pytest
     x, W, A, B, b, d = make_case(M, K, N, r, torch.bfloat16, seed=M + K + N + r, diag=True)
@@ -43,6 +52,7 @@ def test_cluster_splitk_matches_default_schedule(M, K, N, r, split, out_dtype):
 
 
 def test_cluster_splitk_wide_tiles():
+    _skip_forced_long_k(10240, 2)
     from lora_b200 import _C
     from test_kernels_gpu import make_case, rel_err, run_fused     # tests/ is on sys.path under pytest
     x, W, A, B, b, d = make_case(256, 10240, 1280, 4, torch.bfloat16, seed=5, diag=False)
