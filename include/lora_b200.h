@@ -76,20 +76,6 @@ int lb_lora_linear_fwd_dropout(const void* X, const void* W, const float* bias, 
                                int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
                                void* stream);
 
-/* Input gradient of lb_lora_linear_fwd_dropout in ONE launch:
- *     dX[M, K_in] = gY . W + (((mask o gY) . B) * (scale * diag / (1-p))) . A ,  T_out = (mask o gY) . B
- * with gY [M, N_out], Wt = W^T [K_in, N_out] (pre-transposed frozen weight), upT16 = B^T padded [16, N_out],
- * `down` = A read transposed (element (k, j) at down[k*down_rs + j*down_cs]: down_rs = 1, down_cs = K_in).
- * The mask (same counter hash as the forward, element index m*N_out + n) is applied to a shared-memory
- * copy of every gY tile by the consumer warpgroups inside the MMA loop (one named barrier per K
- * block) and feeds only the rank-r MMA -- no separate pass over gY (the alternative is
- * lb_lora_dropout_dt + T_in). dA then is lb_lora_wgrad(X, T_out) with
- * scale / (1-p); dB the masked reduction. */
-int lb_lora_linear_dx_dropout(const void* gY, const void* Wt, const void* upT16, const float* down,
-                              long long down_rs, long long down_cs, const float* diag, float scale,
-                              void* dX, float* T_out, int M, int N_out, int K_in, int r, int in_dtype,
-                              int out_dtype, float drop_p, const void* seed_dev, void* stream);
-
 /* Up to 4 independent lb_lora_linear_fwd problems of the same operand/output dtype in ONE launch
  * (sites that share an input -- q/k/v of a self-attention, k/v of a cross-attention, CLIP's k/v/q --
  * each under-fill 132 SMs on their own). All array arguments are HOST arrays of length n; per-problem
@@ -232,16 +218,6 @@ int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias, 
                                float scale, void* Y, float* T_out, int n_img, int H, int Wd, int Cin,
                                int Cout, int kh, int kw, int pad_h, int pad_w, int r, int in_dtype,
                                int out_dtype, float drop_p, const void* seed_dev, void* stream);
-
-/* Input gradient of lb_lora_conv2d_fwd_dropout in one launch (the conv analogue of
- * lb_lora_linear_dx_dropout): gY NHWC [n_img, H, Wd, Cout], Wb = flipped/transposed frozen weight
- * [Cin, kh*kw*Cout], upT16 = B^T padded [16, Cout], `down` = A read flipped (see lb_lora_conv2d_fwd,
- * per_tap_T = 1), pad_* = kh-1-pad of the forward. T_out = (mask o gY) . B at the unshifted tap. */
-int lb_lora_conv2d_dx_dropout(const void* gY, const void* Wb, const void* upT16, const float* down,
-                              long long down_rs, long long down_cs, long long down_gs, const float* diag,
-                              float scale, void* dX, float* T_out, int n_img, int H, int Wd, int Cout,
-                              int Cin, int kh, int kw, int pad_h, int pad_w, int r, int in_dtype,
-                              int out_dtype, float drop_p, const void* seed_dev, void* stream);
 
 /* Frozen conv-weight preparation: src [Cout,Cin,kh,kw] (LB_F32/LB_BF16/LB_F16) ->
  *   dst16  [Cout, kh*kw*Cin]  (tap-major K; forward operand)              and/or

@@ -47,10 +47,6 @@ def _load():
         "lb_lora_conv2d_fwd_dropout": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp,
                                         i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
                                         f32, vp, vp], i32),
-        "lb_lora_linear_dx_dropout": ([vp, vp, vp, vp, ll, ll, vp, f32, vp, vp, i32, i32, i32, i32, i32, i32,
-                                       f32, vp, vp], i32),
-        "lb_lora_conv2d_dx_dropout": ([vp, vp, vp, vp, ll, ll, ll, vp, f32, vp, vp, i32, i32, i32, i32, i32,
-                                       i32, i32, i32, i32, i32, i32, i32, f32, vp, vp], i32),
         "lb_tiled_weight_elems": ([i32, i32], ll),
         "lb_tile_weight": ([vp, i32, ll, ll, i32, i32, vp, i32, vp], i32),
         "lb_lora_wgrad": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, vp], i32),
@@ -135,8 +131,7 @@ EXPORTED = [n for n in ("lb_abi_version", "lb_lora_linear_fwd", "lb_lora_wgrad",
                         "lb_svd_chol_inv", "lb_svd_apply", "lb_svd_jacobi", "lb_svd_randn", "lb_split_bf16x3", "lb_lora_merge", "lb_ti_embed_step", "lb_lora_linear_fwd_grouped", "lb_lora_wgrad_multi", "lb_lora_wgrad_conv",
                         "lb_lora_linear_fwd_dropout", "lb_lora_conv2d_fwd_dropout", "lb_debug_set_pdl", "lb_svd_workspace_bytes", "lb_svd_truncated_batched",
                         "lb_optim_step_fused", "lb_step_prologue", "lb_masked_mse_fwd_bwd",
-                        "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_lora_linear_dx_dropout", "lb_tiled_weight_elems", "lb_tile_weight",
-                        "lb_lora_conv2d_dx_dropout")]
+                        "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight")]
 
 
 def check(status: int, what: str):

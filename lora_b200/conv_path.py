@@ -124,14 +124,14 @@ class _FusedLoraConv2dFn(torch.autograd.Function):
         if need_a:
             tgt = sink[0] if sink is not None else torch.zeros((r, cin * taps), device=gy.device,
                                                                dtype=torch.float32)
-            ops.wgrad_conv(x16, dTs, ctx.diag, ctx.scale, tgt, r, cin, h, w, kh, kw, ph, pw, async_ok=sink is not None)
+            ops.wgrad_conv(x16, dTs, ctx.diag, ctx.scale, tgt, r, cin, h, w, kh, kw, ph, pw, deferrable=sink is not None)
             if sink is None:
                 dA = tgt.view_as(A).to(A.dtype)
         if need_b:
             tgt = sink[1] if sink is not None else torch.zeros((cout, r), device=gy.device,
                                                                dtype=torch.float32)
             gy2d = gy16.permute(0, 2, 3, 1).reshape(n * h * w, cout)       # NHWC bytes as [pixels, Cout]
-            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tgt, 1, r, r, async_ok=sink is not None)
+            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tgt, 1, r, r, deferrable=sink is not None)
             if sink is None:
                 dB = tgt.view_as(B).to(B.dtype)
         dx = dX.to(ctx.x_dtype) if need_x else None

@@ -1,20 +1,19 @@
 // C-ABI entry point for the fused LoRA Conv2d (NHWC implicit GEMM, stride 1, dilation 1,
 // groups 1; 1x1 and 3x3 in the SD1.5 ResnetBlock2D sites). Forward and, on flipped/transposed
 // frozen weights, the input gradient. Replaces LoraInjectedConv2d.forward
-// (/root/reference/lora_diffusion/lora.py:130-135) and the dX part of its autograd backward.
+// (lora_diffusion/lora.py:130-135 of cloneofsimo/lora) and the dX part of its autograd backward.
 // Kernel: fused_core.cuh.
-#include <stdlib.h>
 #include "fused_core.cuh"
 #include "lora_b200.h"
 #include "tmap.h"
 
 namespace lb {
 
-template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, bool SPLITK = false, bool BMASK = false>
+template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, bool SPLITK = false>
 static int launch_conv(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p_in,
                        int n_img, int down_cols, int out_dtype, cudaStream_t stream, int split = 1) {
-  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP, BMASK>;
-  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, true, G, 1, DROP, SPLITK, BMASK>;
+  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP>;
+  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, true, G, 1, DROP, SPLITK>;
   FusedParams p = p_in;
   p.split = 1;
   if constexpr (SPLITK) {
@@ -71,12 +70,10 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
                                   void* Y, float* T_out, const float* T_in, int n_img, int H, int Wd, int Cin,
                                   int Cout, int kh, int kw, int pad_h, int pad_w, int r,
                                   int per_tap_T, int in_dtype, int out_dtype, float drop_p,
-                                  const void* seed_dev, void* stream, int mask_input = 0) {
+                                  const void* seed_dev, void* stream) {
   using namespace lb;
-  if (!(drop_p >= 0.f && drop_p < 1.f) ||
-      (drop_p > 0.f && (seed_dev == nullptr || T_in != nullptr || (per_tap_T != 0 && !mask_input))))
+  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && (seed_dev == nullptr || T_in != nullptr || per_tap_T != 0)))
     return LB_ERR_SHAPE;
-  if (mask_input && !(drop_p > 0.f)) return LB_ERR_SHAPE;
   if (n_img <= 0 || H <= 0 || Wd <= 0 || Cin <= 0 || Cout <= 0) return LB_ERR_SHAPE;
   if (!((kh == 1 && kw == 1) || (kh == 3 && kw == 3))) return LB_ERR_SHAPE;
   // "same" geometry only (output extent == input extent), which is what stride-1 SD convs use
@@ -107,40 +104,14 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
   const int down_cols = groups ? Cin : taps * Cin;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 
-  const long long tiles128 = static_cast<long long>(n_img) * p.tiles_h * p.tiles_w * ((Cout + 127) / 128);
   // 64-wide tiles only while they still fit ONE wave (one CTA per SM: two of these rings do not fit an SM):
-  // the 64x64-pixel, Cout = 320 sites are 96 tiles of 128 but 160 of 64 -- a second wave over 45-135 K
-  // blocks (LB_CONV_NARROW_OLD=1 restores the round-2a rule `tiles128 < 120` for A/B)
-  static int old_rule = -1;
-  if (old_rule < 0) { const char* e = getenv("LB_CONV_NARROW_OLD"); old_rule = (e && e[0] == '1') ? 1 : 0; }
+  // the 64x64-pixel, Cout = 320 sites are 96 tiles of 128 but 160 of 64 -- a second wave over 45-135 K blocks
   const long long tiles64c = static_cast<long long>(n_img) * p.tiles_h * p.tiles_w * ((Cout + 63) / 64);
-  const bool narrow = old_rule ? tiles128 < 120 : tiles64c <= sm_count();
+  const bool narrow = tiles64c <= sm_count();
 #define LB_CONV(BN, OT, GG) launch_conv<BN, 4, OT, GG>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
   const int cblocks = (Cin + BLOCK_K - 1) / BLOCK_K;
   const ConvPlan sp = plan_conv_split(static_cast<long long>(n_img) * p.tiles_h * p.tiles_w, taps * cblocks, Cout,
                                       groups ? taps : 1, sm_count());
-  if (mask_input) {
-    // dropout BACKWARD (input gradient): the T path sees mask o gY (fused_core.cuh, BMASK); mask index
-    // = pixel * Cin' + channel of the gY element (Cin' = this pass's input channels = the forward's Cout)
-#define LB_CONVM(BN, ST, OT, GG) launch_conv<BN, ST, OT, GG, false, false, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
-#define LB_CONVMS(BN, ST, OT, GG) launch_conv<BN, ST, OT, GG, false, true, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, sp.split)
-    if (sp.split > 1) {
-      if (groups) {
-        if (out_dtype == LB_F32) return LB_CONVMS(64, 3, float, 9);
-        return LB_CONVMS(64, 3, uint16_t, 9);
-      }
-      if (out_dtype == LB_F32) return LB_CONVMS(64, 4, float, 1);
-      return LB_CONVMS(64, 4, uint16_t, 1);
-    }
-    if (groups) {
-      if (out_dtype == LB_F32) return narrow ? LB_CONVM(64, 3, float, 9) : LB_CONVM(128, 2, float, 9);
-      return narrow ? LB_CONVM(64, 3, uint16_t, 9) : LB_CONVM(128, 3, uint16_t, 9);
-    }
-    if (out_dtype == LB_F32) return narrow ? LB_CONVM(64, 4, float, 1) : LB_CONVM(128, 3, float, 1);
-    return narrow ? LB_CONVM(64, 4, uint16_t, 1) : LB_CONVM(128, 3, uint16_t, 1);
-#undef LB_CONVM
-#undef LB_CONVMS
-  }
   if (drop_p > 0.f) {   // forward with dropout on the branch: masked in the drain (DROP kernels)
 #define LB_CONVD(BN, OT) launch_conv<BN, 4, OT, 1, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
 #define LB_CONVDS(BN, OT) launch_conv<BN, 4, OT, 1, true, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, sp.split)
@@ -194,15 +165,4 @@ extern "C" int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const fl
   return conv2d_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, 0, diag, scale, Y, T_out, nullptr, n_img, H,
                          Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, 0, in_dtype, out_dtype, drop_p, seed_dev,
                          stream);
-}
-
-extern "C" int lb_lora_conv2d_dx_dropout(const void* gY, const void* Wb, const void* upT16, const float* down,
-                                         long long down_rs, long long down_cs, long long down_gs,
-                                         const float* diag, float scale, void* dX, float* T_out, int n_img,
-                                         int H, int Wd, int Cout, int Cin, int kh, int kw, int pad_h, int pad_w,
-                                         int r, int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                                         void* stream) {
-  return conv2d_fwd_impl(gY, Wb, nullptr, upT16, down, down_rs, down_cs, down_gs, diag, scale, dX, T_out, nullptr,
-                         n_img, H, Wd, Cout, Cin, kh, kw, pad_h, pad_w, r, 1, in_dtype, out_dtype, drop_p, seed_dev,
-                         stream, 1);
 }

@@ -111,14 +111,11 @@ __device__ __forceinline__ unsigned long long gtimer() {
 }
 #define LB_STAMP(i) do { if (p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0) p.dbg[i] = gtimer(); } while (0)
 
-template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, bool BMASK = false, int CL = 1>
+template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, int CL = 1>
 struct Smem {
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_BYTES = (BLOCK_N + R_PAD) * BLOCK_K * 2;
-  // BMASK (dropout backward): every stage also holds the MASKED copy of the A tile (mask o gY), the
-  // operand of the T MMA; the TMA transaction still covers A + B only
-  static constexpr int TX_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES + (BMASK ? A_BYTES : 0);
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // one TMA transaction: X tile, W tile + D rows
   // fp32 accumulator parked after the K loop: base columns, T group(s), and (DROP) the LoRA product,
   // which the mask separates from the sum. Row pitch padded by 8 floats against bank conflicts.
   static constexpr int L_COL0 = BLOCK_N + R_PAD * G;
@@ -202,16 +199,15 @@ __device__ __forceinline__ void ld_acc16(const float* src, float* v) {
 
 // One output tile (n_blk, m_blk) of one problem; called by the single-problem and the grouped kernel.
 template <int BLOCK_N, int STAGES, typename OutT, bool CONV, int G, bool DROP = false, bool SPLITK = false,
-          bool BMASK = false, int CL = 1, bool INLINE_TMA = false>
+          int CL = 1, bool INLINE_TMA = false>
 __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtensorMap& tmW,
                                            const CUtensorMap& tmD, const CUtensorMap& tmY,
                                            const FusedParams& p, const int n_blk, const int m_blk) {
-  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP, BMASK, CL>;
-  static_assert(!(BMASK && DROP), "BMASK is the backward of DROP");
-  static_assert(CL == 1 || (!CONV && G == 1 && !DROP && !SPLITK && !BMASK), "cluster split-K: plain linear tiles");
-  static_assert(!INLINE_TMA || (!CONV && G == 1 && !DROP && !SPLITK && !BMASK && CL == 1), "inline TMA: plain linear tiles");
+  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP, CL>;
+  static_assert(CL == 1 || (!CONV && G == 1 && !DROP && !SPLITK), "cluster split-K: plain linear tiles");
+  static_assert(!INLINE_TMA || (!CONV && G == 1 && !DROP && !SPLITK && CL == 1), "inline TMA: plain linear tiles");
   constexpr int PCOLS = BLOCK_N + R_PAD * G;          // columns of one partial accumulator
-  constexpr bool WIDE = (G == 1 && !BMASK);           // T rides the base MMA as 16 extra columns
+  constexpr bool WIDE = G == 1;                       // T rides the base MMA as 16 extra columns
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sgen = smem_raw + (sbase - smem_u32(smem_raw));  // generic pointer to the aligned base
@@ -273,7 +269,7 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
     const int it = kb - kb_begin;
     const int s = it % STAGES;
     mbar_wait(bar_empty(s), ((it / STAGES) & 1) ^ 1);
-    mbar_expect_tx(bar_full(s), S::TX_BYTES);
+    mbar_expect_tx(bar_full(s), S::STAGE_BYTES);
     const uint32_t sa = sbase + s * S::STAGE_BYTES;
     const uint32_t sb = sa + S::A_BYTES;
     if constexpr (CONV) {
@@ -343,14 +339,6 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
 #pragma unroll
     for (int i = 0; i < R_PAD / 2; ++i) tacc[g][i] = 0.f;
 
-  uint32_t ms0 = 0, ms1 = 0, mthr = 0;
-  if constexpr (BMASK) {
-    const unsigned long long msd = __ldg(p.seed);
-    ms0 = static_cast<uint32_t>(msd);
-    ms1 = static_cast<uint32_t>(msd >> 32);
-    mthr = drop_threshold(p.drop_p);
-  }
-
   // one K block; `tdst` = the T accumulator of the block's tap (unused when WIDE). The caller picks
   // it with a compile-time index: a wgmma under a data-dependent branch would be serialized.
   auto k_block = [&](const int kb, float* tdst) {
@@ -361,52 +349,6 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
     if (it == 0 && ct == 0) LB_STAMP(2);          // first stage landed
     const uint32_t sa = sbase + s * S::STAGE_BYTES;
     const uint32_t sb = sa + S::A_BYTES;
-    const int tap = (G > 1) ? kb / cblocks : 0;
-    if constexpr (BMASK) {
-      // Dropout backward: dT = (mask o gY / (1-p)) . B needs the MASKED gY tile as the T MMA's A
-      // operand: copy the TMA-landed tile (128 rows x 64 columns, 128B-swizzled) into the stage's
-      // second buffer with the dropped elements zeroed (same counter hash as the forward drain;
-      // 1/(1-p) is folded into coef below). Thread -> logical 16-byte chunk (ct & 7) of rows
-      // (ct >> 3) + 32 i: conflict-free in shared memory.
-      const uint32_t sm = sb + S::B_BYTES;
-      const int mc = ct & 7;
-      const unsigned long long ncols = CONV ? p.C : p.K;      // row pitch of the mask = columns of gY
-      int tdy = 0, tdx = 0, col0 = kb * BLOCK_K;
-      if constexpr (CONV) {
-        const int cb = kb - tap * cblocks;
-        tdy = tap / p.kw - p.pad_h;
-        tdx = tap % p.kw - p.pad_w;
-        col0 = cb * BLOCK_K;
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = (ct >> 3) + 32 * i;
-        long long gr = -1;
-        if constexpr (CONV) {
-          const int hh = h0 + r / p.TW + tdy, ww = w0 + r % p.TW + tdx;
-          if (hh >= 0 && hh < p.H && ww >= 0 && ww < p.W) gr = (static_cast<long long>(img) * p.H + hh) * p.W + ww;
-        } else {
-          if (m0 + r < p.M) gr = m0 + r;
-        }
-        const uint32_t off = r * 128 + ((mc ^ (r & 7)) << 4);
-        uint32_t w0_, w1_, w2_, w3_;
-        asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w0_), "=r"(w1_), "=r"(w2_), "=r"(w3_) : "r"(sa + off));
-        if (gr >= 0) {
-          const unsigned long long e0 = (static_cast<unsigned long long>(gr) * ncols + col0 + mc * 8) >> 1;
-          uint32_t wv[4] = {w0_, w1_, w2_, w3_};
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            const uint32_t bits = drop_bits(ms0, ms1, e0 + qd);
-            const uint32_t keep = ((bits & 0xffffu) >= mthr ? 0x0000ffffu : 0u) | ((bits >> 16) >= mthr ? 0xffff0000u : 0u);
-            wv[qd] &= keep;
-          }
-          w0_ = wv[0]; w1_ = wv[1]; w2_ = wv[2]; w3_ = wv[3];
-        }
-        st_shared_v4(sm + off, w0_, w1_, w2_, w3_);
-      }
-      fence_proxy_async_smem();      // generic-proxy writes -> visible to the tensor-core proxy
-      named_bar_sync(BAR_CONSUMERS, CONSUMER_THREADS);
-    }
     reg_fence<AREG>(acc);
     wgmma_fence();
 #pragma unroll
@@ -418,9 +360,8 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
         wgmma_ss<BLOCK_N + R_PAD>(acc, ad, bd, p.fmt);
       } else {
         const uint64_t dd = wgmma_desc(sb + BLOCK_N * 128 + k * MMA_K * 2, 16, 1024, 1);
-        const uint64_t td = BMASK ? wgmma_desc(sb + S::B_BYTES + wg * (64 * 128) + k * MMA_K * 2, 16, 1024, 1) : ad;
         wgmma_ss<BLOCK_N>(acc, ad, bd, p.fmt);
-        wgmma_ss<R_PAD>(tdst, td, dd, p.fmt);
+        wgmma_ss<R_PAD>(tdst, ad, dd, p.fmt);
       }
     }
     wgmma_commit();
@@ -435,9 +376,9 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
     for (int kb = kb_begin; kb < kb_end; ++kb) k_block(kb, nullptr);
   } else {
 #pragma unroll
-    for (int g = 0; g < TG; ++g) {   // tap g's K blocks (G == 1: all of them) within this CTA's range
-      const int b0 = (G > 1 && g * cblocks > kb_begin) ? g * cblocks : kb_begin;
-      const int b1 = (G > 1 && (g + 1) * cblocks < kb_end) ? (g + 1) * cblocks : kb_end;
+    for (int g = 0; g < TG; ++g) {   // tap g's K blocks within this CTA's range
+      const int b0 = g * cblocks > kb_begin ? g * cblocks : kb_begin;
+      const int b1 = (g + 1) * cblocks < kb_end ? (g + 1) * cblocks : kb_end;
       for (int kb = b0; kb < b1; ++kb) k_block(kb, tacc[g]);
     }
   }
@@ -498,7 +439,7 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
     float coef[R_PAD];
 #pragma unroll
     for (int j = 0; j < R_PAD; ++j)
-      coef[j] = (j < p.r) ? p.scale * (p.diag ? __ldg(p.diag + j) : 1.f) * (BMASK ? p.drop_inv : 1.f) : 0.f;
+      coef[j] = (j < p.r) ? p.scale * (p.diag ? __ldg(p.diag + j) : 1.f) : 0.f;
     if constexpr (CONV) {
       const int hh = h0 + row / p.TW, ww = w0 + row % p.TW;
       if (hh < p.H && ww < p.W) grow = (static_cast<long long>(img) * p.H + hh) * p.W + ww;
@@ -751,13 +692,12 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
 }
 
 template <int BLOCK_N, int STAGES, typename OutT, bool CONV, int G, int MIN_CTAS = 1, bool DROP = false,
-          bool SPLITK = false, bool BMASK = false, int CL = 1, bool INLINE_TMA = false>
+          bool SPLITK = false, int CL = 1, bool INLINE_TMA = false>
 __global__ void __launch_bounds__(kernel_threads<INLINE_TMA>(), MIN_CTAS)
 fused_lora_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                   const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmY,
                   const FusedParams p) {
-  fused_tile<BLOCK_N, STAGES, OutT, CONV, G, DROP, SPLITK, BMASK, CL, INLINE_TMA>(tmX, tmW, tmD, tmY, p, blockIdx.x,
-                                                                                blockIdx.y);
+  fused_tile<BLOCK_N, STAGES, OutT, CONV, G, DROP, SPLITK, CL, INLINE_TMA>(tmX, tmW, tmD, tmY, p, blockIdx.x, blockIdx.y);
 }
 
 // Several same-dtype linear problems in ONE launch (sites that share an input: q/k/v of an
@@ -781,8 +721,8 @@ fused_lora_grouped_kernel(const __grid_constant__ GroupedArgs a) {
     if (i < a.n_problems && static_cast<int>(blockIdx.x) >= a.tile_start[i]) q = i;
   const int local = blockIdx.x - a.tile_start[q];
   const int n_blk = local % a.n_tiles_n[q], m_blk = local / a.n_tiles_n[q];
-  fused_tile<BLOCK_N, STAGES, OutT, false, 1, false, false, false, 1, INLINE_TMA>(a.tmX[q], a.tmW[q], a.tmD[q], a.tmY[q],
-                                                                                a.p[q], n_blk, m_blk);
+  fused_tile<BLOCK_N, STAGES, OutT, false, 1, false, false, 1, INLINE_TMA>(a.tmX[q], a.tmW[q], a.tmD[q], a.tmY[q],
+                                                                         a.p[q], n_blk, m_blk);
 }
 
 }  // namespace lb

@@ -1,7 +1,6 @@
 // C-ABI entry point for the fused LoRA linear (forward and, on transposed operands, dX).
 // Replaces LoraInjectedLinear.forward (lora_diffusion/lora.py:53-58 of cloneofsimo/lora) and the dX
 // part of its autograd backward. Kernel: fused_core.cuh.
-#include <stdlib.h>
 #include "fused_core.cuh"
 #include "lora_b200.h"
 #include "tmap.h"
@@ -17,11 +16,11 @@ static bool tmap_weight(CUtensorMap* tm, const void* W, CUtensorMapDataType dt, 
 }
 
 template <int BLOCK_N, int STAGES, typename OutT, int MIN_CTAS, bool DROP = false, bool SPLITK = false,
-          bool BMASK = false, int CL = 1, bool INLINE_TMA = false>
+          int CL = 1, bool INLINE_TMA = false>
 static int launch_linear(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p_in,
                          int out_dtype, cudaStream_t stream, int split = 1) {
-  using S = Smem<BLOCK_N, STAGES, OutT, 1, DROP, BMASK, CL>;
-  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, false, 1, MIN_CTAS, DROP, SPLITK, BMASK, CL, INLINE_TMA>;
+  using S = Smem<BLOCK_N, STAGES, OutT, 1, DROP, CL>;
+  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, false, 1, MIN_CTAS, DROP, SPLITK, CL, INLINE_TMA>;
   FusedParams p = p_in;
   p.split = 1;
   if constexpr (SPLITK) {
@@ -59,20 +58,6 @@ static SplitPlan plan_split(int M, int K, int N, int n_sms) {
   if (!splitk_enabled() || n_sms <= 0) return {0, 1};
   const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
   const int m_tiles = (M + BLOCK_M - 1) / BLOCK_M;
-  {  // profiling knob: LB_SPLIT_FORCE=<s> forces a split wherever it fits in one wave
-    static int force = -1;
-    const int force_bn = 64;
-    if (force < 0) {
-      const char* e = getenv("LB_SPLIT_FORCE");
-      force = e ? atoi(e) : 0;
-    }
-    if (force > 1) {
-      const long long tiles = static_cast<long long>(m_tiles) * ((N + force_bn - 1) / force_bn);
-      int sp = force < num_kb ? force : num_kb;
-      while (sp > 1 && tiles * sp > n_sms) --sp;
-      return sp > 1 ? SplitPlan{force_bn, sp} : SplitPlan{0, 1};
-    }
-  }
   SplitPlan best = {0, 1};
   double best_t = 1e30, base_t = 1e30;
   {
@@ -154,13 +139,12 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
                                   long long up_cs, const float* diag, float scale, void* Y,
                                   float* T_out, const float* T_in, int M, int K, int N, int r,
                                   int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                                  void* stream, int mask_input = 0) {
+                                  void* stream) {
   using namespace lb;
   const int w_tiled = (in_dtype & LB_W_TILED) ? 1 : 0;
   in_dtype &= ~LB_W_TILED;
   if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && (seed_dev == nullptr || T_in != nullptr)))
     return LB_ERR_SHAPE;
-  if (mask_input && !(drop_p > 0.f)) return LB_ERR_SHAPE;
   if (M <= 0 || N <= 0 || K <= 0) return LB_ERR_SHAPE;
   if (r < 1 || r > R_PAD) return LB_ERR_RANK;
   if (in_dtype != LB_BF16 && in_dtype != LB_F16) return LB_ERR_DTYPE;
@@ -180,23 +164,6 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
   p.drop_p = drop_p; p.drop_inv = 1.f / (1.f - drop_p);
   p.seed = reinterpret_cast<const unsigned long long*>(seed_dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (mask_input) {
-    // Dropout BACKWARD (dX): X = gY, and the T path must see mask o gY -- the consumer warps write a
-    // masked copy of every A tile for the T MMA (fused_core.cuh, BMASK); mask index = row * K + k.
-    const SplitPlan spm = plan_split(M, K, N, sm_count());
-    if (spm.split > 1) {
-      if (out_dtype == LB_F32)
-        return launch_linear<64, 4, float, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split);
-      return launch_linear<64, 4, uint16_t, 1, false, true, true>(X, W, down16, Y, p, out_dtype, st, spm.split);
-    }
-    const long long t128 = static_cast<long long>((M + 127) / 128) * ((N + 127) / 128);
-    const bool nar = t128 < 90 && !(K >= 2048 && t128 >= 64);
-    if (out_dtype == LB_F32)
-      return nar ? launch_linear<64, 4, float, 1, false, false, true>(X, W, down16, Y, p, out_dtype, st)
-                 : launch_linear<128, 3, float, 1, false, false, true>(X, W, down16, Y, p, out_dtype, st);
-    return nar ? launch_linear<64, 4, uint16_t, 1, false, false, true>(X, W, down16, Y, p, out_dtype, st)
-               : launch_linear<128, 3, uint16_t, 1, false, false, true>(X, W, down16, Y, p, out_dtype, st);
-  }
   if (drop_p > 0.f) {
     // Dropout on the branch: the LoRA product keeps its own accumulator and is masked in the
     // drain (fused_core.cuh, DROP). One tile per CTA; BLOCK_N 64 (2 CTAs/SM) unless the site has
@@ -234,8 +201,8 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
     // 16x16 / 8x8 levels, the 77-token k/v sites, CLIP. Two CTAs of a cluster halve the K loop and
     // merge through distributed shared memory (one bulk copy, no global round trip).
     if (K >= 640 && tiles64 * 2 <= n_sms) {
-      if (out_dtype == LB_F32) return launch_linear<64, 4, float, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
-      return launch_linear<64, 6, uint16_t, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      if (out_dtype == LB_F32) return launch_linear<64, 4, float, 1, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      return launch_linear<64, 6, uint16_t, 1, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
     }
     // One balanced wave of 192-wide tiles instead of 1.1 waves of 128-wide ones (256x1280->10240:
     // 160 tiles of 128, 80 of 192)
@@ -258,14 +225,14 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
     if (bn_choice == 2 && split > 2) split = 2;        // 128-wide partials: one peer slot fits
     if (split >= 2) {
       if (out_dtype == LB_F32) {
-        if (split == 2) return launch_linear<64, 4, float, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
-        if (split == 3) return launch_linear<64, 3, float, 1, false, false, false, 3>(X, W, down16, Y, p, out_dtype, st);
-        return launch_linear<64, 2, float, 1, false, false, false, 4>(X, W, down16, Y, p, out_dtype, st);
+        if (split == 2) return launch_linear<64, 4, float, 1, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+        if (split == 3) return launch_linear<64, 3, float, 1, false, false, 3>(X, W, down16, Y, p, out_dtype, st);
+        return launch_linear<64, 2, float, 1, false, false, 4>(X, W, down16, Y, p, out_dtype, st);
       }
-      if (bn_choice == 2) return launch_linear<128, 3, uint16_t, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
-      if (split == 2) return launch_linear<64, 6, uint16_t, 1, false, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
-      if (split == 3) return launch_linear<64, 4, uint16_t, 1, false, false, false, 3>(X, W, down16, Y, p, out_dtype, st);
-      return launch_linear<64, 2, uint16_t, 1, false, false, false, 4>(X, W, down16, Y, p, out_dtype, st);
+      if (bn_choice == 2) return launch_linear<128, 3, uint16_t, 1, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      if (split == 2) return launch_linear<64, 6, uint16_t, 1, false, false, 2>(X, W, down16, Y, p, out_dtype, st);
+      if (split == 3) return launch_linear<64, 4, uint16_t, 1, false, false, 3>(X, W, down16, Y, p, out_dtype, st);
+      return launch_linear<64, 2, uint16_t, 1, false, false, 4>(X, W, down16, Y, p, out_dtype, st);
     }
   }
   if (bn_choice == 3 && out_dtype != LB_F32)
@@ -284,7 +251,7 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
   if (narrow)
     return crowded ? launch_linear<64, 2, uint16_t, 2>(X, W, down16, Y, p, out_dtype, st)
                    : launch_linear<64, 7, uint16_t, 1>(X, W, down16, Y, p, out_dtype, st);
-  return crowded ? launch_linear<128, 2, uint16_t, 2, false, false, false, 1, true>(X, W, down16, Y, p, out_dtype, st)
+  return crowded ? launch_linear<128, 2, uint16_t, 2, false, false, 1, true>(X, W, down16, Y, p, out_dtype, st)
                  : launch_linear<128, 4, uint16_t, 1>(X, W, down16, Y, p, out_dtype, st);
 }
 
@@ -305,15 +272,6 @@ extern "C" int lb_lora_linear_fwd_dropout(const void* X, const void* W, const fl
                                           int out_dtype, float drop_p, const void* seed_dev, void* stream) {
   return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, nullptr, M, K, N, r,
                          in_dtype, out_dtype, drop_p, seed_dev, stream);
-}
-
-extern "C" int lb_lora_linear_dx_dropout(const void* gY, const void* Wt, const void* upT16, const float* down,
-                                         long long down_rs, long long down_cs, const float* diag, float scale,
-                                         void* dX, float* T_out, int M, int N_out, int K_in, int r,
-                                         int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                                         void* stream) {
-  return linear_fwd_impl(gY, Wt, nullptr, upT16, down, down_rs, down_cs, diag, scale, dX, T_out, nullptr, M, N_out,
-                         K_in, r, in_dtype, out_dtype, drop_p, seed_dev, stream, 1);
 }
 
 extern "C" int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W,

@@ -871,7 +871,7 @@ ti_step_kernel(float* __restrict__ rows, float* __restrict__ grad, float* __rest
 // =============================================================================== C ABI
 using namespace lb;
 
-extern "C" int lb_abi_version(void) { return 3; }
+extern "C" int lb_abi_version(void) { return 4; }
 
 extern "C" int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float scale,
                                    float* out, long long out_js, long long out_cs, int M, int C,

@@ -8,28 +8,20 @@ The mask sits between the up-projection and the sum, so the branch cannot be acc
 base accumulator -- but it still never leaves the SM: the fused kernel gives the LoRA product
 T'.U^T its own accumulator and applies keep(m,n)/(1-p) while the tile is drained
 (lb_lora_linear_fwd_dropout / lb_lora_conv2d_fwd_dropout; csrc/fused_core.cuh, DROP): ONE launch,
-no extra pass over Y. Backward recomputes the same counter-based mask INSIDE the dX kernel
-(lb_lora_linear_dx_dropout / lb_lora_conv2d_dx_dropout: the consumer warpgroups, inside the MMA loop,
-write a masked copy of each gY tile that feeds only the rank-r MMA -- dT = (mask o gY) . B without a
-separate pass over gY); dB uses the masked reduction (lb_lora_wgrad_masked).
+no extra pass over Y. Backward recomputes the same counter-based mask: one masked pass over gY gives
+dTs = (mask o gY / (1-p)) . B (lb_lora_dropout_dt), and the plain dX kernel takes its rank-r
+activations from dTs (T_in) instead of computing gY . B; dA reduces X against dTs, and dB uses the
+masked reduction (lb_lora_wgrad_masked).
 
 The keep-mask is a hash of (per-call device seed, element index; csrc/dropmask.cuh) -- NOT ATen's Philox stream, so
 parity with the reference under dropout is distributional (keep probability, 1/(1-p) scaling,
 forward/backward mask consistency; tests/test_dropout_gpu.py), not bitwise.
 """
-import os
-
 import torch
 
 from . import ops
 from ._C import LoraB200Error
 from .modules import _LOW, _SiteState, _compute_dtype, _fp32_master, _out_dtype
-
-# Backward formulation. "twopass" (default): lb_lora_dropout_dt (one masked pass over gY) + the plain dX
-# kernel with T_in. "fused": the mask applied inside the dX kernel (lb_lora_*_dx_dropout, one launch, no
-# extra pass). Same results (tests/test_dropout_gpu.py runs both); the fused form hashes 8192 mask
-# decisions per K block inside the MMA loop, where the separate streaming pass costs one read of gY.
-_TWO_PASS = os.environ.get("LB_DROPOUT_BWD", "twopass") != "fused"
 
 
 class _SeedPool:
@@ -104,16 +96,10 @@ class _LoraLinearDropoutFn(torch.autograd.Function):
         upT16 = st.upT16(B, cdt)
         A32, B32 = _fp32_master(A), _fp32_master(B)
         dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
-        # one launch: the mask is applied to a shared-memory copy of each gY tile that feeds only the
-        # rank-r MMA; dTs = (mask o gY) . B WITHOUT the 1/(1-p) factor (folded into the scales below)
-        if _TWO_PASS:      # round-2a formulation, kept for same-box A/B timing: a masked pass over gY, then T_in
-            dTs = ops.dropout_dt(gy2d, B32, r, 1, ctx.p, seed, r)          # (mask o gY / (1-p)) . B
-            dX, _ = ops.fused_linear(gy2d, wt16, None, upT16, A32, 1, K, ctx.diag, ctx.scale, r,
-                                     dx_dtype, False, t_in=dTs)
-            inv = 1.0
-        else:
-            dX, dTs = ops.fused_linear_dx_dropout(gy2d, wt16, upT16, A32, ctx.diag, ctx.scale, r, dx_dtype, ctx.p, seed)
-            inv = 1.0 / (1.0 - ctx.p)
+        # a masked pass over gY, then the dX kernel takes the rank-r activations from it (T_in)
+        dTs = ops.dropout_dt(gy2d, B32, r, 1, ctx.p, seed, r)          # (mask o gY / (1-p)) . B
+        dX, _ = ops.fused_linear(gy2d, wt16, None, upT16, A32, 1, K, ctx.diag, ctx.scale, r,
+                                 dx_dtype, False, t_in=dTs)
         need_x, need_a, need_b = ctx.needs_input_grad[:3]
         sink = st.grad_sink
         dA = dB = None
@@ -123,9 +109,9 @@ class _LoraLinearDropoutFn(torch.autograd.Function):
         if need_b:
             tB = sink[1] if sink is not None else torch.zeros((N, r), device=gy.device, dtype=torch.float32)
         if need_a:
-            ops.wgrad(x2d, dTs, ctx.diag, ctx.scale * inv, tA, K, 1, r, async_ok=sink is not None)
+            ops.wgrad(x2d, dTs, ctx.diag, ctx.scale, tA, K, 1, r, deferrable=sink is not None)
         if need_b:
-            ops.wgrad_masked(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, ctx.p, seed, async_ok=sink is not None)
+            ops.wgrad_masked(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, ctx.p, seed, deferrable=sink is not None)
         if sink is None:
             dA = tA.to(A.dtype).view_as(A) if need_a else None
             dB = tB.to(B.dtype).view_as(B) if need_b else None
@@ -183,27 +169,21 @@ class _LoraConv2dDropoutFn(torch.autograd.Function):
         upT16 = _upT16(st, B, cdt)
         A32, B32 = _fp32_master(A), _fp32_master(B)
         dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
-        if _TWO_PASS:
-            dTs = ops.dropout_dt(gy2d, B32, r, 1, ctx.p, seed, r)
-            dX, _ = ops.fused_conv2d(gy16, w_b, None, upT16, A32, taps - 1, taps, cin * taps, -1,
-                                     ctx.diag, ctx.scale, r, cin, kh, kw, kh - 1 - ph, kw - 1 - pw,
-                                     True, dx_dtype, False, t_in=dTs)
-            inv = 1.0
-        else:
-            dX, dTs = ops.fused_conv2d_dx_dropout(gy16, w_b, upT16, A32, ctx.diag, ctx.scale, r, cin, kh, kw, ph, pw,
-                                                  dx_dtype, ctx.p, seed)
-            inv = 1.0 / (1.0 - ctx.p)
+        dTs = ops.dropout_dt(gy2d, B32, r, 1, ctx.p, seed, r)
+        dX, _ = ops.fused_conv2d(gy16, w_b, None, upT16, A32, taps - 1, taps, cin * taps, -1,
+                                 ctx.diag, ctx.scale, r, cin, kh, kw, kh - 1 - ph, kw - 1 - pw,
+                                 True, dx_dtype, False, t_in=dTs)
         need_x, need_a, need_b = ctx.needs_input_grad[:3]
         sink = st.grad_sink
         dA = dB = None
         if need_a:
             tgt = sink[0] if sink is not None else torch.zeros((r, cin * taps), device=gy.device, dtype=torch.float32)
-            ops.wgrad_conv(x16, dTs, ctx.diag, ctx.scale * inv, tgt, r, cin, h, w, kh, kw, ph, pw, async_ok=sink is not None)
+            ops.wgrad_conv(x16, dTs, ctx.diag, ctx.scale, tgt, r, cin, h, w, kh, kw, ph, pw, deferrable=sink is not None)
             if sink is None:
                 dA = tgt.view_as(A).to(A.dtype)
         if need_b:
             tgt = sink[1] if sink is not None else torch.zeros((cout, r), device=gy.device, dtype=torch.float32)
-            ops.wgrad_masked(gy2d, T, ctx.diag, ctx.scale, tgt, 1, r, r, ctx.p, seed, async_ok=sink is not None)
+            ops.wgrad_masked(gy2d, T, ctx.diag, ctx.scale, tgt, 1, r, r, ctx.p, seed, deferrable=sink is not None)
             if sink is None:
                 dB = tgt.view_as(B).to(B.dtype)
         dx = dX.to(ctx.x_dtype) if need_x else None

@@ -164,12 +164,12 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
                 if need_a and need_b:
                     multi.append((dTs[j], tA, g2ds[i], Ts[i], tB, diag, scale, r))
                 elif need_a:
-                    ops.wgrad(x2d, dTs[j], diag, scale, tA, K, 1, r, async_ok=sink is not None)
+                    ops.wgrad(x2d, dTs[j], diag, scale, tA, K, 1, r, deferrable=sink is not None)
                 elif need_b:
-                    ops.wgrad(g2ds[i], Ts[i], diag, scale, tB, 1, r, r, async_ok=sink is not None)
+                    ops.wgrad(g2ds[i], Ts[i], diag, scale, tB, 1, r, r, deferrable=sink is not None)
                 temps.append((i, sink, tA, tB, A, B, need_a, need_b))
             if multi:
-                ops.wgrad_multi(x2d, multi, async_ok=all_sink)   # every dA/dB of the family: one launch
+                ops.wgrad_multi(x2d, multi, deferrable=all_sink)   # every dA/dB of the family: one launch
             for (i, sink, tA, tB, A, B, need_a, need_b) in temps:
                 if sink is None:
                     grads[2 * i] = tA.to(A.dtype).view_as(A) if need_a else None

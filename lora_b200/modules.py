@@ -271,13 +271,13 @@ class _FusedLoraLinearFn(torch.autograd.Function):
             tA = sink[0] if sink is not None else torch.zeros((r, K), device=gy.device, dtype=torch.float32)
         if need_b:
             tB = sink[1] if sink is not None else torch.zeros((N, r), device=gy.device, dtype=torch.float32)
-        side = sink is not None      # straight into the arena: nothing downstream waits for it
+        deferrable = sink is not None      # straight into the arena: nothing downstream waits for it
         if need_a and need_b:
-            ops.wgrad_pair(x2d, dTs, tA, gy2d, T, tB, ctx.diag, ctx.scale, r, async_ok=side)
+            ops.wgrad_pair(x2d, dTs, tA, gy2d, T, tB, ctx.diag, ctx.scale, r, deferrable=deferrable)
         elif need_a:
-            ops.wgrad(x2d, dTs, ctx.diag, ctx.scale, tA, K, 1, r, async_ok=side)
+            ops.wgrad(x2d, dTs, ctx.diag, ctx.scale, tA, K, 1, r, deferrable=deferrable)
         elif need_b:
-            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, async_ok=side)
+            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, deferrable=deferrable)
         if sink is None:
             dA = tA.to(A.dtype).view_as(A) if need_a else None
             dB = tB.to(B.dtype).view_as(B) if need_b else None

@@ -21,18 +21,6 @@ def _count(n: int = 1):
     LAUNCH_COUNT += n
 
 
-# Optional side stream for the factor-gradient reductions: dA/dB are consumed only by the optimizer
-# at the very end of the step, so (when they accumulate straight into the arena) they can run
-# concurrently with the rest of the backward pass, which under-fills the GPU at bs = 1. The trainer
-# sets the stream, and joins it before the all-reduce / optimizer.
-_SIDE = None
-
-
-def set_side_stream(stream):
-    global _SIDE
-    _SIDE = stream
-
-
 # Deferred factor gradients: dA / dB feed only the optimizer, so (when they accumulate straight into
 # an arena) a step engine can QUEUE every linear-site reduction of the backward pass and run them
 # all in ceil(n/24) launches at its end (lb_lora_wgrad_batch) instead of one small launch per site.
@@ -50,37 +38,22 @@ class _WgProblemC(_ct.Structure):
 
 
 _WG_QUEUE = None      # None: launch immediately; dict dtype -> [(_WgProblemC fields, keepalive)]
-_WG_SIDE = None       # deferral with overlap: full batches of 24 leave on this stream as soon as they fill
 WG_BATCH = 24
 
 
-def wgrad_defer_begin(side_stream=None):
-    """side_stream: launch every full batch of 24 queued reductions on it right away (after everything
-    enqueued so far on the current stream), so the batches overlap the rest of the backward pass instead
-    of trailing it; the caller joins the stream after wgrad_flush()."""
-    global _WG_QUEUE, _WG_SIDE
+def wgrad_defer_begin():
+    global _WG_QUEUE
     _WG_QUEUE = {}
-    _WG_SIDE = side_stream
 
 
 def wgrad_defer_cancel():
-    global _WG_QUEUE, _WG_SIDE
+    global _WG_QUEUE
     _WG_QUEUE = None
-    _WG_SIDE = None
 
 
-def _wgrad_launch(dtype, items, side):
+def _wgrad_launch(dtype, items):
     arr = (_WgProblemC * len(items))(*[_WgProblemC(*it[0]) for it in items])
-    if side is None:
-        check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
-    else:
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
-        for it in items:                   # the operands must outlive the side-stream launch
-            for t in it[1]:
-                if t is not None:
-                    t.record_stream(side)
+    check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
     n = (len(items) + WG_BATCH - 1) // WG_BATCH
     _count(n)
     return n
@@ -90,38 +63,20 @@ def _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag, drop_p=0.0, 
     dp = lambda t: None if t is None else t.data_ptr()
     item = (dp(S), dp(V), dp(out), int(out_js), int(out_cs), int(M), int(C), int(r), float(scale), dp(diag),
             float(drop_p), dp(seed)) + (tuple(int(v) for v in conv) if conv is not None else (0, 0, 0, 0, 0, 0))
-    lst = _WG_QUEUE.setdefault(S.dtype, [])
-    lst.append((item, (S, V, out, diag, seed)))
-    if _WG_SIDE is not None and len(lst) >= WG_BATCH:
-        _wgrad_launch(S.dtype, lst[:WG_BATCH], _WG_SIDE)
-        del lst[:WG_BATCH]
+    _WG_QUEUE.setdefault(S.dtype, []).append((item, (S, V, out, diag, seed)))
 
 
 def wgrad_flush():
     """Run every queued reduction (lb_lora_wgrad_batch) and leave deferral mode."""
-    global _WG_QUEUE, _WG_SIDE
+    global _WG_QUEUE
     q, _WG_QUEUE = _WG_QUEUE, None
-    side, _WG_SIDE = _WG_SIDE, None
     if not q:
         return 0
     n_launch = 0
     for dtype, items in q.items():
         if items:
-            n_launch += _wgrad_launch(dtype, items, side)
+            n_launch += _wgrad_launch(dtype, items)
     return n_launch
-
-
-def _maybe_side(async_ok: bool, tensors, fn):
-    if _SIDE is None or not async_ok:
-        fn()
-        return
-    cur = torch.cuda.current_stream()
-    _SIDE.wait_stream(cur)                 # everything enqueued so far (incl. the dX kernel) comes first
-    with torch.cuda.stream(_SIDE):
-        fn()
-    for t in tensors:                      # keep the inputs' memory away from the allocator until done
-        if t is not None:
-            t.record_stream(_SIDE)
 
 
 def _req_cuda(*ts):
@@ -238,18 +193,17 @@ def fused_linear(x2d: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tens
 
 
 def wgrad(S: torch.Tensor, V: torch.Tensor, diag: Optional[torch.Tensor], scale: float,
-          out: torch.Tensor, out_js: int, out_cs: int, r: int, async_ok: bool = False):
+          out: torch.Tensor, out_js: int, out_cs: int, r: int, deferrable: bool = False):
     """out[j*out_js + c*out_cs] += scale*diag[j] * sum_m V[m,j]*S[m,c]."""
     _req_cuda(S, V, out)
     M, C = S.shape
     assert S.is_contiguous() and V.shape == (M, R_PAD) and V.dtype == torch.float32
     assert out.dtype == torch.float32
-    if _WG_QUEUE is not None and async_ok:
+    if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag)
         return
-    _maybe_side(async_ok, (S, V, diag), lambda: check(
-        _C.lib.lb_lora_wgrad(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
-                             M, C, r, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad"))
+    check(_C.lib.lb_lora_wgrad(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
+                               M, C, r, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad")
     _count()
 
 
@@ -342,44 +296,6 @@ def wgrad_shift(S_rows: torch.Tensor, V: torch.Tensor, diag, scale: float, out: 
 
 
 # ------------------------------------------------------------------------------------ dropout
-def fused_linear_dx_dropout(gy2d: torch.Tensor, wt16: torch.Tensor, upT16: torch.Tensor, A32: torch.Tensor,
-                            diag, scale: float, r: int, out_dtype, p: float, seed: torch.Tensor):
-    """dX = gY.W + (((mask o gY).B) * scale*diag/(1-p)) . A  and  dTm = (mask o gY).B  (one launch)."""
-    _req_cuda(gy2d, upT16, A32, seed)
-    M, N_out = gy2d.shape
-    wp, K_in, wflag = _w_arg(wt16, N_out)
-    assert upT16.shape == (R_PAD, N_out) and gy2d.is_contiguous()
-    dX = torch.empty((M, K_in), device=gy2d.device, dtype=out_dtype)
-    dTm = torch.empty((M, R_PAD), device=gy2d.device, dtype=torch.float32)
-    check(_C.lib.lb_lora_linear_dx_dropout(ptr(gy2d), wp, ptr(upT16), ptr(A32), 1, K_in, ptr(diag),
-                                           float(scale), ptr(dX), ptr(dTm), M, N_out, K_in, r,
-                                           dtype_code(gy2d.dtype) | wflag, dtype_code(out_dtype), float(p), ptr(seed),
-                                           stream_ptr()), "lb_lora_linear_dx_dropout")
-    _count()
-    return dX, dTm
-
-
-def fused_conv2d_dx_dropout(gy_nhwc: torch.Tensor, w_b: torch.Tensor, upT16: torch.Tensor, A32: torch.Tensor,
-                            diag, scale: float, r: int, cin: int, kh: int, kw: int, ph: int, pw: int, out_dtype,
-                            p: float, seed: torch.Tensor):
-    """Conv analogue: dX (channels_last [N,cin,H,W]) and dTm [pixels,16] = (mask o gY).B, one launch."""
-    _req_cuda(gy_nhwc, w_b, upT16, A32, seed)
-    n, cout, h, w = gy_nhwc.shape
-    taps = kh * kw
-    assert gy_nhwc.is_contiguous(memory_format=torch.channels_last)
-    dX = torch.empty((n, cin, h, w), device=gy_nhwc.device, dtype=out_dtype, memory_format=torch.channels_last)
-    dTm = torch.empty((n * h * w, R_PAD), device=gy_nhwc.device, dtype=torch.float32)
-    import ctypes
-    down_ptr = ctypes.c_void_p(A32.data_ptr() + 4 * (taps - 1))       # A read flipped: last tap first
-    check(_C.lib.lb_lora_conv2d_dx_dropout(ptr(gy_nhwc), ptr(w_b), ptr(upT16), down_ptr, taps, cin * taps, -1,
-                                           ptr(diag), float(scale), ptr(dX), ptr(dTm), n, h, w, cout, cin, kh, kw,
-                                           kh - 1 - ph, kw - 1 - pw, r, dtype_code(gy_nhwc.dtype),
-                                           dtype_code(out_dtype), float(p), ptr(seed), stream_ptr()),
-          "lb_lora_conv2d_dx_dropout")
-    _count()
-    return dX, dTm
-
-
 def up_dropout_(y2d: torch.Tensor, T: torch.Tensor, up: torch.Tensor, up_rs: int, up_cs: int,
                 diag, scale: float, p: float, seed: torch.Tensor, r: int):
     """y2d[m,n] += scale/(1-p) * keep(m,n) * sum_j T[m,j] diag[j] up[n,j]   (in place)."""
@@ -406,10 +322,10 @@ def dropout_dt(gy2d: torch.Tensor, up: torch.Tensor, up_rs: int, up_cs: int, p: 
 
 
 def wgrad_masked(S: torch.Tensor, V: torch.Tensor, diag, scale: float, out: torch.Tensor,
-                 out_js: int, out_cs: int, r: int, p: float, seed: torch.Tensor, async_ok: bool = False):
+                 out_js: int, out_cs: int, r: int, p: float, seed: torch.Tensor, deferrable: bool = False):
     _req_cuda(S, V, out, seed)
     M, C = S.shape
-    if _WG_QUEUE is not None and async_ok:
+    if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag, p, seed)
         return
     check(_C.lib.lb_lora_wgrad_masked(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
@@ -420,20 +336,19 @@ def wgrad_masked(S: torch.Tensor, V: torch.Tensor, diag, scale: float, out: torc
 
 def wgrad_pair(x2d: torch.Tensor, dTs: torch.Tensor, dA: torch.Tensor, gy2d: torch.Tensor,
                T: torch.Tensor, dB: torch.Tensor, diag, scale: float, r: int, p: float = 0.0,
-               seed: Optional[torch.Tensor] = None, async_ok: bool = False):
+               seed: Optional[torch.Tensor] = None, deferrable: bool = False):
     """dA [r,K] += s*d * dTs^T x2d  and  dB [N,r] += s*d * (mask o gy2d)^T T  in one launch."""
     _req_cuda(x2d, dTs, dA, gy2d, T, dB)
     M, K = x2d.shape
     N = gy2d.shape[1]
     assert gy2d.shape[0] == M and dA.dtype == torch.float32 and dB.dtype == torch.float32
-    if _WG_QUEUE is not None and async_ok:
+    if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(x2d, dTs, dA, K, 1, M, K, r, scale, diag)
         _wgrad_enqueue(gy2d, T, dB, 1, r, M, N, r, scale, diag, p, seed)
         return
-    _maybe_side(async_ok, (x2d, dTs, gy2d, T, diag, seed), lambda: check(
-        _C.lib.lb_lora_wgrad_pair(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
-                                  1, r, N, ptr(diag), float(scale), M, r, float(p), ptr(seed),
-                                  dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair"))
+    check(_C.lib.lb_lora_wgrad_pair(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
+                                    1, r, N, ptr(diag), float(scale), M, r, float(p), ptr(seed),
+                                    dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair")
     _count()
 
 
@@ -492,14 +407,14 @@ def fused_linear_grouped(problems, out_dtype, want_t: bool):
     return ys, ts
 
 
-def wgrad_multi(x2d: torch.Tensor, items, async_ok: bool = False):
+def wgrad_multi(x2d: torch.Tensor, items, deferrable: bool = False):
     """items: list (<= 4) of (dTs, dA [r,K] fp32, gy2d [M,N], T, dB [N,r] fp32, diag|None, scale, r):
     all dA/dB of a family that shares x2d in one launch."""
     import ctypes
     n = len(items)
     VP, I, F = ctypes.c_void_p, ctypes.c_int, ctypes.c_float
     M, K = x2d.shape
-    if _WG_QUEUE is not None and async_ok:
+    if _WG_QUEUE is not None and deferrable:
         for (dTs, dA, gy2d, T, dB, diag, scale, r) in items:
             _wgrad_enqueue(x2d, dTs, dA, K, 1, M, K, r, scale, diag)
             _wgrad_enqueue(gy2d, T, dB, 1, r, M, gy2d.shape[1], r, scale, diag)
@@ -511,19 +426,17 @@ def wgrad_multi(x2d: torch.Tensor, items, async_ok: bool = False):
          arr(VP, [it[4].data_ptr() for it in items]), arr(I, [it[2].shape[1] for it in items]),
          arr(VP, [dp(it[5]) for it in items]), arr(F, [float(it[6]) for it in items]),
          arr(I, [it[7] for it in items]))
-    used = [x2d] + [t for it in items for t in (it[0], it[2], it[3], it[5])]
-    _maybe_side(async_ok, used, lambda: check(
-        _C.lib.lb_lora_wgrad_multi(n, ptr(x2d), a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], a[8], M, K,
-                                   dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_multi"))
+    check(_C.lib.lb_lora_wgrad_multi(n, ptr(x2d), a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], a[8], M, K,
+                                     dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_multi")
     _count()
 
 
 def wgrad_conv(x_nhwc_rows: torch.Tensor, V: torch.Tensor, diag, scale: float, out: torch.Tensor, r: int,
-               C: int, H: int, W: int, kh: int, kw: int, pad_h: int, pad_w: int, async_ok: bool = False):
+               C: int, H: int, W: int, kh: int, kw: int, pad_h: int, pad_w: int, deferrable: bool = False):
     """dA [r, C*kh*kw] (flat [r,Cin,kh,kw]) += all taps, one launch (see lb_lora_wgrad_conv)."""
     _req_cuda(x_nhwc_rows, V, out)
     M = V.shape[0]
-    if _WG_QUEUE is not None and async_ok:
+    if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(x_nhwc_rows, V, out, C * kh * kw, kh * kw, M, C, r, scale, diag,
                        conv=(H, W, kh, kw, pad_h, pad_w))
         return

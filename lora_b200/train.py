@@ -36,10 +36,6 @@ class StepConfig:
     compute_dtype: torch.dtype = torch.bfloat16
     use_cuda_graph: bool = True
     graph_warmup: int = 3
-    # run the dA/dB reductions on a side stream, concurrently with the rest of the backward pass
-    # (they feed only the optimizer); joined before the all-reduce. Measured neutral on C2
-    # (59.9 vs 60.2 images/s): off by default.
-    async_wgrad: bool = False
     # EXPERIMENTAL (not yet run on hardware): capture the NCCL all-reduce INSIDE one step graph,
     # with capture_error_mode="thread_local" so that the NCCL watchdog thread's event queries do
     # not collide with the capture (the suspected cause of the round-1 dead-lock with a globally
@@ -143,8 +139,6 @@ class LoraTrainStep:
                 self.arena._dp = None
         self.unet.train()
         self.text_encoder.train()
-        self._side = torch.cuda.Stream(device=self.device) if cfg.async_wgrad else None
-        self._wg_side = None       # LB_WGRAD_OVERLAP=1: stream of the overlapped dA/dB batches (created on first use)
 
     # ------------------------------------------------------------------ the step body
     def _fwd_bwd(self):
@@ -212,26 +206,15 @@ class LoraTrainStep:
             else:
                 loss = F.mse_loss(pred.float(), target.float(), reduction="mean")
         from . import ops
-        ops.set_side_stream(self._side)
-        import os as _os
-        defer = (cfg.defer_wgrad and self._side is None and lat.is_cuda and hasattr(self, "arena")
-                 and _os.environ.get("LB_NO_DEFER", "0") != "1")
-        overlap = defer and _os.environ.get("LB_WGRAD_OVERLAP", "0") == "1"
-        if overlap and getattr(self, "_wg_side", None) is None:
-            self._wg_side = torch.cuda.Stream(device=self.device)
+        defer = cfg.defer_wgrad and lat.is_cuda and hasattr(self, "arena")
         if defer:
-            ops.wgrad_defer_begin(self._wg_side if overlap else None)
+            ops.wgrad_defer_begin()
         try:
             loss.backward()
             if defer:
                 ops.wgrad_flush()
         finally:
-            ops.set_side_stream(None)
             ops.wgrad_defer_cancel()
-        if overlap:
-            torch.cuda.current_stream().wait_stream(self._wg_side)   # join: every batch has landed in arena.g
-        if self._side is not None:
-            torch.cuda.current_stream().wait_stream(self._side)   # join: all dA/dB are in arena.g
         dropout_path.end_step()
         self.loss.copy_(loss.detach())
 
@@ -413,8 +396,6 @@ class TextualInversionStep(LoraTrainStep):
         if cfg.train_inpainting:
             self.inpaint_mask = torch.zeros((latent_shape[0], 1, latent_shape[2], latent_shape[3]), device=self.device)
             self.masked_latents = torch.zeros(latent_shape, device=self.device, dtype=torch.float32)
-        self._side = None
-        self._wg_side = None
         self._world = 1
         self.global_step = 0
         self.graph = self.graph_update = None

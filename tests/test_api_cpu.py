@@ -329,7 +329,7 @@ def test_train_step_forward_backward_body_on_cpu_doubles(inpaint, masked, prior)
     tr.cfg = StepConfig(use_cuda_graph=False, t_multiplier=0.8, use_mask=masked, mask_temperature=2.0,
                         train_inpainting=inpaint, with_prior_preservation=prior, prior_loss_weight=0.7)
     tr.unet, tr.text_encoder, tr.device = unet, text, torch.device("cpu")
-    tr.noiser, tr.model_dtype, tr._side = DDPMNoiser(device="cpu"), torch.float32, None
+    tr.noiser, tr.model_dtype = DDPMNoiser(device="cpu"), torch.float32
     tr.latents = torch.randn(shape, generator=g) * 0.18215
     tr.input_ids = torch.randint(0, 1000, (2, 77), generator=g)
     tr.loss = torch.zeros(())

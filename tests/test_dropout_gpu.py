@@ -28,10 +28,7 @@ def _mod(K=320, N=640, r=4, p=0.25, bias=True):
     return m
 
 
-@pytest.mark.parametrize("two_pass", [True, False])
-def test_mask_recovered_from_forward_is_consistent_with_backward(two_pass, monkeypatch):
-    import lora_b200.dropout_path as dp
-    monkeypatch.setattr(dp, "_TWO_PASS", two_pass)     # lb_lora_dropout_dt + T_in  |  mask inside the dX kernel
+def test_mask_recovered_from_forward_is_consistent_with_backward():
     """Recover the realised mask from y (branch/clean-branch ratio), then check dX, dA, dB equal
     the oracle's backward evaluated WITH THAT MASK."""
     p = 0.25
@@ -120,10 +117,7 @@ def test_conv_dropout_statistics_and_grads_finite():
         assert g is not None and torch.isfinite(g).all() and float(g.abs().sum()) > 0
 
 
-@pytest.mark.parametrize("two_pass", [True, False])
-def test_conv_dropout_backward_matches_oracle_with_recovered_mask(two_pass, monkeypatch):
-    import lora_b200.dropout_path as dp
-    monkeypatch.setattr(dp, "_TWO_PASS", two_pass)
+def test_conv_dropout_backward_matches_oracle_with_recovered_mask():
     """Conv site with active dropout: recover the realised keep-mask from the forward output
     (branch / clean-branch ratio, as for the linear site above), then dX, dA, dB must equal the
     oracle's backward (oracle/lora_ops.py::lora_conv2d_backward, autograd of lora.py:130-135)

@@ -272,43 +272,6 @@ def test_training_step_cuda_graph_equals_eager():
     assert rel(finals[1], finals[0]) < 1e-4
 
 
-def test_overlapped_wgrad_batches_match_default(monkeypatch):
-    """LB_WGRAD_OVERLAP=1: full batches of 24 queued dA/dB reductions leave on a side stream during the
-    backward pass (graph branch) instead of trailing it -- same losses and factors as the default flush."""
-    import lora_b200 as L
-    from lora_b200.train import LoraTrainStep, StepConfig
-    losses, finals, launches = [], [], []
-    for overlap in ("0", "1"):
-        monkeypatch.setenv("LB_WGRAD_OVERLAP", overlap)
-        unet, text = _tiny_models(seed=5)
-        unet, text = unet.to(torch.bfloat16), text.to(torch.bfloat16)
-        L.inject_trainable_lora(unet, r=4)
-        L.inject_trainable_lora(text, target_replace_module={"CLIPAttention"}, r=4)
-        g = torch.Generator(device=DEV).manual_seed(3)
-        for m in list(unet.modules()) + list(text.modules()):
-            if type(m).__name__ == "LoraInjectedLinear":
-                m.lora_up.weight.data.normal_(0, 0.05, generator=g)
-        cfg = StepConfig(use_cuda_graph=True, graph_warmup=2, external_noise=True)
-        tr = LoraTrainStep(unet, text, cfg, latent_shape=(1, 4, 16, 16), device=DEV)
-        torch.manual_seed(9)
-        tr.latents.copy_(torch.randn(1, 4, 16, 16, device=DEV) * 0.18215)
-        tr.input_ids.copy_(torch.randint(0, 1000, (1, 77), device=DEV))
-        tr.prepare()
-        assert tr.graph is not None, tr.graph_error
-        out = []
-        for i in range(4):
-            gen = torch.Generator(device=DEV).manual_seed(50 + i)
-            tr.noise.copy_(torch.randn(1, 4, 16, 16, device=DEV, generator=gen))
-            tr.timesteps.copy_(torch.randint(0, 1000, (1,), device=DEV, generator=gen))
-            out.append(float(tr.step_device()))
-        torch.cuda.synchronize()
-        losses.append(out)
-        finals.append(tr.arena.p.clone())
-    for a, b in zip(*losses):
-        assert a == a and a > 0 and abs(a - b) < 2e-3 * abs(a), losses
-    assert rel(finals[1], finals[0]) < 1e-4
-
-
 def test_extended_training_step_matches_reference_step_tiny():
     """--use_extended_lora shape of the step (Linear + ResnetBlock2D Conv2d sites through the arena:
     conv dA/dB land in the flat gradient buffer) vs the oracle's reference step. Dropout is set
@@ -490,36 +453,6 @@ def test_arena_step_after_torch_side_edit_keeps_operands_fresh():
     torch.cuda.synchronize()
     assert not torch.equal(before, site.lora_up.weight.detach())
     assert rel(site(x), want()) < 2 ** -7             # operands follow the fused step too
-
-
-def test_async_wgrad_option_matches_default():
-    """StepConfig.async_wgrad: dA/dB reductions on a side stream joined before the optimizer."""
-    import lora_b200 as L
-    from lora_b200.train import LoraTrainStep, StepConfig
-    traj = []
-    for flag in (False, True):
-        unet, text = _tiny_models(seed=7)
-        unet, text = unet.to(torch.bfloat16), text.to(torch.bfloat16)
-        L.inject_trainable_lora(unet, r=4)
-        L.inject_trainable_lora(text, target_replace_module={"CLIPAttention"}, r=4)
-        g = torch.Generator(device=DEV).manual_seed(3)
-        for m in list(unet.modules()) + list(text.modules()):
-            if type(m).__name__ == "LoraInjectedLinear":
-                m.lora_up.weight.data.normal_(0, 0.05, generator=g)
-        tr = LoraTrainStep(unet, text, StepConfig(use_cuda_graph=False, async_wgrad=flag),
-                           latent_shape=(1, 4, 16, 16), device=DEV)
-        torch.manual_seed(9)
-        tr.latents.copy_(torch.randn(1, 4, 16, 16, device=DEV) * 0.18215)
-        tr.input_ids.copy_(torch.randint(0, 1000, (1, 77), device=DEV))
-        out = []
-        for i in range(3):
-            torch.manual_seed(40 + i)
-            out.append(float(tr.step_device()))
-        torch.cuda.synchronize()
-        traj.append((out, tr.arena.p.clone()))
-    for a, b in zip(traj[0][0], traj[1][0]):
-        assert abs(a - b) < 2e-3 * abs(a)
-    assert rel(traj[1][1], traj[0][1]) < 1e-3
 
 
 @pytest.mark.parametrize("r", [32, 20])
