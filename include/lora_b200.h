@@ -12,8 +12,9 @@
  *   - LoRA master factors are fp32:   down A[r,K] row-major,   up B[N,r] row-major
  *     (reference: lora_down.weight / lora_up.weight, lora_diffusion/lora.py:44-46).
  *   - "down16" operands are 16-bit copies zero-padded to 16 rows: [16,K] row-major
- *     (built by lb_cast_rows_pad16). Rank r <= 16 in this version.
- *   - T buffers are fp32 [M,16] row-major, columns >= r are zero.
+ *     (built by lb_cast_rows_pad16). Rank r <= 16 on these entry points; ranks up to 64 use the
+ *     "_rp" entry points at the end of this header, with 32 or 64 padded rows.
+ *   - T buffers are fp32 [M,16] row-major (the "_rp" entries: [M,r_pad]), columns >= r are zero.
  *   - All base pointers 16-byte aligned; K % 8 == 0; N % 8 == 0 (N % 4 for fp32 outputs).
  */
 #ifndef LORA_B200_H
@@ -26,7 +27,7 @@ extern "C" {
 enum lb_status {
   LB_OK = 0,
   LB_ERR_SHAPE = -1, /* unsupported / misaligned extent */
-  LB_ERR_RANK = -2,  /* r outside [1,16] */
+  LB_ERR_RANK = -2,  /* r outside [1,16] (the "_rp" entry points: [1,r_pad]) */
   LB_ERR_DTYPE = -3,
   LB_ERR_ALIGN = -4, /* pointer not 16-byte aligned */
   LB_ERR_TMAP = -5,  /* cuTensorMapEncodeTiled unavailable or failed */
@@ -242,7 +243,8 @@ int lb_ti_embed_step(float* rows, float* grad, float* m, float* v, const long lo
                      void* stream);
 
 /* Fold a LoRA into its frozen weight: out[n,k] = W[n,k] + alpha * sum_j up[n,j]*down[j,k]
- * (W, out: LB_F32/LB_BF16/LB_F16 [N,K]; conv weights flattened to [Cout, Cin*kh*kw]; out may alias W).
+ * (W, out: LB_F32/LB_BF16/LB_F16 [N,K]; conv weights flattened to [Cout, Cin*kh*kw]; out may alias W;
+ * 1 <= r <= 64).
  * Replaces the up@down GEMM + add of collapse_lora, lora_diffusion/lora.py:635-669. */
 int lb_lora_merge(const void* W, int w_dtype, const float* up, const float* down, float alpha, void* out,
                   int N, int K, int r, void* stream);
@@ -388,6 +390,89 @@ int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long stride_b, 
                           long long stride_p, const float* target, const float* mask,
                           const float* weights, void* grad, float* loss, float* partials64,
                           unsigned int* counter, int B, int C, int H, int W, void* stream);
+
+/* ---- LoRA ranks 17..64: the "_rp" siblings of the entry points whose operand layout holds the rank
+ * pad. Each takes `r_pad` (16, 32 or 64; r <= r_pad) right after `r`: the down / up-transposed operands
+ * are [r_pad, K] / [r_pad, N] 16-bit with rows r.. zero, and every T / dT / V operand is [M, r_pad] fp32.
+ * With r_pad = 16 they compute what the entry points without the suffix compute, which keep
+ * accepting r <= 16 only. r_pad outside {16, 32, 64}: LB_ERR_SHAPE; r > r_pad: LB_ERR_RANK (both
+ * before any CUDA call). At r_pad > 16 the fused kernels run one tile per CTA (no split-K plans), and
+ * the 3x3 conv input gradient (per_tap_T = 1) reads its per-tap T from T_in; without T_in it first
+ * writes T_out = X . down^T (one more launch, so T_out is required) and reads that. T_in and T_out
+ * together are refused there. */
+int lb_lora_linear_fwd_rp(const void* X, const void* W, const float* bias, const void* down,
+                          const float* up, long long up_rs, long long up_cs, const float* diag,
+                          float scale, void* Y, float* T_out, const float* T_in, int M, int K, int N,
+                          int r, int r_pad, int in_dtype, int out_dtype, void* stream);
+int lb_lora_linear_fwd_dropout_rp(const void* X, const void* W, const float* bias, const void* down,
+                                  const float* up, long long up_rs, long long up_cs, const float* diag,
+                                  float scale, void* Y, float* T_out, int M, int K, int N, int r, int r_pad,
+                                  int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
+                                  void* stream);
+int lb_lora_conv2d_fwd_rp(const void* X, const void* W, const float* bias, const void* down,
+                          const float* up, long long up_rs, long long up_cs, long long up_gs,
+                          const float* diag, float scale, void* Y, float* T_out, const float* T_in,
+                          int n_img, int H, int Wd, int Cin, int Cout, int kh, int kw, int pad_h,
+                          int pad_w, int r, int r_pad, int per_tap_T, int in_dtype, int out_dtype,
+                          void* stream);
+int lb_lora_conv2d_fwd_dropout_rp(const void* X, const void* W, const float* bias, const void* down,
+                                  const float* up, long long up_rs, long long up_cs, const float* diag,
+                                  float scale, void* Y, float* T_out, int n_img, int H, int Wd, int Cin,
+                                  int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
+                                  int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
+                                  void* stream);
+int lb_lora_wgrad_rp(const void* S, const float* V, const float* diag, float scale, float* out,
+                     long long out_js, long long out_cs, int M, int C, int r, int r_pad, int in_dtype,
+                     void* stream);
+int lb_lora_wgrad_shift_rp(const void* S, const float* V, const float* diag, float scale, float* out,
+                           long long out_js, long long out_cs, int M, int C, int r, int r_pad, int H,
+                           int W, int dy, int dx, int in_dtype, void* stream);
+int lb_lora_wgrad_masked_rp(const void* S, const float* V, const float* diag, float scale, float* out,
+                            long long out_js, long long out_cs, int M, int C, int r, int r_pad,
+                            float drop_p, const void* seed_dev, int in_dtype, void* stream);
+int lb_lora_wgrad_conv_rp(const void* S, const float* V, const float* diag, float scale, float* out,
+                          int M, int C, int r, int r_pad, int H, int W, int kh, int kw, int pad_h,
+                          int pad_w, int in_dtype, void* stream);
+int lb_lora_wgrad_pair_rp(const void* X, const float* dTs, float* dA, long long dA_js, long long dA_cs,
+                          int K, const void* gY, const float* T, float* dB, long long dB_js,
+                          long long dB_cs, int N, const float* diag, float scale, int M, int r,
+                          int r_pad, float drop_p, const void* seed_dev, int in_dtype, void* stream);
+/* lb_wgrad_problem with the row pitch of V (r_pad) */
+typedef struct lb_wgrad_problem_rp {
+  const void* S;        /* [M, C] rows of in_dtype                         */
+  const float* V;       /* [M, r_pad] fp32                                 */
+  float* out;
+  long long out_js, out_cs;
+  int M, C, r;
+  float scale;
+  const float* diag;
+  float drop_p;
+  const void* seed_dev;
+  int conv_H, conv_W, kh, kw, pad_h, pad_w;
+  int r_pad;
+} lb_wgrad_problem_rp;
+int lb_lora_wgrad_batch_rp(const lb_wgrad_problem_rp* probs, int n, int in_dtype, void* stream);
+int lb_lora_up_dropout_rp(void* Y, int y_dtype, const float* T, const float* up, long long up_rs,
+                          long long up_cs, const float* diag, float scale, float drop_p,
+                          const void* seed_dev, int M, int N, int r, int r_pad, void* stream);
+int lb_lora_dropout_dt_rp(const void* gY, int in_dtype, const float* up, long long up_rs, long long up_cs,
+                          float drop_p, const void* seed_dev, float* dTs, int M, int N, int r, int r_pad,
+                          void* stream);
+int lb_cast_rows_pad16_rp(const float* src, long long src_rs, long long src_cs, void* dst16, int r,
+                          int r_pad, int C, int out_dtype, void* stream);
+/* lb_refresh_shadows / lb_optim_step_fused with 8-column table rows
+ * {src_off, src_rs, src_cs, r, C, dst_off, dst_rs, rows}: `rows` padded rows per entry. The table is
+ * device memory and is not checked: `rows` must be 16, 32 or 64, r <= rows, and the destination slot
+ * must hold `rows` rows of pitch dst_rs (rows * dst_rs elements from dst_off) -- a larger `rows`
+ * writes past the slot. */
+int lb_refresh_shadows_rp(const float* p, const long long* table, int n_entries, int max_C,
+                          void* dst16_base, int out_dtype, void* stream);
+int lb_optim_step_fused_rp(float* p, float* g, float* m, float* v, long long n,
+                           const long long* group_off, int n_groups, const float* lr_dev, float beta1,
+                           float beta2, float eps, float weight_decay, float max_norm, float inv_world,
+                           int* step_dev, float* partials, float* gnorm_out, const long long* table,
+                           int n_entries, int max_C, void* shadow16, int shadow_dtype,
+                           unsigned int* barrier2, void* stream);
 
 #ifdef __cplusplus
 }

@@ -115,6 +115,7 @@ class _FusedLoraConv2dFn(torch.autograd.Function):
         dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
         # dX = conv_T(gY, W) + conv_T((gY.B)*s*d, A); "up" = A read flipped: element (c, tap g, j)
         # at A[j, c, taps-1-g]  ->  base offset taps-1, up_rs = taps, up_cs = cin*taps, up_gs = -1
+        # (rank pads 32 / 64: the entry computes dTs = gY.B first and runs the taps through it)
         dX, dTs = ops.fused_conv2d(gy16, w_b, None, upT16, A32, taps - 1, taps, cin * taps, -1,
                                    ctx.diag, ctx.scale, r, cin, kh, kw, kh - 1 - ph, kw - 1 - pw,
                                    True, dx_dtype, True)
@@ -139,9 +140,9 @@ class _FusedLoraConv2dFn(torch.autograd.Function):
 
 
 def lora_conv2d(mod, x):
-    if mod.r > 16:
-        raise LoraB200Error("LoraInjectedConv2d: LoRA rank > 16 is not supported by the fused conv kernel "
-                            "(linear sites run as rank chunks, rank_chunks.py)")
+    if mod.r > ops.MAX_RANK:
+        raise LoraB200Error(f"LoraInjectedConv2d: LoRA rank {mod.r} > {ops.MAX_RANK} is not supported by the "
+                            "fused conv kernel (linear sites run as rank chunks, rank_chunks.py)")
     if mod.training and mod.dropout.p > 0.0:
         from .dropout_path import lora_conv2d_dropout
         return lora_conv2d_dropout(mod, x)

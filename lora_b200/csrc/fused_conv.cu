@@ -9,11 +9,14 @@
 
 namespace lb {
 
-template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, bool SPLITK = false>
+int launch_t_from16(const void* gY, int fmt, const void* down, int C, int M, int r, int rp, float* T,
+                    cudaStream_t st);   // lora_aux.cu
+
+template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, bool SPLITK = false, int RP = R_PAD>
 static int launch_conv(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p_in,
                        int n_img, int down_cols, int out_dtype, cudaStream_t stream, int split = 1) {
-  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP>;
-  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, true, G, 1, DROP, SPLITK>;
+  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP, 1, RP>;
+  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, true, G, 1, DROP, SPLITK, 1, false, RP>;
   FusedParams p = p_in;
   p.split = 1;
   if constexpr (SPLITK) {
@@ -30,7 +33,7 @@ static int launch_conv(const void* X, const void* W, const void* Dn, void* Y, co
   CUtensorMap tmX, tmW, tmD, tmY;
   if (!tmap_nhwc(&tmX, X, in_dt, 2, p.C, p.W, p.H, n_img, BLOCK_K, p.TW, p.TH)) return LB_ERR_TMAP;
   if (!tmap_2d(&tmW, W, in_dt, 2, p.K, p.N, BLOCK_K, BLOCK_N, true)) return LB_ERR_TMAP;
-  if (!tmap_2d(&tmD, Dn, in_dt, 2, down_cols, R_PAD, BLOCK_K, R_PAD, true)) return LB_ERR_TMAP;
+  if (!tmap_2d(&tmD, Dn, in_dt, 2, down_cols, RP, BLOCK_K, RP, true)) return LB_ERR_TMAP;
   if (!tmap_nhwc(&tmY, Y, out_dt, sizeof(OutT), p.N, p.W, p.H, n_img, S::BOX_COLS, p.TW, p.TH)) return LB_ERR_TMAP;
   dim3 grid((p.N + BLOCK_N - 1) / BLOCK_N, n_img * p.tiles_h * p.tiles_w, SPLITK ? split : 1);
   return launch_ex(kern, grid, dim3(NUM_THREADS), S::DYN_BYTES, stream, 1, tmX, tmW, tmD, tmY, p) == cudaSuccess
@@ -62,23 +65,54 @@ static ConvPlan plan_conv_split(long long m_tiles, int num_kb, int N, int g, int
   return {0, 1};
 }
 
+// Ranks 17..64 (RP = 32 or 64): one tile per CTA, 64 wide while those tiles fit one wave, else 128;
+// no split-K plans at these pads (a scope choice, not a measured one). The 3x3 input gradient runs the
+// tap loop (T from t_in, fused_core.cuh TAPLOOP). A 128-wide fp32-output dropout tile at RP = 64 does not
+// fit shared memory; it runs 64 wide.
+template <int RP>
+static int launch_conv_wide(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p,
+                            int n_img, int down_cols, int out_dtype, cudaStream_t st, bool drop, bool groups,
+                            bool narrow) {
+#define LB_CONVW(BN, OT, GG, DR) launch_conv<BN, 4, OT, GG, DR, false, RP>(X, W, Dn, Y, p, n_img, down_cols, out_dtype, st)
+  if (drop) {
+    if (out_dtype == LB_F32) {
+      if (narrow || RP == 64) return LB_CONVW(64, float, 1, true);
+      if constexpr (RP != 64) return LB_CONVW(128, float, 1, true);
+    }
+    return narrow ? LB_CONVW(64, uint16_t, 1, true) : LB_CONVW(128, uint16_t, 1, true);
+  }
+  if (groups) {
+    if (out_dtype == LB_F32) return narrow ? LB_CONVW(64, float, 9, false) : LB_CONVW(128, float, 9, false);
+    return narrow ? LB_CONVW(64, uint16_t, 9, false) : LB_CONVW(128, uint16_t, 9, false);
+  }
+  if (out_dtype == LB_F32) return narrow ? LB_CONVW(64, float, 1, false) : LB_CONVW(128, float, 1, false);
+  return narrow ? LB_CONVW(64, uint16_t, 1, false) : LB_CONVW(128, uint16_t, 1, false);
+#undef LB_CONVW
+}
+
 }  // namespace lb
 
 static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
                                   const void* down16, const float* up, long long up_rs,
                                   long long up_cs, long long up_gs, const float* diag, float scale,
                                   void* Y, float* T_out, const float* T_in, int n_img, int H, int Wd, int Cin,
-                                  int Cout, int kh, int kw, int pad_h, int pad_w, int r,
+                                  int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
                                   int per_tap_T, int in_dtype, int out_dtype, float drop_p,
                                   const void* seed_dev, void* stream) {
   using namespace lb;
+  if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
   if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && (seed_dev == nullptr || T_in != nullptr || per_tap_T != 0)))
     return LB_ERR_SHAPE;
   if (n_img <= 0 || H <= 0 || Wd <= 0 || Cin <= 0 || Cout <= 0) return LB_ERR_SHAPE;
   if (!((kh == 1 && kw == 1) || (kh == 3 && kw == 3))) return LB_ERR_SHAPE;
   // "same" geometry only (output extent == input extent), which is what stride-1 SD convs use
   if (2 * pad_h != kh - 1 || 2 * pad_w != kw - 1) return LB_ERR_SHAPE;
-  if (r < 1 || r > R_PAD) return LB_ERR_RANK;
+  if (r < 1 || r > r_pad) return LB_ERR_RANK;
+  // the wide-rank 3x3 input gradient reads its per-tap T from T_in; without T_in it first computes
+  // T_out = X . down^T (one extra pass over X) and reads that
+  const bool t_first = r_pad > R_PAD && per_tap_T != 0 && kh * kw > 1 && T_in == nullptr;
+  if (t_first && T_out == nullptr) return LB_ERR_SHAPE;
+  if (r_pad > R_PAD && per_tap_T != 0 && kh * kw > 1 && T_in != nullptr && T_out != nullptr) return LB_ERR_SHAPE;
   if (in_dtype != LB_BF16 && in_dtype != LB_F16) return LB_ERR_DTYPE;
   if (out_dtype != in_dtype && out_dtype != LB_F32) return LB_ERR_DTYPE;
   if ((Cin % 8) != 0 || (Cout % 8) != 0) return LB_ERR_SHAPE;
@@ -108,6 +142,15 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
   // the 64x64-pixel, Cout = 320 sites are 96 tiles of 128 but 160 of 64 -- a second wave over 45-135 K blocks
   const long long tiles64c = static_cast<long long>(n_img) * p.tiles_h * p.tiles_w * ((Cout + 63) / 64);
   const bool narrow = tiles64c <= sm_count();
+  if (t_first) {
+    const int rc = launch_t_from16(X, p.fmt, down16, Cin, p.M, r, r_pad, T_out, st);
+    if (rc != LB_OK) return rc;
+    p.t_in = T_out;
+    p.t_out = nullptr;
+  }
+  if (r_pad > R_PAD)
+    return r_pad == 32 ? launch_conv_wide<32>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, drop_p > 0.f, groups, narrow)
+                       : launch_conv_wide<64>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, drop_p > 0.f, groups, narrow);
 #define LB_CONV(BN, OT, GG) launch_conv<BN, 4, OT, GG>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
   const int cblocks = (Cin + BLOCK_K - 1) / BLOCK_K;
   const ConvPlan sp = plan_conv_split(static_cast<long long>(n_img) * p.tiles_h * p.tiles_w, taps * cblocks, Cout,
@@ -152,8 +195,19 @@ extern "C" int lb_lora_conv2d_fwd(const void* X, const void* W, const float* bia
                                   int Cout, int kh, int kw, int pad_h, int pad_w, int r,
                                   int per_tap_T, int in_dtype, int out_dtype, void* stream) {
   return conv2d_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, up_gs, diag, scale, Y, T_out, T_in, n_img, H,
-                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, per_tap_T, in_dtype, out_dtype, 0.f, nullptr,
+                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, 16, per_tap_T, in_dtype, out_dtype, 0.f, nullptr,
                          stream);
+}
+
+extern "C" int lb_lora_conv2d_fwd_rp(const void* X, const void* W, const float* bias,
+                                     const void* down, const float* up, long long up_rs,
+                                     long long up_cs, long long up_gs, const float* diag, float scale,
+                                     void* Y, float* T_out, const float* T_in, int n_img, int H, int Wd, int Cin,
+                                     int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
+                                     int per_tap_T, int in_dtype, int out_dtype, void* stream) {
+  return conv2d_fwd_impl(X, W, bias, down, up, up_rs, up_cs, up_gs, diag, scale, Y, T_out, T_in, n_img, H,
+                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, r_pad, per_tap_T, in_dtype, out_dtype, 0.f,
+                         nullptr, stream);
 }
 
 extern "C" int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias,
@@ -163,6 +217,17 @@ extern "C" int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const fl
                                           int kw, int pad_h, int pad_w, int r, int in_dtype, int out_dtype,
                                           float drop_p, const void* seed_dev, void* stream) {
   return conv2d_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, 0, diag, scale, Y, T_out, nullptr, n_img, H,
-                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, 0, in_dtype, out_dtype, drop_p, seed_dev,
+                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, 16, 0, in_dtype, out_dtype, drop_p, seed_dev,
+                         stream);
+}
+
+extern "C" int lb_lora_conv2d_fwd_dropout_rp(const void* X, const void* W, const float* bias,
+                                             const void* down, const float* up, long long up_rs,
+                                             long long up_cs, const float* diag, float scale, void* Y,
+                                             float* T_out, int n_img, int H, int Wd, int Cin, int Cout, int kh,
+                                             int kw, int pad_h, int pad_w, int r, int r_pad, int in_dtype,
+                                             int out_dtype, float drop_p, const void* seed_dev, void* stream) {
+  return conv2d_fwd_impl(X, W, bias, down, up, up_rs, up_cs, 0, diag, scale, Y, T_out, nullptr, n_img, H,
+                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, r_pad, 0, in_dtype, out_dtype, drop_p, seed_dev,
                          stream);
 }

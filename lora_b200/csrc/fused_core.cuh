@@ -9,14 +9,17 @@
 //                          4-D TMA box whose out-of-image part is zero-filled by the hardware
 //                          (that IS the padding). Stride 1, dilation 1, groups 1.
 //
-// The LoRA down factor D ([16, K] 16-bit, zero-padded rank) rides the main K loop: its 16 rows are
-// appended below every W tile in shared memory, so the tensor core produces T = X.D^T alongside
-// the base accumulator from the same X tile -- X is read from HBM exactly once.
-//   G == 1: one wgmma per K-step with N = BLOCK_N + 16; T is accumulator columns [BLOCK_N, +16).
+// The LoRA down factor D ([RP, K] 16-bit, rank zero-padded to RP = 16, 32 or 64) rides the main K
+// loop: its RP rows are appended below every W tile in shared memory, so the tensor core produces
+// T = X.D^T alongside the base accumulator from the same X tile -- X is read from HBM exactly once.
+//   G == 1: one wgmma per K-step with N = BLOCK_N + RP; T is accumulator columns [BLOCK_N, +RP).
 //                                                         (linear fwd / dX, conv fwd, 1x1 conv dX)
 //   G  > 1: the conv input-gradient. dX needs a separate T_t = gY(shifted by tap t) . B per tap,
 //           so each K-step issues N = BLOCK_N into the base accumulator and N = 16 into the tap's
-//           own accumulator.
+//           own accumulator (RP = 16). At RP > 16 the taps' T come from t_in instead (TAPLOOP in
+//           Smem): the K loop issues N = BLOCK_N only, and the epilogue adds T'_t . U_t^T tap by tap.
+// The up-projection is a K = RP wgmma chain (RP / 16 K-steps per T group) over an interleaved
+// core-matrix layout of T' and U.
 //
 // Roles: warps 0-7 are two consumer warpgroups -- warpgroup w owns accumulator rows [64 w, 64 w + 64)
 // and issues wgmma.m64nNk16 on the shared-memory stages, the accumulators live in its registers;
@@ -60,8 +63,8 @@ struct FusedParams {
   const float* up;     // fp32 LoRA-up factor: element (n, g, j) at up[n*up_rs + j*up_cs + g*up_gs]
   long long up_rs, up_cs, up_gs;
   const float* diag;   // [r] or null (selector diagonal)
-  float* t_out;        // [M,16] fp32 side output (group t_group, unscaled), n_blk == 0 CTAs; or null
-  const float* t_in;   // [M,16] fp32 or null: when set, the rank-r activations are TAKEN from here
+  float* t_out;        // [M,RP] fp32 side output (group t_group, unscaled), n_blk == 0 CTAs; or null
+  const float* t_in;   // [M,RP] fp32 or null: when set, the rank-r activations are TAKEN from here
                        // (row = this row / the tap-shifted pixel) instead of from the accumulator. Used
                        // by the dropout path, where T = (mask o gY).B cannot share the base operand.
   float scale;
@@ -111,23 +114,30 @@ __device__ __forceinline__ unsigned long long gtimer() {
 }
 #define LB_STAMP(i) do { if (p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0) p.dbg[i] = gtimer(); } while (0)
 
-template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, int CL = 1>
+template <int BLOCK_N, int STAGES, typename OutT, int G, bool DROP = false, int CL = 1, int RP = R_PAD>
 struct Smem {
+  // TAPLOOP: conv input-gradient (G taps) at RP > 16. Per-tap T accumulators would not fit, so T is
+  // taken from t_in and the epilogue runs the taps one after another through ONE T'/U buffer pair;
+  // the main loop carries no D rows and no T columns.
+  static constexpr bool TAPLOOP = G > 1 && RP > R_PAD;
+  static constexpr int DROWS = TAPLOOP ? 0 : RP;        // D rows below each W tile
+  static constexpr int TCOLS = TAPLOOP ? 0 : RP * G;    // T columns of the parked accumulator
+  static constexpr int TG = TAPLOOP ? 1 : G;            // T'/U groups staged at once
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = (BLOCK_N + R_PAD) * BLOCK_K * 2;
+  static constexpr int B_BYTES = (BLOCK_N + DROWS) * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // one TMA transaction: X tile, W tile + D rows
   // fp32 accumulator parked after the K loop: base columns, T group(s), and (DROP) the LoRA product,
   // which the mask separates from the sum. Row pitch padded by 8 floats against bank conflicts.
-  static constexpr int L_COL0 = BLOCK_N + R_PAD * G;
-  static constexpr int ACC_COLS = BLOCK_N + R_PAD * G + (DROP ? BLOCK_N : 0);
+  static constexpr int L_COL0 = BLOCK_N + TCOLS;
+  static constexpr int ACC_COLS = BLOCK_N + TCOLS + (DROP ? BLOCK_N : 0);
   static constexpr int ACC_LD = ACC_COLS + 8;
   static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
   static constexpr int BOX_COLS = 128 / sizeof(OutT);  // columns per 128-byte store box
   static constexpr int NUM_BOXES = BLOCK_N / BOX_COLS;
   static constexpr int BOX_BYTES = BLOCK_M * 128;
-  static constexpr int T_BYTES = BLOCK_M * R_PAD * G * 2;   // T' operand(s)
-  static constexpr int UP_BYTES = BLOCK_N * R_PAD * G * 2;  // U tile(s)
+  static constexpr int T_BYTES = BLOCK_M * RP * TG * 2;   // T' operand(s)
+  static constexpr int UP_BYTES = BLOCK_N * RP * TG * 2;  // U tile(s)
   // the accumulator is parked only after the last stage has been consumed: it aliases the ring
   static constexpr int OFF_ACC = 0;
   static constexpr int OFF_EPI = (((RING_BYTES > ACC_BYTES ? RING_BYTES : ACC_BYTES) + 1023) / 1024) * 1024;
@@ -199,15 +209,21 @@ __device__ __forceinline__ void ld_acc16(const float* src, float* v) {
 
 // One output tile (n_blk, m_blk) of one problem; called by the single-problem and the grouped kernel.
 template <int BLOCK_N, int STAGES, typename OutT, bool CONV, int G, bool DROP = false, bool SPLITK = false,
-          int CL = 1, bool INLINE_TMA = false>
+          int CL = 1, bool INLINE_TMA = false, int RP = R_PAD>
 __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtensorMap& tmW,
                                            const CUtensorMap& tmD, const CUtensorMap& tmY,
                                            const FusedParams& p, const int n_blk, const int m_blk) {
-  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP, CL>;
+  using S = Smem<BLOCK_N, STAGES, OutT, G, DROP, CL, RP>;
   static_assert(CL == 1 || (!CONV && G == 1 && !DROP && !SPLITK), "cluster split-K: plain linear tiles");
   static_assert(!INLINE_TMA || (!CONV && G == 1 && !DROP && !SPLITK && CL == 1), "inline TMA: plain linear tiles");
-  constexpr int PCOLS = BLOCK_N + R_PAD * G;          // columns of one partial accumulator
-  constexpr bool WIDE = G == 1;                       // T rides the base MMA as 16 extra columns
+  // wider ranks run the one-tile-per-CTA schedules only (a scope choice, not a measured one)
+  static_assert(RP == R_PAD || ((RP == 32 || RP == 64) && !SPLITK && CL == 1 && !INLINE_TMA), "rank pad");
+  static_assert(!S::TAPLOOP || (CONV && !DROP), "tap loop: conv input-gradient");
+  constexpr bool TAPLOOP = S::TAPLOOP;
+  constexpr int GQ = RP / 16;                         // 16-wide K-steps per T group
+  constexpr int KG = S::TG * GQ;                      // 16-wide K-steps of the staged up-projection
+  constexpr int PCOLS = BLOCK_N + S::TCOLS;           // columns of one partial accumulator
+  constexpr bool WIDE = G == 1;                       // T rides the base MMA as RP extra columns
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* sgen = smem_raw + (sbase - smem_u32(smem_raw));  // generic pointer to the aligned base
@@ -277,8 +293,9 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
       const int dy = tap / p.kw, dx = tap - dy * p.kw;
       tma_load_4d(&tmX, bar_full(s), sa, cb * BLOCK_K, w0 + dx - p.pad_w, h0 + dy - p.pad_h, img);
       load_w_tile<BLOCK_N>(&tmW, bar_full(s), sb, tap * p.C + cb * BLOCK_K, kb, num_kb, n0, p.w_tiled);
-      tma_load_2d(&tmD, bar_full(s), sb + BLOCK_N * 128,
-                  (p.down_per_tap ? tap * p.C : 0) + cb * BLOCK_K, 0);
+      if constexpr (!TAPLOOP)
+        tma_load_2d(&tmD, bar_full(s), sb + BLOCK_N * 128,
+                    (p.down_per_tap ? tap * p.C : 0) + cb * BLOCK_K, 0);
     } else {
       tma_load_2d(&tmX, bar_full(s), sa, kb * BLOCK_K, m0);
       load_w_tile<BLOCK_N>(&tmW, bar_full(s), sb, kb * BLOCK_K, kb, num_kb, n0, p.w_tiled);
@@ -307,18 +324,21 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
   const int wg = ct >> 7;              // accumulator rows [64 wg, 64 wg + 64)
   float* bias_s = reinterpret_cast<float*>(sgen + S::OFF_BIAS);
 
-  // Stage the U tile(s) (fp32 master -> 16-bit, interleaved core-matrix layout) and the bias; the
-  // TMA producer is already streaming the first stages.
+  // Stage the U tile(s) (fp32 master -> 16-bit, interleaved core-matrix layout: 16-wide K-step kk of
+  // row i at (i >> 3) * 256 KG + kk * 256 + (i & 7) * 16) and the bias; the TMA producer is already
+  // streaming the first stages. TAPLOOP stages each tap's U in the epilogue instead.
   for (int i = ct; i < BLOCK_N; i += CONSUMER_THREADS) {
     const int n = n0 + i;
     const bool ok = n < p.N;
 #pragma unroll
-    for (int g = 0; g < G; ++g) {
-      float u[R_PAD];
+    for (int g = 0; g < S::TG * !TAPLOOP; ++g)
 #pragma unroll
-      for (int j = 0; j < R_PAD; ++j)
-        u[j] = (ok && j < p.r) ? __ldg(p.up + n * p.up_rs + j * p.up_cs + g * p.up_gs) : 0.f;
-      const uint32_t dst = sbase + S::OFF_UP + (i >> 3) * (256 * G) + g * 256 + (i & 7) * 16;
+    for (int q = 0; q < GQ; ++q) {
+      float u[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        u[j] = (ok && 16 * q + j < p.r) ? __ldg(p.up + n * p.up_rs + (16 * q + j) * p.up_cs + g * p.up_gs) : 0.f;
+      const uint32_t dst = sbase + S::OFF_UP + (i >> 3) * (256 * KG) + (g * GQ + q) * 256 + (i & 7) * 16;
       st_shared_v4(dst, pack2(u[0], u[1], p.fmt), pack2(u[2], u[3], p.fmt),
                    pack2(u[4], u[5], p.fmt), pack2(u[6], u[7], p.fmt));
       st_shared_v4(dst + 128, pack2(u[8], u[9], p.fmt), pack2(u[10], u[11], p.fmt),
@@ -329,7 +349,7 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
 
   // register accumulators (zero-initialised: every wgmma accumulates)
   constexpr int AREG = (WIDE ? PCOLS : BLOCK_N) / 2;
-  constexpr int TG = WIDE ? 1 : G;     // separate T accumulators (unused when WIDE)
+  constexpr int TG = (WIDE || TAPLOOP) ? 1 : G;   // separate T accumulators (unused when WIDE / TAPLOOP)
   float acc[AREG];
   float tacc[TG][R_PAD / 2];
 #pragma unroll
@@ -357,7 +377,9 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
       const uint64_t ad = wgmma_desc(sa + wg * (64 * 128) + k * MMA_K * 2, 16, 1024, 1);
       const uint64_t bd = wgmma_desc(sb + k * MMA_K * 2, 16, 1024, 1);
       if constexpr (WIDE) {
-        wgmma_ss<BLOCK_N + R_PAD>(acc, ad, bd, p.fmt);
+        wgmma_ss<BLOCK_N + RP>(acc, ad, bd, p.fmt);
+      } else if constexpr (TAPLOOP) {
+        wgmma_ss<BLOCK_N>(acc, ad, bd, p.fmt);
       } else {
         const uint64_t dd = wgmma_desc(sb + BLOCK_N * 128 + k * MMA_K * 2, 16, 1024, 1);
         wgmma_ss<BLOCK_N>(acc, ad, bd, p.fmt);
@@ -372,7 +394,7 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
     // inline TMA: the stage just released takes K block kb - 1 + STAGES
     if (INLINE_TMA && ct == 0 && it > 0 && kb - 1 + STAGES < kb_end) load_stage(kb - 1 + STAGES);
   };
-  if constexpr (WIDE) {
+  if constexpr (WIDE || TAPLOOP) {
     for (int kb = kb_begin; kb < kb_end; ++kb) k_block(kb, nullptr);
   } else {
 #pragma unroll
@@ -391,7 +413,7 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
   // retired: park the accumulator over it
   named_bar_sync(BAR_CONSUMERS, CONSUMER_THREADS);
   park_acc<WIDE ? PCOLS : BLOCK_N, S::ACC_LD>(acc_s, acc, wg * 64, 0);
-  if constexpr (!WIDE) {
+  if constexpr (!WIDE && !TAPLOOP) {
 #pragma unroll
     for (int g = 0; g < TG; ++g) park_acc<R_PAD, S::ACC_LD>(acc_s, tacc[g], wg * 64, BLOCK_N + R_PAD * g);
   }
@@ -436,10 +458,14 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
   long long grow = -1;          // global row (pixel) this thread owns, for the T side output
   if (ct < EPI_THREADS) {
     // ------------------------------------------------------------ epilogue part 1 (row per thread)
-    float coef[R_PAD];
+    // T is scaled 16 columns at a time: t[RP] and coef[RP] at once would not fit beside the accumulator
+    float coef[16];
+    auto load_coef = [&](const int j0) {
 #pragma unroll
-    for (int j = 0; j < R_PAD; ++j)
-      coef[j] = (j < p.r) ? p.scale * (p.diag ? __ldg(p.diag + j) : 1.f) : 0.f;
+      for (int j = 0; j < 16; ++j)
+        coef[j] = (j0 + j < p.r) ? p.scale * (p.diag ? __ldg(p.diag + j0 + j) : 1.f) : 0.f;
+    };
+    if constexpr (RP == R_PAD) load_coef(0);
     if constexpr (CONV) {
       const int hh = h0 + row / p.TW, ww = w0 + row % p.TW;
       if (hh < p.H && ww < p.W) grow = (static_cast<long long>(img) * p.H + hh) * p.W + ww;
@@ -493,10 +519,12 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
         for (int i = 0; i < PCOLS / 4; ++i) __stcg(dstz + i, make_float4(0.f, 0.f, 0.f, 0.f));
       }
     }
-    if (elected) {
+    if (!TAPLOOP && elected) {
 #pragma unroll
-      for (int g = 0; g < G; ++g) {
-        float t[R_PAD];
+      for (int g = 0; g < S::TG; ++g)
+#pragma unroll
+      for (int q = 0; q < GQ; ++q) {
+        float t[16];
         if (p.t_in == nullptr) {
           if constexpr (SPLITK) {
             if constexpr (G == 1) {
@@ -512,7 +540,7 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
               }
             }
           } else {
-            ld_acc16(arow + BLOCK_N + R_PAD * g, t);
+            ld_acc16(arow + BLOCK_N + RP * g + 16 * q, t);
           }
         } else {
           long long srow = grow;
@@ -523,25 +551,26 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
                        ? (static_cast<long long>(img) * p.H + hh) * p.W + ww : -1;
           }
           if (srow >= 0) {
-            const float4* src = reinterpret_cast<const float4*>(p.t_in + srow * R_PAD);
+            const float4* src = reinterpret_cast<const float4*>(p.t_in + srow * RP + 16 * q);
             const float4 a = __ldg(src), b = __ldg(src + 1), c = __ldg(src + 2), d = __ldg(src + 3);
             t[0] = a.x; t[1] = a.y; t[2] = a.z; t[3] = a.w; t[4] = b.x; t[5] = b.y; t[6] = b.z; t[7] = b.w;
             t[8] = c.x; t[9] = c.y; t[10] = c.z; t[11] = c.w; t[12] = d.x; t[13] = d.y; t[14] = d.z; t[15] = d.w;
           } else {
 #pragma unroll
-            for (int j = 0; j < R_PAD; ++j) t[j] = 0.f;
+            for (int j = 0; j < 16; ++j) t[j] = 0.f;
           }
         }
         if (p.t_out != nullptr && n_blk == 0 && g == p.t_group && grow >= 0) {
-          float4* dst = reinterpret_cast<float4*>(p.t_out + grow * R_PAD);
+          float4* dst = reinterpret_cast<float4*>(p.t_out + grow * RP + 16 * q);
           dst[0] = make_float4(t[0], t[1], t[2], t[3]);
           dst[1] = make_float4(t[4], t[5], t[6], t[7]);
           dst[2] = make_float4(t[8], t[9], t[10], t[11]);
           dst[3] = make_float4(t[12], t[13], t[14], t[15]);
         }
+        if constexpr (RP > R_PAD) load_coef(16 * q);
 #pragma unroll
-        for (int j = 0; j < R_PAD; ++j) t[j] *= coef[j];
-        const uint32_t dst = sbase + S::OFF_T + (row >> 3) * (256 * G) + g * 256 + (row & 7) * 16;
+        for (int j = 0; j < 16; ++j) t[j] *= coef[j];
+        const uint32_t dst = sbase + S::OFF_T + (row >> 3) * (256 * KG) + (g * GQ + q) * 256 + (row & 7) * 16;
         st_shared_v4(dst, pack2(t[0], t[1], p.fmt), pack2(t[2], t[3], p.fmt),
                      pack2(t[4], t[5], p.fmt), pack2(t[6], t[7], p.fmt));
         st_shared_v4(dst + 128, pack2(t[8], t[9], p.fmt), pack2(t[10], t[11], p.fmt),
@@ -555,10 +584,71 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
   // split-K: only the elected CTA continues (the others have delivered their partial)
   if (SPLITK && *flag == 0u) return;
 
-  // LoRA up-projection(s): acc[:, 0:BLOCK_N] += T'_g[128,16] . U_g[BLOCK_N,16]^T, this warpgroup's rows.
-  // No-swizzle K-major operand of total K = 16 G: core matrix = 8 rows x 16 B (128 B contiguous);
-  // LBO = 128 B (next K core matrix), SBO = 256 G bytes (next 8-row group).
-  {
+  // LoRA up-projection(s): acc[:, 0:BLOCK_N] += T'_g[128,RP] . U_g[BLOCK_N,RP]^T, this warpgroup's rows.
+  // No-swizzle K-major operand of total K = 16 KG: core matrix = 8 rows x 16 B (128 B contiguous);
+  // LBO = 128 B (next K core matrix), SBO = 256 KG bytes (next 8-row group).
+  if constexpr (TAPLOOP) {
+    // one tap at a time through the one T'/U buffer pair: stage U_t (all consumers) and T'_t
+    // (warpgroup 0, row per thread, from t_in at the tap-shifted pixel), then K = RP into acc
+#pragma unroll 1
+    for (int g = 0; g < G; ++g) {
+      for (int i = ct; i < BLOCK_N; i += CONSUMER_THREADS) {   // U_t
+        const int n = n0 + i;
+#pragma unroll
+        for (int q = 0; q < GQ; ++q) {
+          float u[16];
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+            u[j] = (n < p.N && 16 * q + j < p.r) ? __ldg(p.up + n * p.up_rs + (16 * q + j) * p.up_cs + g * p.up_gs) : 0.f;
+          const uint32_t dst = sbase + S::OFF_UP + (i >> 3) * (256 * KG) + q * 256 + (i & 7) * 16;
+          st_shared_v4(dst, pack2(u[0], u[1], p.fmt), pack2(u[2], u[3], p.fmt),
+                       pack2(u[4], u[5], p.fmt), pack2(u[6], u[7], p.fmt));
+          st_shared_v4(dst + 128, pack2(u[8], u[9], p.fmt), pack2(u[10], u[11], p.fmt),
+                       pack2(u[12], u[13], p.fmt), pack2(u[14], u[15], p.fmt));
+        }
+      }
+      if (ct < EPI_THREADS) {
+        const int hh = h0 + row / p.TW + g / p.kw - p.pad_h;
+        const int ww = w0 + row % p.TW + g % p.kw - p.pad_w;
+        const bool in = grow >= 0 && hh >= 0 && hh < p.H && ww >= 0 && ww < p.W;
+        const float4* src = reinterpret_cast<const float4*>(
+            p.t_in + (in ? ((static_cast<long long>(img) * p.H + hh) * p.W + ww) * RP : 0));
+#pragma unroll
+        for (int q = 0; q < GQ; ++q) {
+          float t[16];
+#pragma unroll
+          for (int j = 0; j < 16; j += 4) {
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (in) v = __ldg(src + (16 * q + j) / 4);
+            t[j] = v.x; t[j + 1] = v.y; t[j + 2] = v.z; t[j + 3] = v.w;
+          }
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+            t[j] *= (16 * q + j < p.r) ? p.scale * (p.diag ? __ldg(p.diag + 16 * q + j) : 1.f) : 0.f;
+          const uint32_t dst = sbase + S::OFF_T + (row >> 3) * (256 * KG) + q * 256 + (row & 7) * 16;
+          st_shared_v4(dst, pack2(t[0], t[1], p.fmt), pack2(t[2], t[3], p.fmt),
+                       pack2(t[4], t[5], p.fmt), pack2(t[6], t[7], p.fmt));
+          st_shared_v4(dst + 128, pack2(t[8], t[9], p.fmt), pack2(t[10], t[11], p.fmt),
+                       pack2(t[12], t[13], p.fmt), pack2(t[14], t[15], p.fmt));
+        }
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(BAR_CONSUMERS, CONSUMER_THREADS);   // T'_t, U_t staged
+      reg_fence<AREG>(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < KG; ++kk) {
+        const uint64_t ad = wgmma_desc(sbase + S::OFF_T + wg * (8 * 256 * KG) + kk * 256, 128, 256 * KG, 0);
+        const uint64_t bd = wgmma_desc(sbase + S::OFF_UP + kk * 256, 128, 256 * KG, 0);
+        wgmma_ss<BLOCK_N>(acc, ad, bd, p.fmt);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence<AREG>(acc);
+      named_bar_sync(BAR_CONSUMERS, CONSUMER_THREADS);   // both warpgroups done with the buffers
+    }
+    park_acc<BLOCK_N, S::ACC_LD>(acc_s, acc, wg * 64, 0);
+  } else {
     constexpr int LREG = DROP ? BLOCK_N / 2 : 1;
     float lacc[LREG];              // DROP: the LoRA product's own accumulator (masked in the drain)
 #pragma unroll
@@ -571,9 +661,9 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
     reg_fence<LREG>(lacc);
     wgmma_fence();
 #pragma unroll
-    for (int g = 0; g < G; ++g) {
-      const uint64_t ad = wgmma_desc(sbase + S::OFF_T + wg * (8 * 256 * G) + g * 256, 128, 256 * G, 0);
-      const uint64_t bd = wgmma_desc(sbase + S::OFF_UP + g * 256, 128, 256 * G, 0);
+    for (int kk = 0; kk < KG; ++kk) {
+      const uint64_t ad = wgmma_desc(sbase + S::OFF_T + wg * (8 * 256 * KG) + kk * 256, 128, 256 * KG, 0);
+      const uint64_t bd = wgmma_desc(sbase + S::OFF_UP + kk * 256, 128, 256 * KG, 0);
       if constexpr (DROP) wgmma_ss<BLOCK_N>(lacc, ad, bd, p.fmt);
       else wgmma_ss<BLOCK_N>(acc, ad, bd, p.fmt);
     }
@@ -692,12 +782,13 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
 }
 
 template <int BLOCK_N, int STAGES, typename OutT, bool CONV, int G, int MIN_CTAS = 1, bool DROP = false,
-          bool SPLITK = false, int CL = 1, bool INLINE_TMA = false>
+          bool SPLITK = false, int CL = 1, bool INLINE_TMA = false, int RP = R_PAD>
 __global__ void __launch_bounds__(kernel_threads<INLINE_TMA>(), MIN_CTAS)
 fused_lora_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                   const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmY,
                   const FusedParams p) {
-  fused_tile<BLOCK_N, STAGES, OutT, CONV, G, DROP, SPLITK, CL, INLINE_TMA>(tmX, tmW, tmD, tmY, p, blockIdx.x, blockIdx.y);
+  fused_tile<BLOCK_N, STAGES, OutT, CONV, G, DROP, SPLITK, CL, INLINE_TMA, RP>(tmX, tmW, tmD, tmY, p, blockIdx.x,
+                                                                             blockIdx.y);
 }
 
 // Several same-dtype linear problems in ONE launch (sites that share an input: q/k/v of an

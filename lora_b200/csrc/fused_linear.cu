@@ -16,11 +16,11 @@ static bool tmap_weight(CUtensorMap* tm, const void* W, CUtensorMapDataType dt, 
 }
 
 template <int BLOCK_N, int STAGES, typename OutT, int MIN_CTAS, bool DROP = false, bool SPLITK = false,
-          int CL = 1, bool INLINE_TMA = false>
+          int CL = 1, bool INLINE_TMA = false, int RP = R_PAD>
 static int launch_linear(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p_in,
                          int out_dtype, cudaStream_t stream, int split = 1) {
-  using S = Smem<BLOCK_N, STAGES, OutT, 1, DROP, CL>;
-  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, false, 1, MIN_CTAS, DROP, SPLITK, CL, INLINE_TMA>;
+  using S = Smem<BLOCK_N, STAGES, OutT, 1, DROP, CL, RP>;
+  auto kern = fused_lora_kernel<BLOCK_N, STAGES, OutT, false, 1, MIN_CTAS, DROP, SPLITK, CL, INLINE_TMA, RP>;
   FusedParams p = p_in;
   p.split = 1;
   if constexpr (SPLITK) {
@@ -38,7 +38,7 @@ static int launch_linear(const void* X, const void* W, const void* Dn, void* Y, 
   CUtensorMap tmX, tmW, tmD, tmY;
   if (!tmap_2d(&tmX, X, in_dt, 2, p.K, p.M, BLOCK_K, BLOCK_M, true)) return LB_ERR_TMAP;
   if (!tmap_weight(&tmW, W, in_dt, p.N, p.K, BLOCK_N, p.w_tiled)) return LB_ERR_TMAP;
-  if (!tmap_2d(&tmD, Dn, in_dt, 2, p.K, R_PAD, BLOCK_K, R_PAD, true)) return LB_ERR_TMAP;
+  if (!tmap_2d(&tmD, Dn, in_dt, 2, p.K, RP, BLOCK_K, RP, true)) return LB_ERR_TMAP;
   if (!tmap_2d(&tmY, Y, out_dt, sizeof(OutT), p.N, p.M, S::BOX_COLS, BLOCK_M, true)) return LB_ERR_TMAP;
   dim3 grid((p.N + BLOCK_N - 1) / BLOCK_N, (p.M + BLOCK_M - 1) / BLOCK_M, SPLITK ? split : CL);
   return launch_ex(kern, dim3(grid), dim3(kernel_threads<INLINE_TMA>()), S::DYN_BYTES, stream, CL, tmX, tmW, tmD, tmY,
@@ -105,6 +105,28 @@ static int launch_grouped(GroupedArgs& a, const void* const* X, const void* cons
 }
 
 
+// Ranks 17..64 (RP = 32 or 64): one tile per CTA, 64 or 128 wide, one CTA per SM. 64-wide tiles while
+// they fit one wave. Split-K, cluster split-K, inline-TMA and 192-wide plans are not built at these
+// pads: a scope choice, not a measured one. A 128-wide fp32-output dropout tile at RP = 64 does not
+// fit shared memory (accumulator + LoRA product + fp32 staging); it runs 64 wide.
+template <int RP>
+static int launch_linear_wide(const void* X, const void* W, const void* Dn, void* Y, const FusedParams& p,
+                              int out_dtype, cudaStream_t st, bool drop, bool narrow) {
+  if (out_dtype == LB_F32) {
+    if (drop) {
+      if (narrow || RP == 64) return launch_linear<64, 4, float, 1, true, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st);
+      if constexpr (RP != 64) return launch_linear<128, 4, float, 1, true, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st);
+    }
+    return narrow ? launch_linear<64, 4, float, 1, false, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st)
+                  : launch_linear<128, 4, float, 1, false, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st);
+  }
+  if (drop)
+    return narrow ? launch_linear<64, 4, uint16_t, 1, true, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st)
+                  : launch_linear<128, 4, uint16_t, 1, true, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st);
+  return narrow ? launch_linear<64, 4, uint16_t, 1, false, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st)
+                : launch_linear<128, 4, uint16_t, 1, false, false, 1, false, RP>(X, W, Dn, Y, p, out_dtype, st);
+}
+
 static int g_linear_mode = 0;
 static unsigned long long* g_dbg = nullptr;  // profiling: device buffer of 16 timestamps
 
@@ -137,16 +159,17 @@ extern "C" int lb_debug_set_stamp_buffer(void* dev_buf) {
 static int linear_fwd_impl(const void* X, const void* W, const float* bias,
                                   const void* down16, const float* up, long long up_rs,
                                   long long up_cs, const float* diag, float scale, void* Y,
-                                  float* T_out, const float* T_in, int M, int K, int N, int r,
+                                  float* T_out, const float* T_in, int M, int K, int N, int r, int r_pad,
                                   int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
                                   void* stream) {
   using namespace lb;
   const int w_tiled = (in_dtype & LB_W_TILED) ? 1 : 0;
   in_dtype &= ~LB_W_TILED;
+  if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
   if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && (seed_dev == nullptr || T_in != nullptr)))
     return LB_ERR_SHAPE;
   if (M <= 0 || N <= 0 || K <= 0) return LB_ERR_SHAPE;
-  if (r < 1 || r > R_PAD) return LB_ERR_RANK;
+  if (r < 1 || r > r_pad) return LB_ERR_RANK;
   if (in_dtype != LB_BF16 && in_dtype != LB_F16) return LB_ERR_DTYPE;
   if (out_dtype != in_dtype && out_dtype != LB_F32) return LB_ERR_DTYPE;
   // TMA: 16-byte aligned base pointers and row pitches
@@ -164,6 +187,13 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
   p.drop_p = drop_p; p.drop_inv = 1.f / (1.f - drop_p);
   p.seed = reinterpret_cast<const unsigned long long*>(seed_dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (r_pad > R_PAD) {
+    const int bn_choice = (g_linear_mode >> 2) & 3;
+    const long long tiles64 = static_cast<long long>((M + 127) / 128) * ((N + 63) / 64);
+    const bool narrow = bn_choice == 1 || (bn_choice != 2 && tiles64 <= sm_count());
+    return r_pad == 32 ? launch_linear_wide<32>(X, W, down16, Y, p, out_dtype, st, drop_p > 0.f, narrow)
+                       : launch_linear_wide<64>(X, W, down16, Y, p, out_dtype, st, drop_p > 0.f, narrow);
+  }
   if (drop_p > 0.f) {
     // Dropout on the branch: the LoRA product keeps its own accumulator and is masked in the
     // drain (fused_core.cuh, DROP). One tile per CTA; BLOCK_N 64 (2 CTAs/SM) unless the site has
@@ -261,7 +291,16 @@ extern "C" int lb_lora_linear_fwd(const void* X, const void* W, const float* bia
                                   long long up_cs, const float* diag, float scale, void* Y,
                                   float* T_out, const float* T_in, int M, int K, int N, int r,
                                   int in_dtype, int out_dtype, void* stream) {
-  return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, T_in, M, K, N, r,
+  return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, T_in, M, K, N, r, 16,
+                         in_dtype, out_dtype, 0.f, nullptr, stream);
+}
+
+extern "C" int lb_lora_linear_fwd_rp(const void* X, const void* W, const float* bias,
+                                     const void* down, const float* up, long long up_rs,
+                                     long long up_cs, const float* diag, float scale, void* Y,
+                                     float* T_out, const float* T_in, int M, int K, int N, int r, int r_pad,
+                                     int in_dtype, int out_dtype, void* stream) {
+  return linear_fwd_impl(X, W, bias, down, up, up_rs, up_cs, diag, scale, Y, T_out, T_in, M, K, N, r, r_pad,
                          in_dtype, out_dtype, 0.f, nullptr, stream);
 }
 
@@ -270,7 +309,16 @@ extern "C" int lb_lora_linear_fwd_dropout(const void* X, const void* W, const fl
                                           long long up_cs, const float* diag, float scale, void* Y,
                                           float* T_out, int M, int K, int N, int r, int in_dtype,
                                           int out_dtype, float drop_p, const void* seed_dev, void* stream) {
-  return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, nullptr, M, K, N, r,
+  return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, nullptr, M, K, N, r, 16,
+                         in_dtype, out_dtype, drop_p, seed_dev, stream);
+}
+
+extern "C" int lb_lora_linear_fwd_dropout_rp(const void* X, const void* W, const float* bias,
+                                             const void* down, const float* up, long long up_rs,
+                                             long long up_cs, const float* diag, float scale, void* Y,
+                                             float* T_out, int M, int K, int N, int r, int r_pad, int in_dtype,
+                                             int out_dtype, float drop_p, const void* seed_dev, void* stream) {
+  return linear_fwd_impl(X, W, bias, down, up, up_rs, up_cs, diag, scale, Y, T_out, nullptr, M, K, N, r, r_pad,
                          in_dtype, out_dtype, drop_p, seed_dev, stream);
 }
 

@@ -37,12 +37,13 @@ __device__ __forceinline__ float from16(uint16_t x, int fmt) {
 }
 
 // ------------------------------------------------------------------------------- wgrad
-// out[j, c] += coef_j * sum_m V[m, j] * S[m, c]   -- a [r x M] . [M x C] product with r <= 16:
+// out[j, c] += coef_j * sum_m V[m, j] * S[m, c]   -- a [r x M] . [M x C] product with r <= 64:
 // pure streaming over S (HBM/L2-bound), so the kernel is organised for memory-level parallelism:
 // CTA = 8 warps over a [64-row x 128-column] slab; a lane owns 4 adjacent columns (one 8-byte
 // load; a warp covers 256 B of a row), a warp owns 8 rows and issues all 8 row loads before the
 // first FMA. Partials are combined with shared-memory atomics, then one global atomicAdd per
-// output element per CTA.
+// output element per CTA. Ranks above 16 (RG kernels) split into 16-wide rank groups on grid z, each
+// re-reading its S slab (through L2): 64 accumulators per lane instead of 256.
 constexpr int WG_COLS = 128;
 constexpr int WG_WARPS = 8;
 constexpr int WG_RPW = 8;                    // rows per warp
@@ -50,7 +51,7 @@ constexpr int WG_ROWS = WG_WARPS * WG_RPW;   // 64 rows per CTA
 
 struct WgProblem {
   const uint2* S;      // [M, C] 16-bit rows (8-byte words)
-  const float* V;      // [M, 16] fp32
+  const float* V;      // [M, vp] fp32
   float* out;          // out[j*js + c*cs]
   long long js, cs;
   int C;
@@ -64,6 +65,7 @@ struct WgProblem {
   // pixel shifted by (dy, dx) (zero outside the image); taps > 1: blockIdx.z = filter tap t with
   // shift (dy + t/kw, dx + t%kw) and out += t. cH == 0: plain rows.
   int cH, cW, dy, dx, kw, taps;
+  int vp;              // row pitch of V (the rank pad: 16, 32 or 64)
 };
 constexpr int WG_MAXP = 24;
 struct WgArgs {
@@ -73,9 +75,10 @@ struct WgArgs {
   const unsigned long long* seed_dev;
   int M, fmt;
   int slabs;           // 64-row slabs per CTA
+  int rgroups;         // RG kernels: 16-wide rank groups per tap on grid z (grid.z = taps x rgroups)
 };
 
-template <int RQ>  // number of float4 groups of V actually used: ceil(r/4)
+template <int RQ, bool RG = false>  // RQ: float4 groups of V used: ceil(r/4); RG: r > 16, rank groups
 __global__ void __launch_bounds__(WG_WARPS * 32)
 wgrad_kernel(const WgArgs a) {
   __shared__ float red[RQ * 4][WG_COLS];
@@ -93,8 +96,10 @@ wgrad_kernel(const WgArgs a) {
   const size_t pitch = static_cast<size_t>(C) >> 2;    // row pitch in 8-byte words (16-bit rows)
   const int cH = P.cH, cW = P.cW;
   const int ntaps = (cH > 0 && P.taps > 1) ? P.taps : 1;
-  if (static_cast<int>(blockIdx.z) >= ntaps) return;     // grid.z = most taps of any problem in the launch
-  const int tap = blockIdx.z;
+  const int tap = RG ? static_cast<int>(blockIdx.z) / a.rgroups : static_cast<int>(blockIdx.z);
+  const int j0 = RG ? (static_cast<int>(blockIdx.z) % a.rgroups) * 16 : 0;   // first rank of this group
+  if (tap >= ntaps) return;     // grid.z = most taps of any problem in the launch (x rank groups)
+  if (RG && j0 >= P.r) return;
   const int sdy = P.dy + (ntaps > 1 ? tap / P.kw : 0), sdx = P.dx + (ntaps > 1 ? tap % P.kw : 0);
   for (int i = threadIdx.x; i < RQ * 4 * WG_COLS; i += WG_WARPS * 32) (&red[0][0])[i] = 0.f;
   __syncthreads();
@@ -156,7 +161,7 @@ wgrad_kernel(const WgArgs a) {
 #pragma unroll
           for (int k = 0; k < 4; ++k) x[k] = drop_keep(sd, e + k, drop_p) ? x[k] * inv : 0.f;
         }
-        const float4* vrow = reinterpret_cast<const float4*>(P.V + static_cast<size_t>(m) * 16);
+        const float4* vrow = reinterpret_cast<const float4*>(P.V + static_cast<size_t>(m) * (RG ? P.vp : 16) + j0);
 #pragma unroll
         for (int qd = 0; qd < RQ; ++qd) {
           const float4 v = __ldg(vrow + qd);
@@ -183,9 +188,9 @@ wgrad_kernel(const WgArgs a) {
   for (int idx = threadIdx.x; idx < RQ * 4 * WG_COLS; idx += WG_WARPS * 32) {
     const int j = idx / WG_COLS, c = idx % WG_COLS;
     const int cg = cblk * WG_COLS + c;
-    if (j < P.r && cg < C) {
-      const float coef = P.scale * (P.diag ? P.diag[j] : 1.f);
-      atomicAdd(P.out + j * P.js + cg * P.cs + tap, coef * red[j][c]);
+    if (j0 + j < P.r && cg < C) {
+      const float coef = P.scale * (P.diag ? P.diag[j0 + j] : 1.f);
+      atomicAdd(P.out + (j0 + j) * P.js + cg * P.cs + tap, coef * red[j][c]);
     }
   }
 }
@@ -193,7 +198,7 @@ wgrad_kernel(const WgArgs a) {
 // ------------------------------------------------------------------------------- dropout branch
 // Y[m, n] += scale/(1-p) * keep(m,n) * sum_j (T[m,j] * diag[j]) * up[n, j]     (in place)
 // one thread = 8 consecutive columns of one row (16-byte access for 16-bit Y)
-template <typename YT>
+template <typename YT, int RP = 16>   // RP: row pitch of T (the rank pad)
 __global__ void __launch_bounds__(256)
 up_dropout_kernel(YT* __restrict__ Y, int y_fmt, const float* __restrict__ T,
                   const float* __restrict__ up, long long up_rs, long long up_cs,
@@ -206,9 +211,9 @@ up_dropout_kernel(YT* __restrict__ Y, int y_fmt, const float* __restrict__ T,
   const int n0 = static_cast<int>(gid % groups) << 3;
   const unsigned long long sd = seed_dev[0];
   const float inv = scale / (1.f - drop_p);
-  float t[16];
+  float t[RP];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) t[j] = (j < r) ? T[static_cast<size_t>(m) * 16 + j] * (diag ? diag[j] : 1.f) : 0.f;
+  for (int j = 0; j < RP; ++j) t[j] = (j < r) ? T[static_cast<size_t>(m) * RP + j] * (diag ? diag[j] : 1.f) : 0.f;
   float add[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -235,14 +240,24 @@ up_dropout_kernel(YT* __restrict__ Y, int y_fmt, const float* __restrict__ T,
 // 16-byte loads, 8 pair-hashes), a warp owns 4 rows and re-uses the staged factors across them.
 // Column slabs are combined with fp32 atomics (dTs zeroed by the launcher when there are several),
 // so small-M sites (the 8x8 convs, time_emb_proj with M = 1) still spread over the chip.
+// RG kernels (r > 16): dTs has row pitch rp, grid z = 16-wide rank group (gY slab re-read through L2).
+// UP16 (RG only, p = 0, no seed): `up` is a 16-bit operand in gY's format -- T = gY . B of the wide-rank
+// 3x3 conv input gradient, from the same padded B^T [rp, N] rows the fused kernel reads.
 constexpr int DT_ROWS = 32, DT_COLS = 512;
+template <bool RG = false, bool UP16 = false>
 __global__ void __launch_bounds__(256)
 dropout_dt_kernel(const uint4* __restrict__ gY, int fmt, const float* __restrict__ up,
                   long long up_rs, long long up_cs, float drop_p,
                   const unsigned long long* __restrict__ seed_dev, float* __restrict__ dTs, int M,
-                  int N, int r, int use_atomics) {
+                  int N, int r, int use_atomics, int rp = 16) {
   __shared__ float ups[16][DT_COLS + 4];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int pitch_t = RG ? rp : 16;
+  if (RG) {   // this group's ranks [16 z, 16 z + 16): shift the factor and the output, r = ranks left
+    const int j0 = static_cast<int>(blockIdx.z) * 16;
+    up = UP16 ? reinterpret_cast<const float*>(reinterpret_cast<const uint16_t*>(up) + j0 * up_cs) : up + j0 * up_cs;
+    dTs += j0; r = r - j0 < 16 ? r - j0 : 16;
+  }
   const int n_base = blockIdx.x * DT_COLS;
   const int m_base = blockIdx.y * DT_ROWS + warp * 4;
   for (int i = threadIdx.x; i < 16 * DT_COLS; i += 256) {
@@ -250,10 +265,13 @@ dropout_dt_kernel(const uint4* __restrict__ gY, int fmt, const float* __restrict
     const int n = n_base + c;
     // column c = lane*16 + 4q + w is stored at (q*32 + lane)*4 + w: a warp's float4 reads are contiguous
     const int pos = ((((c >> 2) & 3) * 32 + (c >> 4)) << 2) + (c & 3);
-    ups[j][pos] = (j < r && n < N) ? __ldg(up + n * up_rs + j * up_cs) : 0.f;
+    if constexpr (UP16)
+      ups[j][pos] = (j < r && n < N) ? from16(reinterpret_cast<const uint16_t*>(up)[n * up_rs + j * up_cs], fmt) : 0.f;
+    else
+      ups[j][pos] = (j < r && n < N) ? __ldg(up + n * up_rs + j * up_cs) : 0.f;
   }
   __syncthreads();
-  const unsigned long long sd = seed_dev[0];
+  const unsigned long long sd = UP16 ? 0ull : seed_dev[0];
   const uint32_t s0 = static_cast<uint32_t>(sd), s1 = static_cast<uint32_t>(sd >> 32);
   const uint32_t thr = drop_threshold(drop_p);
   const float inv = 1.f / (1.f - drop_p);
@@ -295,15 +313,15 @@ dropout_dt_kernel(const uint4* __restrict__ gY, int fmt, const float* __restrict
       for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
       const int m = m_base + rr;
       if (lane == 0 && m < M) {
-        if (use_atomics) atomicAdd(dTs + static_cast<size_t>(m) * 16 + j, acc);
-        else dTs[static_cast<size_t>(m) * 16 + j] = acc;
+        if (use_atomics) atomicAdd(dTs + static_cast<size_t>(m) * pitch_t + j, acc);
+        else dTs[static_cast<size_t>(m) * pitch_t + j] = acc;
       }
     }
   }
   if (!use_atomics && lane < 16 && lane >= r) {                 // padded ranks stay zero
 #pragma unroll
     for (int rr = 0; rr < 4; ++rr)
-      if (m_base + rr < M) dTs[static_cast<size_t>(m_base + rr) * 16 + lane] = 0.f;
+      if (m_base + rr < M) dTs[static_cast<size_t>(m_base + rr) * pitch_t + lane] = 0.f;
   }
 }
 
@@ -317,17 +335,20 @@ __global__ void cast_rows_pad16_kernel(const float* __restrict__ src, long long 
   dst[static_cast<size_t>(j) * C + c] = to16(x, fmt);
 }
 
+// PADCOL: 8-column table entries whose last column is the padded row count (16, 32 or 64), else 16
+template <bool PADCOL = false>
 __global__ void refresh_shadows_kernel(const float* __restrict__ p,
                                        const long long* __restrict__ table,
                                        uint16_t* __restrict__ dst_base, int fmt) {
-  const long long* e = table + static_cast<size_t>(blockIdx.y) * 7;
+  const long long* e = table + static_cast<size_t>(blockIdx.y) * (PADCOL ? 8 : 7);
   const long long src_off = e[0], rs = e[1], cs = e[2];
   const int r = static_cast<int>(e[3]), C = static_cast<int>(e[4]);
   const long long dst_off = e[5], dst_rs = e[6];
+  const int rows = PADCOL ? static_cast<int>(e[7]) : 16;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
+#pragma unroll 16
+  for (int j = 0; j < rows; ++j) {
     const float x = (j < r) ? p[src_off + j * rs + c * cs] : 0.f;
     dst_base[dst_off + j * dst_rs + c] = to16(x, fmt);
   }
@@ -410,16 +431,16 @@ __global__ void split_bf16x3_kernel(const float* __restrict__ src, long long src
 // ------------------------------------------------------------------------------- merge / collapse
 // out[n,k] = W[n,k] + alpha * sum_j up[n,j] * down[j,k]   (lora.py:646-669; conv: flattened [Cout, Cin*kh*kw])
 // HBM-bound over W: one read + one write of the weight, the rank-r factors stay in L1/L2.
-template <typename WT>
+template <typename WT, int RMAX = 16>
 __global__ void __launch_bounds__(256)
 merge_kernel(const WT* __restrict__ W, int w_fmt, const float* __restrict__ up,
              const float* __restrict__ down, float alpha, WT* __restrict__ out, int N, int K, int r) {
   const int k = blockIdx.x * 256 + threadIdx.x;
   const int n0 = blockIdx.y * 8;
   if (k >= K) return;
-  float d[16];
+  float d[RMAX];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) d[j] = (j < r) ? __ldg(down + static_cast<size_t>(j) * K + k) : 0.f;
+  for (int j = 0; j < RMAX; ++j) d[j] = (j < r) ? __ldg(down + static_cast<size_t>(j) * K + k) : 0.f;
   for (int n = n0; n < min(N, n0 + 8); ++n) {
     float acc = 0.f;
     for (int j = 0; j < r; ++j) acc += __ldg(up + static_cast<size_t>(n) * r + j) * d[j];
@@ -573,6 +594,7 @@ __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int nbl
   __syncthreads();
 }
 
+template <bool PADCOL = false>   // shadow table format as refresh_shadows_kernel
 __global__ void __launch_bounds__(OPT_THREADS)
 optim_step_fused_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                         float* __restrict__ v, long long n, OptGroups groups,
@@ -642,13 +664,14 @@ optim_step_fused_kernel(float* __restrict__ p, float* __restrict__ g, float* __r
   {
     // one table entry per block iteration (entries have 64 ... 10240 columns: no empty work items)
     for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb) {
-      const long long* e = table + static_cast<size_t>(e_i) * 7;
+      const long long* e = table + static_cast<size_t>(e_i) * (PADCOL ? 8 : 7);
       const long long src_off = __ldg(e), rs = __ldg(e + 1), cs = __ldg(e + 2);
       const int r = static_cast<int>(__ldg(e + 3)), C = static_cast<int>(__ldg(e + 4));
       const long long dst_off = __ldg(e + 5), dst_rs = __ldg(e + 6);
+      const int rows = PADCOL ? static_cast<int>(__ldg(e + 7)) : 16;
       for (int c = threadIdx.x; c < C; c += OPT_THREADS) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
+#pragma unroll 16
+        for (int j = 0; j < rows; ++j) {
           const float x = (j < r) ? __ldcg(p + src_off + j * rs + c * cs) : 0.f;
           shadow[dst_off + j * dst_rs + c] = to16(x, fmt);
         }
@@ -866,12 +889,26 @@ ti_step_kernel(float* __restrict__ rows, float* __restrict__ grad, float* __rest
 }
 
 
+// T[m, j] = sum_c gY[m, c] * down[j, c] for j < r (16-bit gY [M, C] and down [rp, C], fp32 T [M, rp]):
+// the per-pixel T of the wide-rank conv input gradient (fused_conv.cu)
+int launch_t_from16(const void* gY, int fmt, const void* down, int C, int M, int r, int rp, float* T,
+                    cudaStream_t st) {
+  dim3 grid((C + DT_COLS - 1) / DT_COLS, (M + DT_ROWS - 1) / DT_ROWS, rp / 16);
+  const int use_atomics = grid.x > 1;
+  if (use_atomics && cudaMemsetAsync(T, 0, sizeof(float) * static_cast<size_t>(M) * rp, st) != cudaSuccess)
+    return LB_ERR_CUDA;
+  dropout_dt_kernel<true, true><<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(gY), fmt,
+                                                      reinterpret_cast<const float*>(down), 1, C, 0.f, nullptr, T,
+                                                      M, C, r, use_atomics, rp);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
 }  // namespace lb
 
 // =============================================================================== C ABI
 using namespace lb;
 
-extern "C" int lb_abi_version(void) { return 4; }
+extern "C" int lb_abi_version(void) { return 5; }
 
 extern "C" int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float scale,
                                    float* out, long long out_js, long long out_cs, int M, int C,
@@ -881,7 +918,7 @@ extern "C" int lb_lora_wgrad_masked(const void* S, const float* V, const float* 
                                     int r, float drop_p, const void* seed_dev, int in_dtype,
                                     void* stream);
 static int wgrad_launch(const void* S, const float* V, const float* diag, float scale, float* out,
-                        long long out_js, long long out_cs, int M, int C, int r, int H, int W,
+                        long long out_js, long long out_cs, int M, int C, int r, int r_pad, int H, int W,
                         int dy, int dx, float drop_p, const void* seed_dev, int in_dtype,
                         void* stream);
 
@@ -895,7 +932,22 @@ extern "C" int lb_lora_wgrad(const void* S, const float* V, const float* diag, f
 extern "C" int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float scale,
                                    float* out, long long out_js, long long out_cs, int M, int C,
                                    int r, int H, int W, int dy, int dx, int in_dtype, void* stream) {
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, H, W, dy, dx, 0.f, nullptr,
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, 16, H, W, dy, dx, 0.f, nullptr,
+                      in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_rp(const void* S, const float* V, const float* diag, float scale,
+                                float* out, long long out_js, long long out_cs, int M, int C, int r,
+                                int r_pad, int in_dtype, void* stream) {
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, 0, 0, 0, 0, 0.f, nullptr,
+                      in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_shift_rp(const void* S, const float* V, const float* diag, float scale,
+                                      float* out, long long out_js, long long out_cs, int M, int C,
+                                      int r, int r_pad, int H, int W, int dy, int dx, int in_dtype,
+                                      void* stream) {
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, H, W, dy, dx, 0.f, nullptr,
                       in_dtype, stream);
 }
 
@@ -904,22 +956,37 @@ extern "C" int lb_lora_wgrad_masked(const void* S, const float* V, const float* 
                                     int r, float drop_p, const void* seed_dev, int in_dtype,
                                     void* stream) {
   if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, 0, 0, 0, 0, drop_p, seed_dev,
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, 16, 0, 0, 0, 0, drop_p, seed_dev,
                       in_dtype, stream);
 }
+
+extern "C" int lb_lora_wgrad_masked_rp(const void* S, const float* V, const float* diag, float scale,
+                                       float* out, long long out_js, long long out_cs, int M, int C,
+                                       int r, int r_pad, float drop_p, const void* seed_dev, int in_dtype,
+                                       void* stream) {
+  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, 0, 0, 0, 0, drop_p, seed_dev,
+                      in_dtype, stream);
+}
+
+static int prob_pad(const lb_wgrad_problem&) { return 16; }
+static int prob_pad(const lb_wgrad_problem_rp& q) { return q.r_pad; }
 
 static int wgrad_run(WgArgs& a, int in_dtype, void* stream) {
   if (a.M <= 0 || a.n_pr < 1 || a.n_pr > WG_MAXP) return LB_ERR_SHAPE;
   if (in_dtype != LB_BF16 && in_dtype != LB_F16 && in_dtype != LB_F32) return LB_ERR_DTYPE;
   int nblk = 0, rmax = 0;
+  bool wide = false;   // any V pitch other than 16: the rank-group kernel (it reads the pitch)
   for (int i = 0; i < a.n_pr; ++i) {
     const WgProblem& P = a.pr[i];
-    if (P.r < 1 || P.r > 16) return LB_ERR_RANK;
+    if (P.vp != 16 && P.vp != 32 && P.vp != 64) return LB_ERR_SHAPE;
+    if (P.r < 1 || P.r > P.vp) return LB_ERR_RANK;
     if (P.C <= 0 || (P.C % 8) != 0) return LB_ERR_SHAPE;
     if ((reinterpret_cast<uintptr_t>(P.S) | reinterpret_cast<uintptr_t>(P.V)) & 15) return LB_ERR_ALIGN;
     a.nb_start[i] = nblk;
     nblk += (P.C + WG_COLS - 1) / WG_COLS;
     rmax = P.r > rmax ? P.r : rmax;
+    wide = wide || P.vp != 16;
   }
   for (int i = a.n_pr; i <= WG_MAXP; ++i) a.nb_start[i] = nblk;
   a.fmt = in_dtype == LB_BF16 ? 1 : (in_dtype == LB_F32 ? 2 : 0);
@@ -932,8 +999,14 @@ static int wgrad_run(WgArgs& a, int in_dtype, void* stream) {
   int max_taps = 1;
   for (int i = 0; i < a.n_pr; ++i)
     if (a.pr[i].cH > 0 && a.pr[i].taps > max_taps) max_taps = a.pr[i].taps;
-  dim3 grid(nblk, (slabs_total + slabs - 1) / slabs, max_taps);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (wide) {
+    a.rgroups = (rmax + 15) / 16;
+    dim3 grid(nblk, (slabs_total + slabs - 1) / slabs, max_taps * a.rgroups);
+    wgrad_kernel<4, true><<<grid, WG_WARPS * 32, 0, st>>>(a);
+    return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+  }
+  dim3 grid(nblk, (slabs_total + slabs - 1) / slabs, max_taps);
   switch ((rmax + 3) / 4) {
     case 1: wgrad_kernel<1><<<grid, WG_WARPS * 32, 0, st>>>(a); break;
     case 2: wgrad_kernel<2><<<grid, WG_WARPS * 32, 0, st>>>(a); break;
@@ -944,7 +1017,7 @@ static int wgrad_run(WgArgs& a, int in_dtype, void* stream) {
 }
 
 static int wgrad_launch(const void* S, const float* V, const float* diag, float scale, float* out,
-                        long long out_js, long long out_cs, int M, int C, int r, int H, int W,
+                        long long out_js, long long out_cs, int M, int C, int r, int r_pad, int H, int W,
                         int dy, int dx, float drop_p, const void* seed_dev, int in_dtype,
                         void* stream) {
   if (H < 0 || W < 0 || (H > 0) != (W > 0)) return LB_ERR_SHAPE;
@@ -952,7 +1025,7 @@ static int wgrad_launch(const void* S, const float* V, const float* diag, float 
   WgArgs a = {};
   a.pr[0].S = reinterpret_cast<const uint2*>(S); a.pr[0].V = V; a.pr[0].out = out;
   a.pr[0].js = out_js; a.pr[0].cs = out_cs; a.pr[0].C = C; a.pr[0].drop_p = drop_p;
-  a.pr[0].diag = diag; a.pr[0].scale = scale; a.pr[0].r = r;
+  a.pr[0].diag = diag; a.pr[0].scale = scale; a.pr[0].r = r; a.pr[0].vp = r_pad;
   a.n_pr = 1;
   a.seed_dev = reinterpret_cast<const unsigned long long*>(seed_dev);
   a.M = M; a.pr[0].cH = H; a.pr[0].cW = W; a.pr[0].dy = dy; a.pr[0].dx = dx; a.pr[0].kw = 1; a.pr[0].taps = 1;
@@ -961,17 +1034,47 @@ static int wgrad_launch(const void* S, const float* V, const float* diag, float 
 
 // All kh*kw taps of a conv down-factor gradient in one launch: tap t reads S shifted by
 // (t/kw - pad_h, t%kw - pad_w) and accumulates into out[j*out_js + c*out_cs + t].
-extern "C" int lb_lora_wgrad_conv(const void* S, const float* V, const float* diag, float scale,
-                                  float* out, int M, int C, int r, int H, int W, int kh, int kw,
-                                  int pad_h, int pad_w, int in_dtype, void* stream) {
+static int wgrad_conv_impl(const void* S, const float* V, const float* diag, float scale,
+                           float* out, int M, int C, int r, int r_pad, int H, int W, int kh, int kw,
+                           int pad_h, int pad_w, int in_dtype, void* stream) {
   if (H <= 0 || W <= 0 || kh <= 0 || kw <= 0 || (M % (H * W)) != 0) return LB_ERR_SHAPE;
   WgArgs a = {};
   const int taps = kh * kw;
   a.pr[0].S = reinterpret_cast<const uint2*>(S); a.pr[0].V = V; a.pr[0].out = out;
   a.pr[0].js = static_cast<long long>(C) * taps; a.pr[0].cs = taps; a.pr[0].C = C; a.pr[0].drop_p = 0.f;
-  a.pr[0].diag = diag; a.pr[0].scale = scale; a.pr[0].r = r;
+  a.pr[0].diag = diag; a.pr[0].scale = scale; a.pr[0].r = r; a.pr[0].vp = r_pad;
   a.n_pr = 1;
   a.M = M; a.pr[0].cH = H; a.pr[0].cW = W; a.pr[0].dy = -pad_h; a.pr[0].dx = -pad_w; a.pr[0].kw = kw; a.pr[0].taps = taps;
+  return wgrad_run(a, in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_conv(const void* S, const float* V, const float* diag, float scale,
+                                  float* out, int M, int C, int r, int H, int W, int kh, int kw,
+                                  int pad_h, int pad_w, int in_dtype, void* stream) {
+  return wgrad_conv_impl(S, V, diag, scale, out, M, C, r, 16, H, W, kh, kw, pad_h, pad_w, in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_conv_rp(const void* S, const float* V, const float* diag, float scale,
+                                     float* out, int M, int C, int r, int r_pad, int H, int W, int kh, int kw,
+                                     int pad_h, int pad_w, int in_dtype, void* stream) {
+  return wgrad_conv_impl(S, V, diag, scale, out, M, C, r, r_pad, H, W, kh, kw, pad_h, pad_w, in_dtype, stream);
+}
+
+static int wgrad_pair_impl(const void* X, const float* dTs, float* dA, long long dA_js,
+                           long long dA_cs, int K, const void* gY, const float* T, float* dB,
+                           long long dB_js, long long dB_cs, int N, const float* diag,
+                           float scale, int M, int r, int r_pad, float drop_p, const void* seed_dev,
+                           int in_dtype, void* stream) {
+  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
+  WgArgs a = {};
+  a.pr[0].S = reinterpret_cast<const uint2*>(X); a.pr[0].V = dTs; a.pr[0].out = dA;
+  a.pr[0].js = dA_js; a.pr[0].cs = dA_cs; a.pr[0].C = K; a.pr[0].drop_p = 0.f;
+  a.pr[1].S = reinterpret_cast<const uint2*>(gY); a.pr[1].V = T; a.pr[1].out = dB;
+  a.pr[1].js = dB_js; a.pr[1].cs = dB_cs; a.pr[1].C = N; a.pr[1].drop_p = drop_p;
+  for (int i = 0; i < 2; ++i) { a.pr[i].diag = diag; a.pr[i].scale = scale; a.pr[i].r = r; a.pr[i].vp = r_pad; }
+  a.n_pr = 2;
+  a.seed_dev = reinterpret_cast<const unsigned long long*>(seed_dev);
+  a.M = M;
   return wgrad_run(a, in_dtype, stream);
 }
 
@@ -980,17 +1083,17 @@ extern "C" int lb_lora_wgrad_pair(const void* X, const float* dTs, float* dA, lo
                                   long long dB_js, long long dB_cs, int N, const float* diag,
                                   float scale, int M, int r, float drop_p, const void* seed_dev,
                                   int in_dtype, void* stream) {
-  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
-  WgArgs a = {};
-  a.pr[0].S = reinterpret_cast<const uint2*>(X); a.pr[0].V = dTs; a.pr[0].out = dA;
-  a.pr[0].js = dA_js; a.pr[0].cs = dA_cs; a.pr[0].C = K; a.pr[0].drop_p = 0.f;
-  a.pr[1].S = reinterpret_cast<const uint2*>(gY); a.pr[1].V = T; a.pr[1].out = dB;
-  a.pr[1].js = dB_js; a.pr[1].cs = dB_cs; a.pr[1].C = N; a.pr[1].drop_p = drop_p;
-  for (int i = 0; i < 2; ++i) { a.pr[i].diag = diag; a.pr[i].scale = scale; a.pr[i].r = r; }
-  a.n_pr = 2;
-  a.seed_dev = reinterpret_cast<const unsigned long long*>(seed_dev);
-  a.M = M;
-  return wgrad_run(a, in_dtype, stream);
+  return wgrad_pair_impl(X, dTs, dA, dA_js, dA_cs, K, gY, T, dB, dB_js, dB_cs, N, diag, scale, M, r, 16, drop_p,
+                         seed_dev, in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_pair_rp(const void* X, const float* dTs, float* dA, long long dA_js,
+                                     long long dA_cs, int K, const void* gY, const float* T, float* dB,
+                                     long long dB_js, long long dB_cs, int N, const float* diag,
+                                     float scale, int M, int r, int r_pad, float drop_p, const void* seed_dev,
+                                     int in_dtype, void* stream) {
+  return wgrad_pair_impl(X, dTs, dA, dA_js, dA_cs, K, gY, T, dB, dB_js, dB_cs, N, diag, scale, M, r, r_pad,
+                         drop_p, seed_dev, in_dtype, stream);
 }
 
 // dA and dB of up to 4 sites that share X (a grouped family) in one launch. HOST arrays of length n.
@@ -1009,6 +1112,7 @@ extern "C" int lb_lora_wgrad_multi(int n, const void* X, const float* const* dTs
     pa.diag = pb.diag = diag ? diag[i] : nullptr;
     pa.scale = pb.scale = scale[i];
     pa.r = pb.r = r[i];
+    pa.vp = pb.vp = 16;
   }
   a.n_pr = 2 * n;
   a.M = M;
@@ -1019,20 +1123,22 @@ extern "C" int lb_lora_wgrad_multi(int n, const void* X, const float* const* dTs
 // possible (24 problems per launch): the dA / dB of EVERY linear site of a step, queued during
 // backward and flushed once at its end -- they feed only the optimizer, and one launch over
 // hundreds of MB fills the chip where 120-270 launches over a few MB each were latency-bound.
-extern "C" int lb_lora_wgrad_batch(const lb_wgrad_problem* probs, int n, int in_dtype, void* stream) {
+template <typename Prob>
+static int wgrad_batch_impl(const Prob* probs, int n, int in_dtype, void* stream) {
   if (probs == nullptr || n < 1) return LB_ERR_SHAPE;
   for (int base = 0; base < n; base += WG_MAXP) {
     const int cnt = (n - base) < WG_MAXP ? (n - base) : WG_MAXP;
     WgArgs a = {};
     int max_m = 0;
     for (int i = 0; i < cnt; ++i) {
-      const lb_wgrad_problem& q = probs[base + i];
+      const Prob& q = probs[base + i];
       if (q.M <= 0 || !(q.drop_p >= 0.f && q.drop_p < 1.f) || (q.drop_p > 0.f && q.seed_dev == nullptr))
         return LB_ERR_SHAPE;
       WgProblem& w = a.pr[i];
       w.S = reinterpret_cast<const uint2*>(q.S); w.V = q.V; w.out = q.out; w.js = q.out_js; w.cs = q.out_cs;
       w.C = q.C; w.drop_p = q.drop_p; w.diag = q.diag; w.scale = q.scale; w.r = q.r; w.M = q.M;
       w.seed = reinterpret_cast<const unsigned long long*>(q.seed_dev);
+      w.vp = prob_pad(q);
       if (q.conv_H > 0) {       // conv lora_down weight-gradient: all taps of one site as one problem
         if (q.conv_W <= 0 || q.kh <= 0 || q.kw <= 0 || (q.M % (q.conv_H * q.conv_W)) != 0) return LB_ERR_SHAPE;
         w.cH = q.conv_H; w.cW = q.conv_W; w.dy = -q.pad_h; w.dx = -q.pad_w; w.kw = q.kw; w.taps = q.kh * q.kw;
@@ -1045,6 +1151,44 @@ extern "C" int lb_lora_wgrad_batch(const lb_wgrad_problem* probs, int n, int in_
     if (rc != LB_OK) return rc;
   }
   return LB_OK;
+}
+
+extern "C" int lb_lora_wgrad_batch(const lb_wgrad_problem* probs, int n, int in_dtype, void* stream) {
+  return wgrad_batch_impl(probs, n, in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_batch_rp(const lb_wgrad_problem_rp* probs, int n, int in_dtype, void* stream) {
+  return wgrad_batch_impl(probs, n, in_dtype, stream);
+}
+
+template <int RP>
+static void up_dropout_launch(void* Y, int y_dtype, const float* T, const float* up, long long up_rs,
+                              long long up_cs, const float* diag, float scale, float drop_p,
+                              const unsigned long long* sd, int M, int N, int r, int blocks, cudaStream_t st) {
+  if (y_dtype == LB_F32)
+    up_dropout_kernel<float, RP><<<blocks, 256, 0, st>>>(reinterpret_cast<float*>(Y), 0, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r);
+  else
+    up_dropout_kernel<uint16_t, RP><<<blocks, 256, 0, st>>>(reinterpret_cast<uint16_t*>(Y), y_dtype == LB_BF16, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r);
+}
+
+extern "C" int lb_lora_up_dropout_rp(void* Y, int y_dtype, const float* T, const float* up,
+                                     long long up_rs, long long up_cs, const float* diag, float scale,
+                                     float drop_p, const void* seed_dev, int M, int N, int r, int r_pad,
+                                     void* stream) {
+  if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
+  if (M <= 0 || N <= 0 || (N % 8) != 0) return LB_ERR_SHAPE;
+  if (r < 1 || r > r_pad) return LB_ERR_RANK;
+  if (!(drop_p >= 0.f && drop_p < 1.f) || seed_dev == nullptr) return LB_ERR_SHAPE;
+  if (reinterpret_cast<uintptr_t>(Y) & 15) return LB_ERR_ALIGN;
+  if (y_dtype != LB_F32 && y_dtype != LB_BF16 && y_dtype != LB_F16) return LB_ERR_DTYPE;
+  const long long threads = static_cast<long long>(M) * (N / 8);
+  const int blocks = static_cast<int>((threads + 255) / 256);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const unsigned long long* sd = reinterpret_cast<const unsigned long long*>(seed_dev);
+  if (r_pad == 16) up_dropout_launch<16>(Y, y_dtype, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r, blocks, st);
+  else if (r_pad == 32) up_dropout_launch<32>(Y, y_dtype, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r, blocks, st);
+  else up_dropout_launch<64>(Y, y_dtype, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r, blocks, st);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
 extern "C" int lb_lora_up_dropout(void* Y, int y_dtype, const float* T, const float* up,
@@ -1087,6 +1231,27 @@ extern "C" int lb_lora_dropout_dt(const void* gY, int in_dtype, const float* up,
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
+extern "C" int lb_lora_dropout_dt_rp(const void* gY, int in_dtype, const float* up, long long up_rs,
+                                     long long up_cs, float drop_p, const void* seed_dev, float* dTs,
+                                     int M, int N, int r, int r_pad, void* stream) {
+  if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
+  if (r_pad == 16) return lb_lora_dropout_dt(gY, in_dtype, up, up_rs, up_cs, drop_p, seed_dev, dTs, M, N, r, stream);
+  if (M <= 0 || N <= 0 || (N % 8) != 0) return LB_ERR_SHAPE;
+  if (r < 1 || r > r_pad) return LB_ERR_RANK;
+  if (in_dtype != LB_BF16 && in_dtype != LB_F16) return LB_ERR_DTYPE;
+  if (!(drop_p >= 0.f && drop_p < 1.f) || seed_dev == nullptr) return LB_ERR_SHAPE;
+  if (reinterpret_cast<uintptr_t>(gY) & 15) return LB_ERR_ALIGN;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  dim3 grid((N + DT_COLS - 1) / DT_COLS, (M + DT_ROWS - 1) / DT_ROWS, r_pad / 16);
+  const int use_atomics = grid.x > 1;
+  if (use_atomics && cudaMemsetAsync(dTs, 0, sizeof(float) * static_cast<size_t>(M) * r_pad, st) != cudaSuccess)
+    return LB_ERR_CUDA;
+  dropout_dt_kernel<true><<<grid, 256, 0, st>>>(
+      reinterpret_cast<const uint4*>(gY), in_dtype == LB_BF16, up, up_rs, up_cs, drop_p,
+      reinterpret_cast<const unsigned long long*>(seed_dev), dTs, M, N, r, use_atomics, r_pad);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
 extern "C" int lb_cast_rows_pad16(const float* src, long long src_rs, long long src_cs,
                                   void* dst16, int r, int C, int out_dtype, void* stream) {
   if (C <= 0) return LB_ERR_SHAPE;
@@ -1098,12 +1263,34 @@ extern "C" int lb_cast_rows_pad16(const float* src, long long src_rs, long long 
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
+extern "C" int lb_cast_rows_pad16_rp(const float* src, long long src_rs, long long src_cs,
+                                     void* dst16, int r, int r_pad, int C, int out_dtype, void* stream) {
+  if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
+  if (C <= 0) return LB_ERR_SHAPE;
+  if (r < 1 || r > r_pad) return LB_ERR_RANK;
+  if (out_dtype != LB_BF16 && out_dtype != LB_F16) return LB_ERR_DTYPE;
+  dim3 grid((C + 255) / 256, r_pad);
+  cast_rows_pad16_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      src, src_rs, src_cs, reinterpret_cast<uint16_t*>(dst16), r, C, out_dtype == LB_BF16);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
 extern "C" int lb_refresh_shadows(const float* p, const long long* table, int n_entries,
                                   int max_C, void* dst16_base, int out_dtype, void* stream) {
   if (n_entries <= 0 || max_C <= 0) return LB_ERR_SHAPE;
   if (out_dtype != LB_BF16 && out_dtype != LB_F16) return LB_ERR_DTYPE;
   dim3 grid((max_C + 255) / 256, n_entries);
   refresh_shadows_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      p, table, reinterpret_cast<uint16_t*>(dst16_base), out_dtype == LB_BF16);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_refresh_shadows_rp(const float* p, const long long* table, int n_entries,
+                                     int max_C, void* dst16_base, int out_dtype, void* stream) {
+  if (n_entries <= 0 || max_C <= 0) return LB_ERR_SHAPE;
+  if (out_dtype != LB_BF16 && out_dtype != LB_F16) return LB_ERR_DTYPE;
+  dim3 grid((max_C + 255) / 256, n_entries);
+  refresh_shadows_kernel<true><<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       p, table, reinterpret_cast<uint16_t*>(dst16_base), out_dtype == LB_BF16);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
@@ -1168,15 +1355,22 @@ extern "C" int lb_ti_embed_step(float* rows, float* grad, float* m, float* v, co
 extern "C" int lb_lora_merge(const void* W, int w_dtype, const float* up, const float* down, float alpha,
                              void* out, int N, int K, int r, void* stream) {
   if (N <= 0 || K <= 0) return LB_ERR_SHAPE;
-  if (r < 1 || r > 16) return LB_ERR_RANK;
+  if (r < 1 || r > 64) return LB_ERR_RANK;
+  if (w_dtype != LB_F32 && w_dtype != LB_BF16 && w_dtype != LB_F16) return LB_ERR_DTYPE;
   dim3 grid((K + 255) / 256, (N + 7) / 8);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (w_dtype == LB_F32)
-    merge_kernel<float><<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(W), 0, up, down, alpha, reinterpret_cast<float*>(out), N, K, r);
-  else if (w_dtype == LB_BF16 || w_dtype == LB_F16)
-    merge_kernel<uint16_t><<<grid, 256, 0, st>>>(reinterpret_cast<const uint16_t*>(W), w_dtype == LB_BF16, up, down, alpha, reinterpret_cast<uint16_t*>(out), N, K, r);
-  else
-    return LB_ERR_DTYPE;
+  const int wf = w_dtype == LB_BF16;
+  float* o32 = reinterpret_cast<float*>(out);
+  uint16_t* o16 = reinterpret_cast<uint16_t*>(out);
+  const float* w32 = reinterpret_cast<const float*>(W);
+  const uint16_t* w16 = reinterpret_cast<const uint16_t*>(W);
+  if (r <= 16) {
+    if (w_dtype == LB_F32) merge_kernel<float><<<grid, 256, 0, st>>>(w32, 0, up, down, alpha, o32, N, K, r);
+    else merge_kernel<uint16_t><<<grid, 256, 0, st>>>(w16, wf, up, down, alpha, o16, N, K, r);
+  } else {   // ranks 17..64 (joined or wide LoRAs)
+    if (w_dtype == LB_F32) merge_kernel<float, 64><<<grid, 256, 0, st>>>(w32, 0, up, down, alpha, o32, N, K, r);
+    else merge_kernel<uint16_t, 64><<<grid, 256, 0, st>>>(w16, wf, up, down, alpha, o16, N, K, r);
+  }
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
@@ -1234,13 +1428,14 @@ extern "C" int lb_adamw_clip_step(float* p, float* g, float* m, float* v, long l
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
-extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
-                                   const long long* group_off, int n_groups, const float* lr_dev,
-                                   float beta1, float beta2, float eps, float weight_decay,
-                                   float max_norm, float inv_world, int* step_dev, float* partials,
-                                   float* gnorm_out, const long long* table, int n_entries, int max_C,
-                                   void* shadow16, int shadow_dtype, unsigned int* barrier2,
-                                   void* stream) {
+template <bool PADCOL>
+static int optim_step_fused_impl(float* p, float* g, float* m, float* v, long long n,
+                                 const long long* group_off, int n_groups, const float* lr_dev,
+                                 float beta1, float beta2, float eps, float weight_decay,
+                                 float max_norm, float inv_world, int* step_dev, float* partials,
+                                 float* gnorm_out, const long long* table, int n_entries, int max_C,
+                                 void* shadow16, int shadow_dtype, unsigned int* barrier2,
+                                 void* stream) {
   if (n <= 0 || n_groups < 1 || n_groups > OPT_MAX_GROUPS) return LB_ERR_SHAPE;
   if (reinterpret_cast<uintptr_t>(g) & 15) return LB_ERR_ALIGN;
   if (n_entries > 0 && (table == nullptr || shadow16 == nullptr || max_C <= 0)) return LB_ERR_SHAPE;
@@ -1269,10 +1464,34 @@ extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long 
   cfg.numAttrs = 1;
   const int fmt = shadow_dtype == LB_BF16;
   uint16_t* sh = reinterpret_cast<uint16_t*>(shadow16);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, optim_step_fused_kernel, p, g, m, v, n, groups, lr_dev, beta1, beta2,
-                                     eps, weight_decay, max_norm, inv_world, step_dev, partials, gnorm_out,
+  cudaError_t e = cudaLaunchKernelEx(&cfg, optim_step_fused_kernel<PADCOL>, p, g, m, v, n, groups, lr_dev, beta1,
+                                     beta2, eps, weight_decay, max_norm, inv_world, step_dev, partials, gnorm_out,
                                      table, n_entries, max_C, sh, fmt, barrier2);
   return e == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
+                                   const long long* group_off, int n_groups, const float* lr_dev,
+                                   float beta1, float beta2, float eps, float weight_decay,
+                                   float max_norm, float inv_world, int* step_dev, float* partials,
+                                   float* gnorm_out, const long long* table, int n_entries, int max_C,
+                                   void* shadow16, int shadow_dtype, unsigned int* barrier2,
+                                   void* stream) {
+  return optim_step_fused_impl<false>(p, g, m, v, n, group_off, n_groups, lr_dev, beta1, beta2, eps, weight_decay,
+                                      max_norm, inv_world, step_dev, partials, gnorm_out, table, n_entries, max_C,
+                                      shadow16, shadow_dtype, barrier2, stream);
+}
+
+extern "C" int lb_optim_step_fused_rp(float* p, float* g, float* m, float* v, long long n,
+                                      const long long* group_off, int n_groups, const float* lr_dev,
+                                      float beta1, float beta2, float eps, float weight_decay,
+                                      float max_norm, float inv_world, int* step_dev, float* partials,
+                                      float* gnorm_out, const long long* table, int n_entries, int max_C,
+                                      void* shadow16, int shadow_dtype, unsigned int* barrier2,
+                                      void* stream) {
+  return optim_step_fused_impl<true>(p, g, m, v, n, group_off, n_groups, lr_dev, beta1, beta2, eps, weight_decay,
+                                     max_norm, inv_world, step_dev, partials, gnorm_out, table, n_entries, max_C,
+                                     shadow16, shadow_dtype, barrier2, stream);
 }
 
 // ------------------------------------------------------------------------------- CUDA IPC helpers

@@ -119,8 +119,8 @@ class _SiteState:
     def __init__(self):
         self.w = {}        # dtype -> (key, w16, wt16)
         self.bias = None   # (key, bias fp32)
-        self.down = {}     # dtype -> (key, down16 [16,K])
-        self.upT = {}      # dtype -> (key, upT16 [16,N])
+        self.down = {}     # dtype -> (key, down16 [RP,K]), RP = ops.rank_pad(r)
+        self.upT = {}      # dtype -> (key, upT16 [RP,N])
         self.grad_sink = None  # (gA view, gB view) when the arena owns the gradients
         self.parent = None     # weakref to the module this site was injected into (grouping.py)
 
@@ -138,7 +138,7 @@ class _SiteState:
     def frozen(self, weight2d: torch.Tensor, dtype, need_t: bool, tiled: Optional[bool] = None):
         """16-bit copies of the frozen weight: (W [N,K], W^T [K,N] or None), row-major tensors -- or, with
         ops.TILED_WEIGHTS (opt-in, LB_TILED_W=1), ops.TiledWeight in contiguous
-        64 x 64 blocks. tiled=False forces row-major (row slicing: the rank > 16 chunks)."""
+        64 x 64 blocks. tiled=False forces row-major (row slicing: the rank > 64 chunks)."""
         tiled = ops.TILED_WEIGHTS if tiled is None else tiled
         k = _key(weight2d)
         slot = (dtype, "tiled") if tiled else dtype
@@ -175,7 +175,7 @@ class _SiteState:
         return self.bias[1]
 
     def down16(self, a2d: torch.Tensor, dtype):
-        """A [r,K] fp32 master -> [16,K] 16-bit."""
+        """A [r,K] fp32 master -> [RP,K] 16-bit, rows r.. zero (RP = ops.rank_pad(r))."""
         k = _key(a2d)
         ent = self.down.get(dtype)
         if ent is None or ent[0] != k:
@@ -187,7 +187,7 @@ class _SiteState:
         return ent[1]
 
     def upT16(self, b2d: torch.Tensor, dtype):
-        """B [N,r] fp32 master -> B^T [16,N] 16-bit."""
+        """B [N,r] fp32 master -> B^T [RP,N] 16-bit, rows r.. zero."""
         k = _key(b2d)
         ent = self.upT.get(dtype)
         if ent is None or ent[0] != k:
@@ -315,7 +315,7 @@ class LoraInjectedLinear(nn.Module):
         return torch.diagonal(w.reshape(self.r, self.r)).to(torch.float32).contiguous()
 
     def forward(self, input):
-        if self.r > 16:        # joined LoRAs (lora_manager.py:13-71): rank chunks of 16
+        if self.r > ops.MAX_RANK:   # joined LoRAs above rank 64 (lora_manager.py:13-71): rank chunks of 64
             from .rank_chunks import lora_linear_chunked
             return lora_linear_chunked(self, input)
         if self.training and self.dropout.p > 0.0:

@@ -13,7 +13,15 @@ from . import _C
 from ._C import check, dtype_code, ptr, stream_ptr
 
 R_PAD = 16
+MAX_RANK = 64      # widest rank the fused kernels run natively (rank pads 16, 32, 64)
 LAUNCH_COUNT = 0  # kernels of liblora_b200.so enqueued through this process (bench.py reads it)
+
+
+def rank_pad(r: int) -> int:
+    """Rows of the zero-padded rank operands for a rank-r site: 16, 32 or 64 (r <= 64)."""
+    if not 1 <= r <= MAX_RANK:
+        raise _C.LoraB200Error(f"LoRA rank {r} outside 1..{MAX_RANK} of the fused kernels")
+    return 16 if r <= 16 else (32 if r <= 32 else 64)
 
 
 def _count(n: int = 1):
@@ -37,6 +45,10 @@ class _WgProblemC(_ct.Structure):
                 ("pad_h", _ct.c_int), ("pad_w", _ct.c_int)]
 
 
+class _WgProblemRpC(_ct.Structure):
+    _fields_ = _WgProblemC._fields_ + [("r_pad", _ct.c_int)]
+
+
 _WG_QUEUE = None      # None: launch immediately; dict dtype -> [(_WgProblemC fields, keepalive)]
 WG_BATCH = 24
 
@@ -52,8 +64,13 @@ def wgrad_defer_cancel():
 
 
 def _wgrad_launch(dtype, items):
-    arr = (_WgProblemC * len(items))(*[_WgProblemC(*it[0]) for it in items])
-    check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
+    if all(it[0][-1] == R_PAD for it in items):
+        arr = (_WgProblemC * len(items))(*[_WgProblemC(*it[0][:-1]) for it in items])
+        check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
+    else:
+        arr = (_WgProblemRpC * len(items))(*[_WgProblemRpC(*it[0]) for it in items])
+        check(_C.lib.lb_lora_wgrad_batch_rp(arr, len(items), dtype_code(dtype), stream_ptr()),
+              "lb_lora_wgrad_batch_rp")
     n = (len(items) + WG_BATCH - 1) // WG_BATCH
     _count(n)
     return n
@@ -62,7 +79,8 @@ def _wgrad_launch(dtype, items):
 def _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag, drop_p=0.0, seed=None, conv=None):
     dp = lambda t: None if t is None else t.data_ptr()
     item = (dp(S), dp(V), dp(out), int(out_js), int(out_cs), int(M), int(C), int(r), float(scale), dp(diag),
-            float(drop_p), dp(seed)) + (tuple(int(v) for v in conv) if conv is not None else (0, 0, 0, 0, 0, 0))
+            float(drop_p), dp(seed)) + (tuple(int(v) for v in conv) if conv is not None else (0, 0, 0, 0, 0, 0)) + (
+            int(V.shape[1]),)
     _WG_QUEUE.setdefault(S.dtype, []).append((item, (S, V, out, diag, seed)))
 
 
@@ -86,11 +104,16 @@ def _req_cuda(*ts):
 
 
 def cast_rows_pad16(src: torch.Tensor, rs: int, cs: int, r: int, C: int, dtype) -> torch.Tensor:
-    """fp32 factor -> zero-padded 16-bit [16, C] operand (see lb_cast_rows_pad16)."""
+    """fp32 factor -> zero-padded 16-bit [rank_pad(r), C] operand (see lb_cast_rows_pad16[_rp])."""
     _req_cuda(src)
-    out = torch.empty((R_PAD, C), device=src.device, dtype=dtype)
-    check(_C.lib.lb_cast_rows_pad16(ptr(src), rs, cs, ptr(out), r, C, dtype_code(dtype),
-                                    stream_ptr()), "lb_cast_rows_pad16")
+    rp = rank_pad(r) if r >= 1 else R_PAD
+    out = torch.empty((rp, C), device=src.device, dtype=dtype)
+    if rp == R_PAD:
+        check(_C.lib.lb_cast_rows_pad16(ptr(src), rs, cs, ptr(out), r, C, dtype_code(dtype),
+                                        stream_ptr()), "lb_cast_rows_pad16")
+    else:
+        check(_C.lib.lb_cast_rows_pad16_rp(ptr(src), rs, cs, ptr(out), r, rp, C, dtype_code(dtype),
+                                           stream_ptr()), "lb_cast_rows_pad16_rp")
     _count()
     return out
 
@@ -166,15 +189,33 @@ def fused_linear(x2d: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tens
                  seed: Optional[torch.Tensor] = None
                  ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """Y = x2d.w16^T + bias + ((x2d.down16^T) * scale*diag) . up^T ; returns (Y, T or None).
-    t_in: use these rank-r activations [M,16] instead of x2d.down16^T (dropout backward).
+    down16: [RP, K] with RP = 16, 32 or 64 rows (the rank pad); T is [M, RP].
+    t_in: use these rank-r activations [M,RP] instead of x2d.down16^T (dropout backward).
     drop_p > 0 (+ seed: int64[1] on the device): nn.Dropout on the branch, masked in the drain."""
     _req_cuda(x2d, down16, up)
     M, K = x2d.shape
     wp, N, wflag = _w_arg(w16, K)
-    assert down16.shape == (R_PAD, K)
+    rp = down16.shape[0]
+    assert down16.shape == (rp, K) and rp in (16, 32, 64)
     assert x2d.is_contiguous() and down16.is_contiguous()
     y = torch.empty((M, N), device=x2d.device, dtype=out_dtype)
-    t = torch.empty((M, R_PAD), device=x2d.device, dtype=torch.float32) if want_t else None
+    t = torch.empty((M, rp), device=x2d.device, dtype=torch.float32) if want_t else None
+    if rp != R_PAD:
+        assert t_in is None or t_in.shape == (M, rp)
+        if drop_p > 0.0:
+            assert t_in is None and seed is not None and seed.dtype == torch.int64 and seed.is_cuda
+            check(_C.lib.lb_lora_linear_fwd_dropout_rp(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up), up_rs, up_cs,
+                                                       ptr(diag), float(scale), ptr(y), ptr(t), M, K, N, r, rp,
+                                                       dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype),
+                                                       float(drop_p), ptr(seed), stream_ptr()),
+                  "lb_lora_linear_fwd_dropout_rp")
+        else:
+            check(_C.lib.lb_lora_linear_fwd_rp(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up), up_rs, up_cs, ptr(diag),
+                                               float(scale), ptr(y), ptr(t), ptr(t_in), M, K, N, r, rp,
+                                               dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype), stream_ptr()),
+                  "lb_lora_linear_fwd_rp")
+        _count()
+        return y, t
     if drop_p > 0.0:
         assert t_in is None and seed is not None and seed.dtype == torch.int64 and seed.is_cuda
         check(_C.lib.lb_lora_linear_fwd_dropout(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up),
@@ -197,13 +238,18 @@ def wgrad(S: torch.Tensor, V: torch.Tensor, diag: Optional[torch.Tensor], scale:
     """out[j*out_js + c*out_cs] += scale*diag[j] * sum_m V[m,j]*S[m,c]."""
     _req_cuda(S, V, out)
     M, C = S.shape
-    assert S.is_contiguous() and V.shape == (M, R_PAD) and V.dtype == torch.float32
+    rp = V.shape[1]
+    assert S.is_contiguous() and V.shape == (M, rp) and V.dtype == torch.float32
     assert out.dtype == torch.float32
     if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag)
         return
-    check(_C.lib.lb_lora_wgrad(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
-                               M, C, r, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad")
+    if rp == R_PAD:
+        check(_C.lib.lb_lora_wgrad(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
+                                   M, C, r, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad")
+    else:
+        check(_C.lib.lb_lora_wgrad_rp(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
+                                      M, C, r, rp, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad_rp")
     _count()
 
 
@@ -225,22 +271,24 @@ def cast_conv_weight(w: torch.Tensor, dtype, want_fwd: bool, want_bwd: bool):
 
 
 def conv_down16(a4d: torch.Tensor, dtype, table_cache: dict) -> torch.Tensor:
-    """A [r,Cin,kh,kw] fp32 -> [16, kh*kw*Cin] 16-bit with K ordered tap-major, channel-minor."""
+    """A [r,Cin,kh,kw] fp32 -> [rank_pad(r), kh*kw*Cin] 16-bit with K ordered tap-major, channel-minor."""
     _req_cuda(a4d)
     r, cin, kh, kw = a4d.shape
     taps = kh * kw
+    rp = rank_pad(r)
     key = (r, cin, taps, a4d.device)
     tab = table_cache.get(key)
     if tab is None:
-        rows = [(t, cin * taps, taps, r, cin, t * cin, taps * cin) for t in range(taps)]
+        rows = [(t, cin * taps, taps, r, cin, t * cin, taps * cin) + ((rp,) if rp != R_PAD else ())
+                for t in range(taps)]
         tab = torch.tensor(rows, device=a4d.device, dtype=torch.int64)
         table_cache[key] = tab
     src = a4d.detach()
     if src.dtype != torch.float32 or not src.is_contiguous():
         src = src.float().contiguous()
-    out = torch.empty((R_PAD, taps * cin), device=a4d.device, dtype=dtype)
-    check(_C.lib.lb_refresh_shadows(ptr(src), ptr(tab), taps, cin, ptr(out), dtype_code(dtype),
-                                    stream_ptr()), "lb_refresh_shadows")
+    out = torch.empty((rp, taps * cin), device=a4d.device, dtype=dtype)
+    refresh = _C.lib.lb_refresh_shadows if rp == R_PAD else _C.lib.lb_refresh_shadows_rp
+    check(refresh(ptr(src), ptr(tab), taps, cin, ptr(out), dtype_code(dtype), stream_ptr()), "lb_refresh_shadows")
     _count()
     return out
 
@@ -253,15 +301,32 @@ def fused_conv2d(x_nhwc: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.T
                  seed: Optional[torch.Tensor] = None
                  ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """x_nhwc: a [N,C,H,W] tensor in channels_last memory format (NHWC bytes). Returns
-    (Y as [N,cout,H,W] channels_last, T [N*H*W,16] or None)."""
+    (Y as [N,cout,H,W] channels_last, T [N*H*W,RP] or None); RP = down16.shape[0] (16, 32 or 64)."""
     _req_cuda(x_nhwc, w16, down16, up)
     n, cin, h, w = x_nhwc.shape
-    assert x_nhwc.is_contiguous(memory_format=torch.channels_last)
+    rp = down16.shape[0]
+    assert x_nhwc.is_contiguous(memory_format=torch.channels_last) and rp in (16, 32, 64)
     y = torch.empty((n, cout, h, w), device=x_nhwc.device, dtype=out_dtype,
                     memory_format=torch.channels_last)
-    t = torch.empty((n * h * w, R_PAD), device=x_nhwc.device, dtype=torch.float32) if want_t else None
+    t = torch.empty((n * h * w, rp), device=x_nhwc.device, dtype=torch.float32) if want_t else None
     import ctypes
     up_ptr = ctypes.c_void_p(up.data_ptr() + 4 * up_off)
+    if rp != R_PAD:
+        if drop_p > 0.0:
+            assert t_in is None and not per_tap and up_gs == 0 and seed is not None and seed.dtype == torch.int64
+            check(_C.lib.lb_lora_conv2d_fwd_dropout_rp(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
+                                                       up_cs, ptr(diag), float(scale), ptr(y), ptr(t), n, h, w, cin,
+                                                       cout, kh, kw, pad_h, pad_w, r, rp, dtype_code(x_nhwc.dtype),
+                                                       dtype_code(out_dtype), float(drop_p), ptr(seed), stream_ptr()),
+                  "lb_lora_conv2d_fwd_dropout_rp")
+        else:
+            check(_C.lib.lb_lora_conv2d_fwd_rp(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs, up_cs,
+                                               up_gs, ptr(diag), float(scale), ptr(y), ptr(t), ptr(t_in), n, h, w,
+                                               cin, cout, kh, kw, pad_h, pad_w, r, rp, 1 if per_tap else 0,
+                                               dtype_code(x_nhwc.dtype), dtype_code(out_dtype), stream_ptr()),
+                  "lb_lora_conv2d_fwd_rp")
+        _count()
+        return y, t
     if drop_p > 0.0:     # forward with nn.Dropout on the branch: masked in the drain, one launch
         assert t_in is None and not per_tap and up_gs == 0 and seed is not None and seed.dtype == torch.int64
         check(_C.lib.lb_lora_conv2d_fwd_dropout(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
@@ -301,22 +366,34 @@ def up_dropout_(y2d: torch.Tensor, T: torch.Tensor, up: torch.Tensor, up_rs: int
     """y2d[m,n] += scale/(1-p) * keep(m,n) * sum_j T[m,j] diag[j] up[n,j]   (in place)."""
     _req_cuda(y2d, T, up, seed)
     M, N = y2d.shape
+    rp = T.shape[1]
     assert y2d.is_contiguous() and seed.dtype == torch.int64
-    check(_C.lib.lb_lora_up_dropout(ptr(y2d), dtype_code(y2d.dtype), ptr(T), ptr(up), up_rs, up_cs,
-                                    ptr(diag), float(scale), float(p), ptr(seed), M, N, r,
-                                    stream_ptr()), "lb_lora_up_dropout")
+    if rp == R_PAD:
+        check(_C.lib.lb_lora_up_dropout(ptr(y2d), dtype_code(y2d.dtype), ptr(T), ptr(up), up_rs, up_cs,
+                                        ptr(diag), float(scale), float(p), ptr(seed), M, N, r,
+                                        stream_ptr()), "lb_lora_up_dropout")
+    else:
+        check(_C.lib.lb_lora_up_dropout_rp(ptr(y2d), dtype_code(y2d.dtype), ptr(T), ptr(up), up_rs, up_cs,
+                                           ptr(diag), float(scale), float(p), ptr(seed), M, N, r, rp,
+                                           stream_ptr()), "lb_lora_up_dropout_rp")
     _count()
 
 
 def dropout_dt(gy2d: torch.Tensor, up: torch.Tensor, up_rs: int, up_cs: int, p: float,
                seed: torch.Tensor, r: int) -> torch.Tensor:
-    """dTs[m,j] = sum_n keep(m,n)/(1-p) * gY[m,n] * up[n,j]  (fp32 [M,16])."""
+    """dTs[m,j] = sum_n keep(m,n)/(1-p) * gY[m,n] * up[n,j]  (fp32 [M,rank_pad(r)])."""
     _req_cuda(gy2d, up, seed)
     M, N = gy2d.shape
-    out = torch.empty((M, R_PAD), device=gy2d.device, dtype=torch.float32)
-    check(_C.lib.lb_lora_dropout_dt(ptr(gy2d), dtype_code(gy2d.dtype), ptr(up), up_rs, up_cs,
-                                    float(p), ptr(seed), ptr(out), M, N, r, stream_ptr()),
-          "lb_lora_dropout_dt")
+    rp = rank_pad(r)
+    out = torch.empty((M, rp), device=gy2d.device, dtype=torch.float32)
+    if rp == R_PAD:
+        check(_C.lib.lb_lora_dropout_dt(ptr(gy2d), dtype_code(gy2d.dtype), ptr(up), up_rs, up_cs,
+                                        float(p), ptr(seed), ptr(out), M, N, r, stream_ptr()),
+              "lb_lora_dropout_dt")
+    else:
+        check(_C.lib.lb_lora_dropout_dt_rp(ptr(gy2d), dtype_code(gy2d.dtype), ptr(up), up_rs, up_cs,
+                                           float(p), ptr(seed), ptr(out), M, N, r, rp, stream_ptr()),
+              "lb_lora_dropout_dt_rp")
     _count()
     return out
 
@@ -328,9 +405,15 @@ def wgrad_masked(S: torch.Tensor, V: torch.Tensor, diag, scale: float, out: torc
     if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag, p, seed)
         return
-    check(_C.lib.lb_lora_wgrad_masked(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
-                                      out_cs, M, C, r, float(p), ptr(seed), dtype_code(S.dtype),
-                                      stream_ptr()), "lb_lora_wgrad_masked")
+    rp = V.shape[1]
+    if rp == R_PAD:
+        check(_C.lib.lb_lora_wgrad_masked(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
+                                          out_cs, M, C, r, float(p), ptr(seed), dtype_code(S.dtype),
+                                          stream_ptr()), "lb_lora_wgrad_masked")
+    else:
+        check(_C.lib.lb_lora_wgrad_masked_rp(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
+                                             out_cs, M, C, r, rp, float(p), ptr(seed), dtype_code(S.dtype),
+                                             stream_ptr()), "lb_lora_wgrad_masked_rp")
     _count()
 
 
@@ -346,9 +429,16 @@ def wgrad_pair(x2d: torch.Tensor, dTs: torch.Tensor, dA: torch.Tensor, gy2d: tor
         _wgrad_enqueue(x2d, dTs, dA, K, 1, M, K, r, scale, diag)
         _wgrad_enqueue(gy2d, T, dB, 1, r, M, N, r, scale, diag, p, seed)
         return
-    check(_C.lib.lb_lora_wgrad_pair(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
-                                    1, r, N, ptr(diag), float(scale), M, r, float(p), ptr(seed),
-                                    dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair")
+    rp = dTs.shape[1]
+    assert T.shape[1] == rp
+    if rp == R_PAD:
+        check(_C.lib.lb_lora_wgrad_pair(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
+                                        1, r, N, ptr(diag), float(scale), M, r, float(p), ptr(seed),
+                                        dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair")
+    else:
+        check(_C.lib.lb_lora_wgrad_pair_rp(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
+                                           1, r, N, ptr(diag), float(scale), M, r, rp, float(p), ptr(seed),
+                                           dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair_rp")
     _count()
 
 
@@ -374,6 +464,12 @@ def fused_linear_grouped(problems, out_dtype, want_t: bool):
     import ctypes
     n = len(problems)
     assert 1 <= n <= 4
+    if any(p[3].shape[0] != R_PAD for p in problems):
+        # the grouped kernel is built for rank pad 16 only (grouping.py groups only r <= 16 sites);
+        # other callers with wider problems (bench.py's kernel sweep at --rank 32) get one launch each
+        outs = [fused_linear(x, w, b, d, up, rs, cs, diag, sc, r, out_dtype, want_t)
+                for (x, w, b, d, up, rs, cs, diag, sc, r) in problems]
+        return [o[0] for o in outs], [o[1] for o in outs]
     VP, LL, I, F = ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_float
     ys, ts = [], []
     tiled = isinstance(problems[0][1], TiledWeight)
@@ -440,7 +536,13 @@ def wgrad_conv(x_nhwc_rows: torch.Tensor, V: torch.Tensor, diag, scale: float, o
         _wgrad_enqueue(x_nhwc_rows, V, out, C * kh * kw, kh * kw, M, C, r, scale, diag,
                        conv=(H, W, kh, kw, pad_h, pad_w))
         return
-    check(_C.lib.lb_lora_wgrad_conv(ptr(x_nhwc_rows), ptr(V), ptr(diag), float(scale), ptr(out), M, C, r,
-                                    H, W, kh, kw, pad_h, pad_w, dtype_code(x_nhwc_rows.dtype), stream_ptr()),
-          "lb_lora_wgrad_conv")
+    rp = V.shape[1]
+    if rp == R_PAD:
+        check(_C.lib.lb_lora_wgrad_conv(ptr(x_nhwc_rows), ptr(V), ptr(diag), float(scale), ptr(out), M, C, r,
+                                        H, W, kh, kw, pad_h, pad_w, dtype_code(x_nhwc_rows.dtype), stream_ptr()),
+              "lb_lora_wgrad_conv")
+    else:
+        check(_C.lib.lb_lora_wgrad_conv_rp(ptr(x_nhwc_rows), ptr(V), ptr(diag), float(scale), ptr(out), M, C, r,
+                                           rp, H, W, kh, kw, pad_h, pad_w, dtype_code(x_nhwc_rows.dtype),
+                                           stream_ptr()), "lb_lora_wgrad_conv_rp")
     _count()

@@ -29,7 +29,7 @@ def collapse_lora(model, alpha=1.0):
         holder = site.linear if is_lin else site.conv
         print("Collapsing Lin Lora in" if is_lin else "Collapsing Conv Lora in", name)
         w = holder.weight.data
-        if w.is_cuda and site.r <= 16 and w.dtype in (torch.float32, torch.bfloat16, torch.float16):
+        if w.is_cuda and site.r <= 64 and w.dtype in (torch.float32, torch.bfloat16, torch.float16):
             from . import ops   # one HBM pass over W (lb_lora_merge) instead of GEMM + cast + add
             holder.weight = nn.Parameter(ops.merge_lora(w, site.lora_up.weight.data.to(w.device),
                                                         site.lora_down.weight.data.to(w.device), alpha))

@@ -19,8 +19,6 @@ from . import _C, ops
 from ._C import LoraB200Error, check, ptr, stream_ptr
 from .modules import _SiteState, _fp32_master, _key
 
-R_PAD = 16
-
 
 def _split(src2d: torch.Tensor, pattern: int, rows_pad: int = 0) -> torch.Tensor:
     """fp32 [R,C] -> bf16 [max(R, rows_pad), 3C] (extra rows zero)."""
@@ -60,7 +58,7 @@ class _PreciseLoraLinearFn(torch.autograd.Function):
         need_bwd = any(ctx.needs_input_grad[:3])
         w3, _ = _frozen3(st, lin.weight, False)
         b32 = st.bias32(lin.bias)
-        down3 = _split(A, 1, rows_pad=R_PAD)
+        down3 = _split(A, 1, rows_pad=ops.rank_pad(r))
         diag = mod._selector_diag()
         scale = float(mod.scale)
         y, T = ops.fused_linear(_split(x2d, 0), w3, b32, down3, _fp32_master(B), r, 1, diag, scale, r,
@@ -80,7 +78,7 @@ class _PreciseLoraLinearFn(torch.autograd.Function):
         if not gy2d.is_contiguous():
             gy2d = gy2d.contiguous()
         _, wt3 = _frozen3(st, lin.weight, True)
-        upT3 = _split(_fp32_master(B).t().contiguous(), 1, rows_pad=R_PAD)       # B^T [r,N] -> [16,3N]
+        upT3 = _split(_fp32_master(B).t().contiguous(), 1, rows_pad=ops.rank_pad(r))   # B^T [r,N] -> [RP,3N]
         dX, dTs = ops.fused_linear(_split(gy2d, 0), wt3, None, upT3, _fp32_master(A), 1, K, ctx.diag,
                                    ctx.scale, r, torch.float32, True)
         need_x, need_a, need_b = ctx.needs_input_grad[:3]

@@ -1,6 +1,6 @@
-"""LoRA ranks above 16 on a linear site (a `lora_join` of two rank-16 files is rank 32,
-lora_diffusion/lora_manager.py:13-71): the fused kernel carries one 16-wide rank group per launch
-(the rank axis rides the K loop as 16 extra operand rows), so wider ranks run as rank chunks:
+"""LoRA ranks above 64 on a linear site (a `lora_join` of wide files adds their ranks,
+lora_diffusion/lora_manager.py:13-71): the fused kernel carries at most 64 ranks per launch
+(the rank axis rides the K loop as up to 64 extra operand rows), so wider ranks run as rank chunks:
 
     chunk 0     the ordinary fused launch  y = x W^T + b + s (x A_0^T d_0) B_0^T
     chunk c>0   T_c = x A_c^T from the same kernel on an 8-row slice of the frozen weight (its output is
@@ -9,7 +9,7 @@ lora_diffusion/lora_manager.py:13-71): the fused kernel carries one 16-wide rank
 
 and the mirror image in backward (dX chunks accumulate in place; dA_c / dB_c through lb_lora_wgrad on
 views of the gradient tensors). Every extra chunk re-reads x once: correct, not fast -- ranks above
-16 are an inference-time artefact of joined files, the training configurations use r <= 16.
+64 are an inference-time artefact of joined files.
 """
 import torch
 
@@ -17,7 +17,7 @@ from . import ops
 from ._C import LoraB200Error
 from .modules import _LOW, _SiteState, _compute_dtype, _fp32_master, _out_dtype
 
-CH = 16
+CH = 64
 
 
 def _chunks(r):
@@ -30,7 +30,7 @@ class _ChunkedLoraLinearFn(torch.autograd.Function):
         if not x.is_cuda:
             raise LoraB200Error("LoraInjectedLinear.forward: lora_b200 runs on CUDA tensors only")
         if mod.training and mod.dropout.p > 0.0:
-            raise LoraB200Error("LoRA rank > 16 with active dropout is not supported (train with r <= 16, "
+            raise LoraB200Error("LoRA rank > 64 with active dropout is not supported (train with r <= 64, "
                                 "or call .eval() / set dropout.p = 0 on joined LoRAs)")
         st: _SiteState = mod._lb
         lin = mod.linear
@@ -86,7 +86,7 @@ class _ChunkedLoraLinearFn(torch.autograd.Function):
         dX = None
         for c, (j0, j1) in enumerate(_chunks(r)):
             rc = j1 - j0
-            bt16 = ops.cast_rows_pad16(B32[:, j0:], 1, r, rc, N, cdt)          # B_c^T padded [16, N]
+            bt16 = ops.cast_rows_pad16(B32[:, j0:], 1, r, rc, N, cdt)          # B_c^T padded [RP, N]
             dg = None if ctx.diag is None else ctx.diag[j0:j1].contiguous()
             if c == 0:
                 dX, dT = ops.fused_linear(gy2d, wt16, None, bt16, A32[j0:], 1, K, dg, ctx.scale, rc, dx_dtype, True)
