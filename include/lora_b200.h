@@ -11,10 +11,12 @@
  *   - "16-bit" operands are bf16 (LB_BF16) or fp16 (LB_F16), chosen per call by in_dtype.
  *   - LoRA master factors are fp32:   down A[r,K] row-major,   up B[N,r] row-major
  *     (reference: lora_down.weight / lora_up.weight, lora_diffusion/lora.py:44-46).
- *   - "down16" operands are 16-bit copies zero-padded to 16 rows: [16,K] row-major
- *     (built by lb_cast_rows_pad16). Rank r <= 16 on these entry points; ranks up to 64 use the
- *     "_rp" entry points at the end of this header, with 32 or 64 padded rows.
- *   - T buffers are fp32 [M,16] row-major (the "_rp" entries: [M,r_pad]), columns >= r are zero.
+ *   - Rank pad: entry points whose operands hold the rank take `r_pad` (16, 32 or 64) right after
+ *     `r`, with 1 <= r <= r_pad <= 64. "down" operands are 16-bit copies zero-padded to r_pad
+ *     rows: [r_pad,K] row-major (built by lb_cast_rows_pad). T / dT / V buffers are fp32
+ *     [M,r_pad] row-major, columns >= r are zero. r_pad outside {16, 32, 64}: LB_ERR_SHAPE;
+ *     r > r_pad: LB_ERR_RANK (both before any CUDA call). The grouped entry points
+ *     (lb_lora_linear_fwd_grouped, lb_lora_wgrad_multi) take r <= 16 at a pad of 16 only.
  *   - All base pointers 16-byte aligned; K % 8 == 0; N % 8 == 0 (N % 4 for fp32 outputs).
  */
 #ifndef LORA_B200_H
@@ -27,7 +29,7 @@ extern "C" {
 enum lb_status {
   LB_OK = 0,
   LB_ERR_SHAPE = -1, /* unsupported / misaligned extent */
-  LB_ERR_RANK = -2,  /* r outside [1,16] (the "_rp" entry points: [1,r_pad]) */
+  LB_ERR_RANK = -2,  /* r outside [1,r_pad] */
   LB_ERR_DTYPE = -3,
   LB_ERR_ALIGN = -4, /* pointer not 16-byte aligned */
   LB_ERR_TMAP = -5,  /* cuTensorMapEncodeTiled unavailable or failed */
@@ -46,41 +48,42 @@ enum lb_dtype { LB_BF16 = 0, LB_F16 = 1, LB_F32 = 2 };
 int lb_abi_version(void);
 
 /* Fused frozen linear + LoRA forward (wgmma/TMA), one launch:
- *     Y[M,N] = X[M,K] . W[N,K]^T (+ bias[N]) + ((X . down16^T) * (scale * diag)) . up^T
+ *     Y[M,N] = X[M,K] . W[N,K]^T (+ bias[N]) + ((X . down^T) * (scale * diag)) . up^T
  * up element (n, j) is read from the fp32 master at up[n*up_rs + j*up_cs]; diag is the optional
- * selector diagonal [r] (NULL = identity); T_out (NULL = skip) receives X . down16^T (unscaled);
- * T_in (normally NULL): when given, the rank-r activations are read from this fp32 [M,16] buffer
+ * selector diagonal [r] (NULL = identity); T_out (NULL = skip) receives X . down^T (unscaled);
+ * T_in (normally NULL): when given, the rank-r activations are read from this fp32 [M,r_pad] buffer
  * instead of being computed (dropout path: T = (mask o gY) . B comes from lb_lora_dropout_dt).
+ * At r_pad > 16 only one-tile-per-CTA plans run (no split-K).
  * Replaces LoraInjectedLinear.forward, lora_diffusion/lora.py:53-58 (F.linear + lora_down +
  * selector + lora_up + scale + add), dropout handled by the caller (see INTEGRATION.md).
  *
  * The SAME entry point is the backward-dX kernel: with W := W^T[K,N] (pre-transposed frozen
- * weight), down16 := B^T padded [16,N], up := A read transposed (up_rs = 1, up_cs = K) it returns
+ * weight), down := B^T padded [r_pad,N], up := A read transposed (up_rs = 1, up_cs = K) it returns
  *     dX[M,K] = gY . W + ((gY . B) * (scale * diag)) . A       and  T_out = gY . B.
  */
-int lb_lora_linear_fwd(const void* X, const void* W, const float* bias, const void* down16,
+int lb_lora_linear_fwd(const void* X, const void* W, const float* bias, const void* down,
                        const float* up, long long up_rs, long long up_cs, const float* diag,
                        float scale, void* Y, float* T_out, const float* T_in, int M, int K, int N,
-                       int r, int in_dtype, int out_dtype, void* stream);
+                       int r, int r_pad, int in_dtype, int out_dtype, void* stream);
 
 /* lb_lora_linear_fwd with an ACTIVE nn.Dropout(p) on the LoRA branch (lora.py:45,56: module in
  * training mode, p > 0 -- the state of every site built by inject_trainable_lora_extended and the
  * monkeypatch_* loaders), still ONE launch:
- *     Y = X . W^T (+ bias) + keep(m,n)/(1-p) * (((X . down16^T) * (scale * diag)) . up^T)[m,n]
+ *     Y = X . W^T (+ bias) + keep(m,n)/(1-p) * (((X . down^T) * (scale * diag)) . up^T)[m,n]
  * The LoRA product keeps its own accumulator and the keep-mask (csrc/dropmask.cuh: a counter hash
  * of (*seed_dev, m*N + n); seed_dev points to one uint64 in DEVICE memory so that a captured graph
  * draws a new mask per replay) is applied while the tile is drained. Backward recomputes the same
  * mask: lb_lora_dropout_dt, lb_lora_wgrad_masked / lb_lora_wgrad_pair(drop_p). */
-int lb_lora_linear_fwd_dropout(const void* X, const void* W, const float* bias, const void* down16,
+int lb_lora_linear_fwd_dropout(const void* X, const void* W, const float* bias, const void* down,
                                const float* up, long long up_rs, long long up_cs, const float* diag,
                                float scale, void* Y, float* T_out, int M, int K, int N, int r,
-                               int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                               void* stream);
+                               int r_pad, int in_dtype, int out_dtype, float drop_p,
+                               const void* seed_dev, void* stream);
 
 /* Up to 4 independent lb_lora_linear_fwd problems of the same operand/output dtype in ONE launch
  * (sites that share an input -- q/k/v of a self-attention, k/v of a cross-attention, CLIP's k/v/q --
  * each under-fill 132 SMs on their own). All array arguments are HOST arrays of length n; per-problem
- * semantics are exactly lb_lora_linear_fwd's (T_in unsupported). */
+ * semantics are exactly lb_lora_linear_fwd's at r_pad = 16 (r <= 16; T_in unsupported). */
 int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W,
                                const float* const* bias, const void* const* down16,
                                const float* const* up, const long long* up_rs, const long long* up_cs,
@@ -107,12 +110,13 @@ int lb_debug_set_pdl(int on);
 /* Skinny weight-gradient reduction (streams S once, fp32 atomics into out):
  *     out[j*out_js + c*out_cs] += scale * diag[j] * sum_m V[m,j] * S[m,c]     j < r, c < C
  * S may also be fp32 (in_dtype = LB_F32; the fp32-faithful mode keeps X and gY in fp32).
+ * V is fp32 [M, r_pad]; ranks above 16 run as 16-wide rank groups, each re-reading S.
  * dA[r,K]: S = X[M,K],  V = gY.B (T_out of the dX call), out_js = K, out_cs = 1
  * dB[N,r]: S = gY[M,N], V = X.A^T (T_out of the forward), out_js = 1, out_cs = r
  * Replaces the autograd-generated dA/dB GEMMs of lora.py:53-58 (W frozen: no dW).
  */
 int lb_lora_wgrad(const void* S, const float* V, const float* diag, float scale, float* out,
-                  long long out_js, long long out_cs, int M, int C, int r, int in_dtype,
+                  long long out_js, long long out_cs, int M, int C, int r, int r_pad, int in_dtype,
                   void* stream);
 
 /* Both factor gradients of one linear site in ONE launch (the two reductions are independent):
@@ -122,13 +126,13 @@ int lb_lora_wgrad(const void* S, const float* V, const float* diag, float scale,
 int lb_lora_wgrad_pair(const void* X, const float* dTs, float* dA, long long dA_js, long long dA_cs,
                        int K, const void* gY, const float* T, float* dB, long long dB_js,
                        long long dB_cs, int N, const float* diag, float scale, int M, int r,
-                       float drop_p, const void* seed_dev, int in_dtype, void* stream);
+                       int r_pad, float drop_p, const void* seed_dev, int in_dtype, void* stream);
 
 /* One reduction  out[j*out_js + c*out_cs] += scale*diag[j] * sum_{m<M} V[m,j] * S[m,c]  (see
  * lb_lora_wgrad; drop_p > 0: S masked like lb_lora_wgrad_masked with the uint64 at seed_dev). */
 typedef struct lb_wgrad_problem {
   const void* S;        /* [M, C] rows of in_dtype                         */
-  const float* V;       /* [M, 16] fp32                                    */
+  const float* V;       /* [M, r_pad] fp32                                 */
   float* out;
   long long out_js, out_cs;
   int M, C, r;
@@ -141,6 +145,7 @@ typedef struct lb_wgrad_problem {
    * shifted by (ty - pad_h, tx - pad_w), out = dA[r, C, kh, kw] flat with out_js = C*kh*kw,
    * out_cs = kh*kw (+ tap). 0: plain rows. */
   int conv_H, conv_W, kh, kw, pad_h, pad_w;
+  int r_pad;
 } lb_wgrad_problem;
 
 /* n independent reductions (HOST array) in ceil(n/24) launches. The step engine queues the dA / dB
@@ -148,21 +153,12 @@ typedef struct lb_wgrad_problem {
  * the optimizer (autograd's dA/dB GEMMs of lora.py:53-58 for all sites at once). */
 int lb_lora_wgrad_batch(const lb_wgrad_problem* probs, int n, int in_dtype, void* stream);
 
-/* lb_lora_wgrad_pair for up to 4 sites that share X (a grouped family), one launch; HOST arrays. */
+/* lb_lora_wgrad_pair for up to 4 sites that share X (a grouped family), one launch; HOST arrays.
+ * r <= 16, dTs / T at a pad of 16. */
 int lb_lora_wgrad_multi(int n, const void* X, const float* const* dTs, float* const* dA,
                         const void* const* gY, const float* const* T, float* const* dB, const int* N,
                         const float* const* diag, const float* scale, const int* r, int M, int K,
                         int in_dtype, void* stream);
-
-/* Conv tap of the same reduction: rows of S are the pixels of NHWC images [M/(H*W), H, W, C]; S is
- * read at pixel (h+dy, w+dx), zero outside the image (the convolution's zero padding):
- *     out[...] += scale * diag[j] * sum_p V[p,j] * S[p shifted by (dy,dx), c]
- * dA[r,Cin,kh,kw] of a LoraInjectedConv2d: one call per tap t = (ty,tx) with dy = ty - pad_h,
- * dx = tx - pad_w, out = dA + t, out_js = Cin*kh*kw, out_cs = kh*kw, V = gY.B (per pixel).
- * H = W = 0 degenerates to lb_lora_wgrad. Replaces the lora_down wgrad of lora.py:130-135. */
-int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float scale, float* out,
-                        long long out_js, long long out_cs, int M, int C, int r, int H, int W,
-                        int dy, int dx, int in_dtype, void* stream);
 
 /* ---- dropout on the LoRA branch (nn.Dropout inside the operator, lora.py:45,56,115,133; active
  * only when module.training and p > 0). keep(m,n) is a counter-based hash of (*seed_dev, m*N+n),
@@ -173,52 +169,59 @@ int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float 
 /* Y[m,n] += scale/(1-p) * keep(m,n) * sum_j T[m,j]*diag[j]*up[n*up_rs + j*up_cs]   (in place) */
 int lb_lora_up_dropout(void* Y, int y_dtype, const float* T, const float* up, long long up_rs,
                        long long up_cs, const float* diag, float scale, float drop_p,
-                       const void* seed_dev, int M, int N, int r, void* stream);
-/* dTs[m,j] = sum_n keep(m,n)/(1-p) * gY[m,n] * up[n*up_rs + j*up_cs]    (fp32 [M,16]) */
+                       const void* seed_dev, int M, int N, int r, int r_pad, void* stream);
+/* dTs[m,j] = sum_n keep(m,n)/(1-p) * gY[m,n] * up[n*up_rs + j*up_cs]    (fp32 [M,r_pad]) */
 int lb_lora_dropout_dt(const void* gY, int in_dtype, const float* up, long long up_rs,
                        long long up_cs, float drop_p, const void* seed_dev, float* dTs, int M, int N,
-                       int r, void* stream);
+                       int r, int r_pad, void* stream);
 /* lb_lora_wgrad with S := keep o S / (1-p)  (S = gY [M,C], mask index m*C + c) */
 int lb_lora_wgrad_masked(const void* S, const float* V, const float* diag, float scale, float* out,
-                         long long out_js, long long out_cs, int M, int C, int r, float drop_p,
-                         const void* seed_dev, int in_dtype, void* stream);
+                         long long out_js, long long out_cs, int M, int C, int r, int r_pad,
+                         float drop_p, const void* seed_dev, int in_dtype, void* stream);
 
-/* dA[r,Cin,kh,kw] of a LoraInjectedConv2d in ONE launch (all taps; equals kh*kw calls of
- * lb_lora_wgrad_shift): S = X NHWC rows [M = n_img*H*W, C = Cin], V = gY.B per pixel [M,16]. */
+/* dA[r,Cin,kh,kw] of a LoraInjectedConv2d in ONE launch, the lora_down wgrad of lora.py:130-135:
+ * rows of S are the pixels of NHWC images [M = n_img*H*W, C = Cin]; tap t = (ty,tx) reads S at pixel
+ * (h + ty - pad_h, w + tx - pad_w), zero outside the image (the convolution's zero padding), and
+ * accumulates into dA[j, c, ty, tx]. V = gY.B per pixel [M,r_pad]. */
 int lb_lora_wgrad_conv(const void* S, const float* V, const float* diag, float scale, float* out, int M,
-                       int C, int r, int H, int W, int kh, int kw, int pad_h, int pad_w, int in_dtype,
-                       void* stream);
+                       int C, int r, int r_pad, int H, int W, int kh, int kw, int pad_h, int pad_w,
+                       int in_dtype, void* stream);
 
 /* Fused frozen Conv2d + LoRA (NHWC implicit GEMM on wgmma; stride 1, dilation 1, groups 1,
  * 1x1 or 3x3 "same" padding -- the ResnetBlock2D sites of SD1.5):
  *     Y[n,h,w,:] = sum_tap X[n,h+ty-pad,w+tx-pad,:] . W[:, tap, :]^T (+ bias)
- *                  + ((sum_tap X[..] . down16[:, tap, :]^T) * (scale*diag)) . up^T
+ *                  + ((sum_tap X[..] . down[:, tap, :]^T) * (scale*diag)) . up^T
  * X: NHWC 16-bit [n_img,H,W,Cin]; W: 16-bit [Cout, kh*kw*Cin] with K ordered tap-major,
- * channel-minor (built once from the frozen [Cout,Cin,kh,kw] weight); down16: [16, kh*kw*Cin] in
+ * channel-minor (built once from the frozen [Cout,Cin,kh,kw] weight); down: [r_pad, kh*kw*Cin] in
  * the same K order; up element (n, j) at up[n*up_rs + j*up_cs]; Y: NHWC [n_img,H,W,Cout];
- * T_out: fp32 [n_img*H*W, 16] = the rank-r activations (unscaled).
+ * T_out: fp32 [n_img*H*W, r_pad] = the rank-r activations (unscaled).
+ * At r_pad > 16 only one-tile-per-CTA plans run (no split-K).
  * Replaces LoraInjectedConv2d.forward, lora_diffusion/lora.py:130-135.
  *
  * per_tap_T = 1 is the input-gradient form (dX = conv_T(gY, W) + conv_T((gY.B)*s*d, A)): call it
  * with X := gY [n_img,H,W,Cout'], W := the flipped+transposed frozen weight [Cin', taps*Cout'],
- * down16 := B^T padded [16, Cout'] (restarts every tap), up := A read flipped:
+ * down := B^T padded [r_pad, Cout'] (restarts every tap), up := A read flipped:
  * element (c, tap g, j) at up[c*up_rs + j*up_cs + g*up_gs] (up_gs = -1 from the last tap).
- * T_out then receives gY.B of the unshifted tap. */
-int lb_lora_conv2d_fwd(const void* X, const void* W, const float* bias, const void* down16,
+ * T_out then receives gY.B of the unshifted tap. At r_pad > 16 a 3x3 input gradient reads its
+ * per-tap T from T_in; without T_in it first writes T_out = X . down^T (one more launch, so T_out
+ * is required) and reads that. T_in and T_out together are refused there. */
+int lb_lora_conv2d_fwd(const void* X, const void* W, const float* bias, const void* down,
                        const float* up, long long up_rs, long long up_cs, long long up_gs,
                        const float* diag, float scale, void* Y, float* T_out, const float* T_in,
                        int n_img, int H, int Wd, int Cin, int Cout, int kh, int kw, int pad_h,
-                       int pad_w, int r, int per_tap_T, int in_dtype, int out_dtype, void* stream);
+                       int pad_w, int r, int r_pad, int per_tap_T, int in_dtype, int out_dtype,
+                       void* stream);
 
 /* lb_lora_conv2d_fwd (forward direction) with an active nn.Dropout(p) on the LoRA branch
  * (lora.py:115,133; every conv site of inject_trainable_lora_extended): one launch, mask applied in
  * the drain exactly as in lb_lora_linear_fwd_dropout; mask index = pixel * Cout + n with
  * pixel = (img*H + h)*W + w. */
-int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias, const void* down16,
+int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias, const void* down,
                                const float* up, long long up_rs, long long up_cs, const float* diag,
                                float scale, void* Y, float* T_out, int n_img, int H, int Wd, int Cin,
-                               int Cout, int kh, int kw, int pad_h, int pad_w, int r, int in_dtype,
-                               int out_dtype, float drop_p, const void* seed_dev, void* stream);
+                               int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
+                               int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
+                               void* stream);
 
 /* Frozen conv-weight preparation: src [Cout,Cin,kh,kw] (LB_F32/LB_BF16/LB_F16) ->
  *   dst16  [Cout, kh*kw*Cin]  (tap-major K; forward operand)              and/or
@@ -226,10 +229,10 @@ int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias, 
 int lb_cast_conv_weight(const void* src, int src_dtype, void* dst16, void* dstT16, int Cout,
                         int Cin, int kh, int kw, int out_dtype, void* stream);
 
-/* dst16[j, c] = (j < r) ? src[j*src_rs + c*src_cs] : 0   for j < 16, c < C  (16-bit, [16,C]).
- * A[r,K] -> down16:  src_rs = K, src_cs = 1.    B[N,r] -> B^T padded: src_rs = 1, src_cs = r. */
-int lb_cast_rows_pad16(const float* src, long long src_rs, long long src_cs, void* dst16, int r,
-                       int C, int out_dtype, void* stream);
+/* dst16[j, c] = (j < r) ? src[j*src_rs + c*src_cs] : 0   for j < r_pad, c < C  (16-bit, [r_pad,C]).
+ * A[r,K] -> down:  src_rs = K, src_cs = 1.    B[N,r] -> B^T padded: src_rs = 1, src_cs = r. */
+int lb_cast_rows_pad(const float* src, long long src_rs, long long src_cs, void* dst16, int r,
+                     int r_pad, int C, int out_dtype, void* stream);
 
 /* Pivotal-tuning phase 1 (textual inversion) update of the n trained token rows, one launch:
  * AdamW on rows [n,D] (fp32 masters; grad is zeroed), t = ++(*step_dev), then, if clip_decay,
@@ -285,7 +288,7 @@ int lb_adamw_clip_step(float* p, float* g, float* m, float* v, long long n,
                        int* step_dev, float* partials, float* gnorm_out, void* stream);
 
 /* The whole optimizer step in ONE cooperative launch: lb_adamw_clip_step's two passes plus
- * lb_refresh_shadows (the re-cast of every LoRA factor into the 16-bit [16, C] operands of the
+ * lb_refresh_shadows (the re-cast of every LoRA factor into the 16-bit [rows, C] operands of the
  * fused kernels; `table` = the rows lb_refresh_shadows walks, n_entries may be 0), separated by
  * grid barriers on `barrier2` (2 x uint32 of device memory, zero-initialised once by the caller).
  * train_lora_dreambooth.py:878-888 (clip_grad_norm_, optimizer.step, zero_grad). */
@@ -321,10 +324,13 @@ int lb_optim_step_dp(float* p, float* g, float* gsum, float* m, float* v, long l
 int lb_ipc_export(const void* ptr, void* handle64, long long* offset);
 int lb_ipc_open(const void* handle64, void** base_out);
 
-/* Batched 16-bit shadow refresh after an optimizer step: for every table entry e, j < 16, c < e.C
+/* Batched 16-bit shadow refresh after an optimizer step: for every table entry e, j < e.rows, c < e.C
  *   dst16_base[e.dst_off + j*e.dst_rs + c] = (j < e.r) ? p[e.src_off + j*e.src_rs + c*e.src_cs] : 0
- * table: DEVICE array of n_entries x 7 long long {src_off, src_rs, src_cs, r, C, dst_off, dst_rs}.
- * (conv down factors use one entry per filter tap so that K is ordered tap-major, channel-minor) */
+ * table: DEVICE array of n_entries x 8 long long {src_off, src_rs, src_cs, r, C, dst_off, dst_rs, rows}
+ * (conv down factors use one entry per filter tap so that K is ordered tap-major, channel-minor).
+ * The table is not checked: `rows` must be 16, 32 or 64, r <= rows, and the destination slot must
+ * hold `rows` rows of pitch dst_rs (rows * dst_rs elements from dst_off) -- a larger `rows` writes
+ * past the slot. lb_optim_step_fused and lb_optim_step_dp walk the same table. */
 int lb_refresh_shadows(const float* p, const long long* table, int n_entries, int max_C,
                        void* dst16_base, int out_dtype, void* stream);
 
@@ -390,89 +396,6 @@ int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long stride_b, 
                           long long stride_p, const float* target, const float* mask,
                           const float* weights, void* grad, float* loss, float* partials64,
                           unsigned int* counter, int B, int C, int H, int W, void* stream);
-
-/* ---- LoRA ranks 17..64: the "_rp" siblings of the entry points whose operand layout holds the rank
- * pad. Each takes `r_pad` (16, 32 or 64; r <= r_pad) right after `r`: the down / up-transposed operands
- * are [r_pad, K] / [r_pad, N] 16-bit with rows r.. zero, and every T / dT / V operand is [M, r_pad] fp32.
- * With r_pad = 16 they compute what the entry points without the suffix compute, which keep
- * accepting r <= 16 only. r_pad outside {16, 32, 64}: LB_ERR_SHAPE; r > r_pad: LB_ERR_RANK (both
- * before any CUDA call). At r_pad > 16 the fused kernels run one tile per CTA (no split-K plans), and
- * the 3x3 conv input gradient (per_tap_T = 1) reads its per-tap T from T_in; without T_in it first
- * writes T_out = X . down^T (one more launch, so T_out is required) and reads that. T_in and T_out
- * together are refused there. */
-int lb_lora_linear_fwd_rp(const void* X, const void* W, const float* bias, const void* down,
-                          const float* up, long long up_rs, long long up_cs, const float* diag,
-                          float scale, void* Y, float* T_out, const float* T_in, int M, int K, int N,
-                          int r, int r_pad, int in_dtype, int out_dtype, void* stream);
-int lb_lora_linear_fwd_dropout_rp(const void* X, const void* W, const float* bias, const void* down,
-                                  const float* up, long long up_rs, long long up_cs, const float* diag,
-                                  float scale, void* Y, float* T_out, int M, int K, int N, int r, int r_pad,
-                                  int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                                  void* stream);
-int lb_lora_conv2d_fwd_rp(const void* X, const void* W, const float* bias, const void* down,
-                          const float* up, long long up_rs, long long up_cs, long long up_gs,
-                          const float* diag, float scale, void* Y, float* T_out, const float* T_in,
-                          int n_img, int H, int Wd, int Cin, int Cout, int kh, int kw, int pad_h,
-                          int pad_w, int r, int r_pad, int per_tap_T, int in_dtype, int out_dtype,
-                          void* stream);
-int lb_lora_conv2d_fwd_dropout_rp(const void* X, const void* W, const float* bias, const void* down,
-                                  const float* up, long long up_rs, long long up_cs, const float* diag,
-                                  float scale, void* Y, float* T_out, int n_img, int H, int Wd, int Cin,
-                                  int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
-                                  int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                                  void* stream);
-int lb_lora_wgrad_rp(const void* S, const float* V, const float* diag, float scale, float* out,
-                     long long out_js, long long out_cs, int M, int C, int r, int r_pad, int in_dtype,
-                     void* stream);
-int lb_lora_wgrad_shift_rp(const void* S, const float* V, const float* diag, float scale, float* out,
-                           long long out_js, long long out_cs, int M, int C, int r, int r_pad, int H,
-                           int W, int dy, int dx, int in_dtype, void* stream);
-int lb_lora_wgrad_masked_rp(const void* S, const float* V, const float* diag, float scale, float* out,
-                            long long out_js, long long out_cs, int M, int C, int r, int r_pad,
-                            float drop_p, const void* seed_dev, int in_dtype, void* stream);
-int lb_lora_wgrad_conv_rp(const void* S, const float* V, const float* diag, float scale, float* out,
-                          int M, int C, int r, int r_pad, int H, int W, int kh, int kw, int pad_h,
-                          int pad_w, int in_dtype, void* stream);
-int lb_lora_wgrad_pair_rp(const void* X, const float* dTs, float* dA, long long dA_js, long long dA_cs,
-                          int K, const void* gY, const float* T, float* dB, long long dB_js,
-                          long long dB_cs, int N, const float* diag, float scale, int M, int r,
-                          int r_pad, float drop_p, const void* seed_dev, int in_dtype, void* stream);
-/* lb_wgrad_problem with the row pitch of V (r_pad) */
-typedef struct lb_wgrad_problem_rp {
-  const void* S;        /* [M, C] rows of in_dtype                         */
-  const float* V;       /* [M, r_pad] fp32                                 */
-  float* out;
-  long long out_js, out_cs;
-  int M, C, r;
-  float scale;
-  const float* diag;
-  float drop_p;
-  const void* seed_dev;
-  int conv_H, conv_W, kh, kw, pad_h, pad_w;
-  int r_pad;
-} lb_wgrad_problem_rp;
-int lb_lora_wgrad_batch_rp(const lb_wgrad_problem_rp* probs, int n, int in_dtype, void* stream);
-int lb_lora_up_dropout_rp(void* Y, int y_dtype, const float* T, const float* up, long long up_rs,
-                          long long up_cs, const float* diag, float scale, float drop_p,
-                          const void* seed_dev, int M, int N, int r, int r_pad, void* stream);
-int lb_lora_dropout_dt_rp(const void* gY, int in_dtype, const float* up, long long up_rs, long long up_cs,
-                          float drop_p, const void* seed_dev, float* dTs, int M, int N, int r, int r_pad,
-                          void* stream);
-int lb_cast_rows_pad16_rp(const float* src, long long src_rs, long long src_cs, void* dst16, int r,
-                          int r_pad, int C, int out_dtype, void* stream);
-/* lb_refresh_shadows / lb_optim_step_fused with 8-column table rows
- * {src_off, src_rs, src_cs, r, C, dst_off, dst_rs, rows}: `rows` padded rows per entry. The table is
- * device memory and is not checked: `rows` must be 16, 32 or 64, r <= rows, and the destination slot
- * must hold `rows` rows of pitch dst_rs (rows * dst_rs elements from dst_off) -- a larger `rows`
- * writes past the slot. */
-int lb_refresh_shadows_rp(const float* p, const long long* table, int n_entries, int max_C,
-                          void* dst16_base, int out_dtype, void* stream);
-int lb_optim_step_fused_rp(float* p, float* g, float* m, float* v, long long n,
-                           const long long* group_off, int n_groups, const float* lr_dev, float beta1,
-                           float beta2, float eps, float weight_decay, float max_norm, float inv_world,
-                           int* step_dev, float* partials, float* gnorm_out, const long long* table,
-                           int n_entries, int max_C, void* shadow16, int shadow_dtype,
-                           unsigned int* barrier2, void* stream);
 
 #ifdef __cplusplus
 }

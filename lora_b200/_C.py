@@ -41,16 +41,16 @@ def _load():
     sig = {
         "lb_abi_version": ([], i32),
         "lb_lora_linear_fwd": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp, vp,
-                                i32, i32, i32, i32, i32, i32, vp], i32),
+                                i32, i32, i32, i32, i32, i32, i32, vp], i32),
         "lb_lora_linear_fwd_dropout": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp,
-                                        i32, i32, i32, i32, i32, i32, f32, vp, vp], i32),
+                                        i32, i32, i32, i32, i32, i32, i32, f32, vp, vp], i32),
         "lb_lora_conv2d_fwd_dropout": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp,
-                                        i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
+                                        i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
                                         f32, vp, vp], i32),
         "lb_tiled_weight_elems": ([i32, i32], ll),
         "lb_tile_weight": ([vp, i32, ll, ll, i32, i32, vp, i32, vp], i32),
-        "lb_lora_wgrad": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, vp], i32),
-        "lb_cast_rows_pad16": ([vp, ll, ll, vp, i32, i32, i32, vp], i32),
+        "lb_lora_wgrad": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, i32, vp], i32),
+        "lb_cast_rows_pad": ([vp, ll, ll, vp, i32, i32, i32, i32, vp], i32),
         "lb_cast_weight": ([vp, i32, vp, vp, i32, i32, i32, vp], i32),
         "lb_adamw_clip_step": ([vp, vp, vp, vp, ll, ctypes.POINTER(ll), i32, vp, f32, f32, f32,
                                 f32, f32, f32, vp, vp, vp, vp], i32),
@@ -65,7 +65,8 @@ def _load():
         "lb_lora_wgrad_batch": ([vp, i32, i32, vp], i32),
         "lb_refresh_shadows": ([vp, vp, i32, i32, vp, i32, vp], i32),
         "lb_debug_set_linear_mode": ([i32], i32),
-        "lb_lora_wgrad_conv": ([vp, vp, vp, f32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp], i32),
+        "lb_lora_wgrad_conv": ([vp, vp, vp, f32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
+                                vp], i32),
         "lb_lora_wgrad_multi": ([i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp], i32),
         "lb_lora_linear_fwd_grouped": ([i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
                                         i32, i32, vp], i32),
@@ -74,7 +75,7 @@ def _load():
         "lb_split_bf16x3": ([vp, ll, vp, i32, i32, i32, vp], i32),
         "lb_debug_set_stamp_buffer": ([vp], i32),
         "lb_debug_set_pdl": ([i32], i32),
-        "lb_lora_wgrad_pair": ([vp, vp, vp, ll, ll, i32, vp, vp, vp, ll, ll, i32, vp, f32, i32, i32,
+        "lb_lora_wgrad_pair": ([vp, vp, vp, ll, ll, i32, vp, vp, vp, ll, ll, i32, vp, f32, i32, i32, i32,
                                 f32, vp, i32, vp], i32),
         "lb_svd_workspace_bytes": ([ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32], ll),
         "lb_svd_truncated_batched": ([vp, vp, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32, i32, f32,
@@ -85,41 +86,13 @@ def _load():
         "lb_svd_apply": ([vp, vp, vp, i32, vp, i32, i32, ll, i32, ll, i32, vp], i32),
         "lb_svd_jacobi": ([vp, vp, vp, i32, i32, vp], i32),
         "lb_svd_randn": ([vp, ll, ctypes.c_ulonglong, vp], i32),
-        "lb_lora_wgrad_shift": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, i32, i32, i32,
-                                 i32, vp], i32),
         "lb_lora_conv2d_fwd": ([vp, vp, vp, vp, vp, ll, ll, ll, vp, f32, vp, vp, vp,
-                                i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
+                                i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
                                 vp], i32),
         "lb_cast_conv_weight": ([vp, i32, vp, vp, i32, i32, i32, i32, i32, vp], i32),
-        "lb_lora_up_dropout": ([vp, i32, vp, vp, ll, ll, vp, f32, f32, vp, i32, i32, i32, vp], i32),
-        "lb_lora_dropout_dt": ([vp, i32, vp, ll, ll, f32, vp, vp, i32, i32, i32, vp], i32),
-        "lb_lora_wgrad_masked": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, f32, vp, i32, vp], i32),
-        # rank pads 16 / 32 / 64: r_pad follows r
-        "lb_lora_linear_fwd_rp": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp, vp,
-                                   i32, i32, i32, i32, i32, i32, i32, vp], i32),
-        "lb_lora_linear_fwd_dropout_rp": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp,
-                                           i32, i32, i32, i32, i32, i32, i32, f32, vp, vp], i32),
-        "lb_lora_conv2d_fwd_rp": ([vp, vp, vp, vp, vp, ll, ll, ll, vp, f32, vp, vp, vp,
-                                   i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
-                                   vp], i32),
-        "lb_lora_conv2d_fwd_dropout_rp": ([vp, vp, vp, vp, vp, ll, ll, vp, f32, vp, vp,
-                                           i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
-                                           f32, vp, vp], i32),
-        "lb_lora_wgrad_rp": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, i32, vp], i32),
-        "lb_lora_wgrad_shift_rp": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, i32, i32, i32, i32,
-                                    i32, vp], i32),
-        "lb_lora_wgrad_masked_rp": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, f32, vp, i32, vp], i32),
-        "lb_lora_wgrad_conv_rp": ([vp, vp, vp, f32, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32,
-                                   vp], i32),
-        "lb_lora_wgrad_pair_rp": ([vp, vp, vp, ll, ll, i32, vp, vp, vp, ll, ll, i32, vp, f32, i32, i32, i32,
-                                   f32, vp, i32, vp], i32),
-        "lb_lora_wgrad_batch_rp": ([vp, i32, i32, vp], i32),
-        "lb_lora_up_dropout_rp": ([vp, i32, vp, vp, ll, ll, vp, f32, f32, vp, i32, i32, i32, i32, vp], i32),
-        "lb_lora_dropout_dt_rp": ([vp, i32, vp, ll, ll, f32, vp, vp, i32, i32, i32, i32, vp], i32),
-        "lb_cast_rows_pad16_rp": ([vp, ll, ll, vp, i32, i32, i32, i32, vp], i32),
-        "lb_refresh_shadows_rp": ([vp, vp, i32, i32, vp, i32, vp], i32),
-        "lb_optim_step_fused_rp": ([vp, vp, vp, vp, ll, ctypes.POINTER(ll), i32, vp, f32, f32, f32,
-                                    f32, f32, f32, vp, vp, vp, vp, i32, i32, vp, i32, vp, vp], i32),
+        "lb_lora_up_dropout": ([vp, i32, vp, vp, ll, ll, vp, f32, f32, vp, i32, i32, i32, i32, vp], i32),
+        "lb_lora_dropout_dt": ([vp, i32, vp, ll, ll, f32, vp, vp, i32, i32, i32, i32, vp], i32),
+        "lb_lora_wgrad_masked": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, f32, vp, i32, vp], i32),
     }
     for name, s in sig.items():
         if s is None or not hasattr(lib, name):
@@ -150,19 +123,14 @@ lib = _LazyLib()
 def is_loaded() -> bool:
     return _LazyLib._lib is not None
 EXPORTED = [n for n in ("lb_abi_version", "lb_lora_linear_fwd", "lb_lora_wgrad",
-                        "lb_cast_rows_pad16", "lb_cast_weight", "lb_adamw_clip_step",
-                        "lb_refresh_shadows", "lb_lora_wgrad_shift", "lb_lora_conv2d_fwd",
+                        "lb_cast_rows_pad", "lb_cast_weight", "lb_adamw_clip_step",
+                        "lb_refresh_shadows", "lb_lora_conv2d_fwd",
                         "lb_cast_conv_weight", "lb_lora_up_dropout", "lb_lora_dropout_dt",
                         "lb_lora_wgrad_masked", "lb_lora_wgrad_pair", "lb_svd_mul", "lb_svd_gram",
                         "lb_svd_chol_inv", "lb_svd_apply", "lb_svd_jacobi", "lb_svd_randn", "lb_split_bf16x3", "lb_lora_merge", "lb_ti_embed_step", "lb_lora_linear_fwd_grouped", "lb_lora_wgrad_multi", "lb_lora_wgrad_conv",
                         "lb_lora_linear_fwd_dropout", "lb_lora_conv2d_fwd_dropout", "lb_debug_set_pdl", "lb_svd_workspace_bytes", "lb_svd_truncated_batched",
                         "lb_optim_step_fused", "lb_step_prologue", "lb_masked_mse_fwd_bwd",
-                        "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight",
-                        "lb_lora_linear_fwd_rp", "lb_lora_linear_fwd_dropout_rp", "lb_lora_conv2d_fwd_rp",
-                        "lb_lora_conv2d_fwd_dropout_rp", "lb_lora_wgrad_rp", "lb_lora_wgrad_shift_rp",
-                        "lb_lora_wgrad_masked_rp", "lb_lora_wgrad_conv_rp", "lb_lora_wgrad_pair_rp",
-                        "lb_lora_wgrad_batch_rp", "lb_lora_up_dropout_rp", "lb_lora_dropout_dt_rp",
-                        "lb_cast_rows_pad16_rp", "lb_refresh_shadows_rp", "lb_optim_step_fused_rp")]
+                        "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight")]
 
 
 def check(status: int, what: str):

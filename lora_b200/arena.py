@@ -27,7 +27,6 @@ from ._C import check, dtype_code, ptr, stream_ptr
 
 _ALIGN = 8  # elements; keeps every factor 32-byte aligned inside the arena
 _LORA_CLASS_NAMES = ("LoraInjectedLinear", "LoraInjectedConv2d")
-R_PAD = 16
 
 
 def lora_sites(model: nn.Module) -> List[nn.Module]:
@@ -106,24 +105,21 @@ class LoraArena:
         self.sync_replicas()
 
         # ---- 16-bit operand copies ("shadows") + the table the refresh kernel walks
-        # (each site's slots hold rank_pad(r) rows; any pad above 16 switches the table to the 8-column
-        # format whose last column is the row count: lb_refresh_shadows_rp / lb_optim_step_fused_rp)
+        # (each site's slots hold rank_pad(r) rows, the table's last column)
         rows, sh_off, max_c = [], 0, 1
         self._shadow_slots = []  # (site, kind, off, C, rows)
-        self.wide = any(s.r > R_PAD for sg in site_groups for s in sg)
         for s in (s for sg in site_groups for s in sg):
             o_up = self._off_of(s, "up")
             o_dn = self._off_of(s, "down")
             r = s.r
             rp = ops.rank_pad(r)
-            tail = (rp,) if self.wide else ()
             if type(s).__name__ == "LoraInjectedLinear":
                 N, K = s.linear.out_features, s.linear.in_features
                 # down16 [RP,K] <- A[r,K]
-                rows.append((o_dn, K, 1, r, K, sh_off, K) + tail)
+                rows.append((o_dn, K, 1, r, K, sh_off, K, rp))
                 self._shadow_slots.append((s, "down", sh_off, K, rp)); sh_off += rp * K
                 # upT16 [RP,N] <- B[N,r]^T
-                rows.append((o_up, 1, r, r, N, sh_off, N) + tail)
+                rows.append((o_up, 1, r, r, N, sh_off, N, rp))
                 self._shadow_slots.append((s, "upT", sh_off, N, rp)); sh_off += rp * N
                 max_c = max(max_c, K, N)
             else:
@@ -134,9 +130,9 @@ class LoraArena:
                 ktot = taps * cin
                 # down16 [RP, taps*Cin], K index = tap*Cin + c  <- A[r,Cin,kh,kw]
                 for t in range(taps):
-                    rows.append((o_dn + t, cin * taps, taps, r, cin, sh_off + t * cin, ktot) + tail)
+                    rows.append((o_dn + t, cin * taps, taps, r, cin, sh_off + t * cin, ktot, rp))
                 self._shadow_slots.append((s, "down", sh_off, ktot, rp)); sh_off += rp * ktot
-                rows.append((o_up, 1, r, r, cout, sh_off, cout) + tail)
+                rows.append((o_up, 1, r, r, cout, sh_off, cout, rp))
                 self._shadow_slots.append((s, "upT", sh_off, cout, rp)); sh_off += rp * cout
                 max_c = max(max_c, cin, cout)
             sh_off = _round_up(sh_off, 64)
@@ -162,7 +158,7 @@ class LoraArena:
         world, rank = dist.get_world_size(), dist.get_rank()
         if world > 16:
             raise _C.LoraB200Error("enable_peer_allreduce: at most 16 ranks (one NVSwitch node)")
-        if self.wide:
+        if any(rp > 16 for *_, rp in self._shadow_slots):
             raise _C.LoraB200Error("enable_peer_allreduce: LoRA ranks above 16 are not supported by the "
                                    "peer all-reduce step (use the NCCL all-reduce path)")
         dev = self.device
@@ -242,8 +238,7 @@ class LoraArena:
                 s._lb.upT[dt] = (_key(s.lora_up.weight), view)
 
     def refresh_shadows(self):
-        refresh = _C.lib.lb_refresh_shadows_rp if self.wide else _C.lib.lb_refresh_shadows
-        check(refresh(ptr(self.p), ptr(self.table), self.table.shape[0],
+        check(_C.lib.lb_refresh_shadows(ptr(self.p), ptr(self.table), self.table.shape[0],
                                         self.table_max_c, ptr(self.shadow),
                                         dtype_code(self.compute_dtype), stream_ptr()),
               "lb_refresh_shadows")
@@ -281,8 +276,7 @@ class LoraArena:
             self._publish_shadows()
             return
         if self.fused_step:
-            fused = _C.lib.lb_optim_step_fused_rp if self.wide else _C.lib.lb_optim_step_fused
-            check(fused(ptr(self.p), ptr(self.g), ptr(self.m), ptr(self.v), self.n,
+            check(_C.lib.lb_optim_step_fused(ptr(self.p), ptr(self.g), ptr(self.m), ptr(self.v), self.n,
                                              self._group_off_c, len(self.group_off) - 1, ptr(self.lr),
                                              beta1, beta2, eps, weight_decay,
                                              float(max_norm if max_norm else 0.0), 1.0 / world_size,

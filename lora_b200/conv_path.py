@@ -1,5 +1,5 @@
 """autograd glue for LoraInjectedConv2d on the fused NHWC implicit-GEMM kernel
-(lb_lora_conv2d_fwd / lb_lora_wgrad_shift). Replaces lora_diffusion/lora.py:130-135 + autograd.
+(lb_lora_conv2d_fwd / lb_lora_wgrad_conv). Replaces lora_diffusion/lora.py:130-135 + autograd.
 
 Supported geometry = the reference's conv LoRA sites in SD1.5 (`ResnetBlock2D.conv1/conv2`
 3x3 pad 1, `conv_shortcut` 1x1): stride 1, dilation 1, groups 1, "same" padding. Anything else

@@ -189,44 +189,22 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
 }
 
 extern "C" int lb_lora_conv2d_fwd(const void* X, const void* W, const float* bias,
-                                  const void* down16, const float* up, long long up_rs,
+                                  const void* down, const float* up, long long up_rs,
                                   long long up_cs, long long up_gs, const float* diag, float scale,
                                   void* Y, float* T_out, const float* T_in, int n_img, int H, int Wd, int Cin,
-                                  int Cout, int kh, int kw, int pad_h, int pad_w, int r,
+                                  int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
                                   int per_tap_T, int in_dtype, int out_dtype, void* stream) {
-  return conv2d_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, up_gs, diag, scale, Y, T_out, T_in, n_img, H,
-                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, 16, per_tap_T, in_dtype, out_dtype, 0.f, nullptr,
-                         stream);
-}
-
-extern "C" int lb_lora_conv2d_fwd_rp(const void* X, const void* W, const float* bias,
-                                     const void* down, const float* up, long long up_rs,
-                                     long long up_cs, long long up_gs, const float* diag, float scale,
-                                     void* Y, float* T_out, const float* T_in, int n_img, int H, int Wd, int Cin,
-                                     int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
-                                     int per_tap_T, int in_dtype, int out_dtype, void* stream) {
   return conv2d_fwd_impl(X, W, bias, down, up, up_rs, up_cs, up_gs, diag, scale, Y, T_out, T_in, n_img, H,
                          Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, r_pad, per_tap_T, in_dtype, out_dtype, 0.f,
                          nullptr, stream);
 }
 
 extern "C" int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias,
-                                          const void* down16, const float* up, long long up_rs,
+                                          const void* down, const float* up, long long up_rs,
                                           long long up_cs, const float* diag, float scale, void* Y,
                                           float* T_out, int n_img, int H, int Wd, int Cin, int Cout, int kh,
-                                          int kw, int pad_h, int pad_w, int r, int in_dtype, int out_dtype,
-                                          float drop_p, const void* seed_dev, void* stream) {
-  return conv2d_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, 0, diag, scale, Y, T_out, nullptr, n_img, H,
-                         Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, 16, 0, in_dtype, out_dtype, drop_p, seed_dev,
-                         stream);
-}
-
-extern "C" int lb_lora_conv2d_fwd_dropout_rp(const void* X, const void* W, const float* bias,
-                                             const void* down, const float* up, long long up_rs,
-                                             long long up_cs, const float* diag, float scale, void* Y,
-                                             float* T_out, int n_img, int H, int Wd, int Cin, int Cout, int kh,
-                                             int kw, int pad_h, int pad_w, int r, int r_pad, int in_dtype,
-                                             int out_dtype, float drop_p, const void* seed_dev, void* stream) {
+                                          int kw, int pad_h, int pad_w, int r, int r_pad, int in_dtype,
+                                          int out_dtype, float drop_p, const void* seed_dev, void* stream) {
   return conv2d_fwd_impl(X, W, bias, down, up, up_rs, up_cs, 0, diag, scale, Y, T_out, nullptr, n_img, H,
                          Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, r_pad, 0, in_dtype, out_dtype, drop_p, seed_dev,
                          stream);

@@ -287,37 +287,19 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
 
 
 extern "C" int lb_lora_linear_fwd(const void* X, const void* W, const float* bias,
-                                  const void* down16, const float* up, long long up_rs,
+                                  const void* down, const float* up, long long up_rs,
                                   long long up_cs, const float* diag, float scale, void* Y,
-                                  float* T_out, const float* T_in, int M, int K, int N, int r,
+                                  float* T_out, const float* T_in, int M, int K, int N, int r, int r_pad,
                                   int in_dtype, int out_dtype, void* stream) {
-  return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, T_in, M, K, N, r, 16,
-                         in_dtype, out_dtype, 0.f, nullptr, stream);
-}
-
-extern "C" int lb_lora_linear_fwd_rp(const void* X, const void* W, const float* bias,
-                                     const void* down, const float* up, long long up_rs,
-                                     long long up_cs, const float* diag, float scale, void* Y,
-                                     float* T_out, const float* T_in, int M, int K, int N, int r, int r_pad,
-                                     int in_dtype, int out_dtype, void* stream) {
   return linear_fwd_impl(X, W, bias, down, up, up_rs, up_cs, diag, scale, Y, T_out, T_in, M, K, N, r, r_pad,
                          in_dtype, out_dtype, 0.f, nullptr, stream);
 }
 
 extern "C" int lb_lora_linear_fwd_dropout(const void* X, const void* W, const float* bias,
-                                          const void* down16, const float* up, long long up_rs,
+                                          const void* down, const float* up, long long up_rs,
                                           long long up_cs, const float* diag, float scale, void* Y,
-                                          float* T_out, int M, int K, int N, int r, int in_dtype,
+                                          float* T_out, int M, int K, int N, int r, int r_pad, int in_dtype,
                                           int out_dtype, float drop_p, const void* seed_dev, void* stream) {
-  return linear_fwd_impl(X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, nullptr, M, K, N, r, 16,
-                         in_dtype, out_dtype, drop_p, seed_dev, stream);
-}
-
-extern "C" int lb_lora_linear_fwd_dropout_rp(const void* X, const void* W, const float* bias,
-                                             const void* down, const float* up, long long up_rs,
-                                             long long up_cs, const float* diag, float scale, void* Y,
-                                             float* T_out, int M, int K, int N, int r, int r_pad, int in_dtype,
-                                             int out_dtype, float drop_p, const void* seed_dev, void* stream) {
   return linear_fwd_impl(X, W, bias, down, up, up_rs, up_cs, diag, scale, Y, T_out, nullptr, M, K, N, r, r_pad,
                          in_dtype, out_dtype, drop_p, seed_dev, stream);
 }

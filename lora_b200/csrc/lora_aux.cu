@@ -335,23 +335,30 @@ __global__ void cast_rows_pad16_kernel(const float* __restrict__ src, long long 
   dst[static_cast<size_t>(j) * C + c] = to16(x, fmt);
 }
 
-// PADCOL: 8-column table entries whose last column is the padded row count (16, 32 or 64), else 16
-template <bool PADCOL = false>
+// One entry {src_off, src_rs, src_cs, r, C, dst_off, dst_rs, rows} of the shadow table (lb_refresh_shadows):
+// columns c = c0, c0 + dc, ... < C of the `rows` zero-padded 16-bit rows of one LoRA factor. p is read
+// through L2 because the optimizer kernels write it earlier in the same launch.
+__device__ __forceinline__ void refresh_shadow_entry(const float* __restrict__ p, const long long* __restrict__ e,
+                                                     uint16_t* __restrict__ dst, int fmt, int c0, int dc) {
+  const long long src_off = __ldg(e), rs = __ldg(e + 1), cs = __ldg(e + 2);
+  const int r = static_cast<int>(__ldg(e + 3)), C = static_cast<int>(__ldg(e + 4));
+  const long long dst_off = __ldg(e + 5), dst_rs = __ldg(e + 6);
+  const int rows = static_cast<int>(__ldg(e + 7));
+  for (int c = c0; c < C; c += dc) {
+#pragma unroll 2   // deeper unrolling hoists the row loads and raises the optimizer kernels' registers
+    for (int j = 0; j < rows; ++j) {
+      const float x = (j < r) ? __ldcg(p + src_off + j * rs + c * cs) : 0.f;
+      dst[dst_off + j * dst_rs + c] = to16(x, fmt);
+    }
+  }
+}
+
+// grid (column blocks, table entries)
 __global__ void refresh_shadows_kernel(const float* __restrict__ p,
                                        const long long* __restrict__ table,
                                        uint16_t* __restrict__ dst_base, int fmt) {
-  const long long* e = table + static_cast<size_t>(blockIdx.y) * (PADCOL ? 8 : 7);
-  const long long src_off = e[0], rs = e[1], cs = e[2];
-  const int r = static_cast<int>(e[3]), C = static_cast<int>(e[4]);
-  const long long dst_off = e[5], dst_rs = e[6];
-  const int rows = PADCOL ? static_cast<int>(e[7]) : 16;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-#pragma unroll 16
-  for (int j = 0; j < rows; ++j) {
-    const float x = (j < r) ? p[src_off + j * rs + c * cs] : 0.f;
-    dst_base[dst_off + j * dst_rs + c] = to16(x, fmt);
-  }
+  refresh_shadow_entry(p, table + static_cast<size_t>(blockIdx.y) * 8, dst_base, fmt,
+                       blockIdx.x * blockDim.x + threadIdx.x, gridDim.x * blockDim.x);
 }
 
 // src [R,C] -> dst [R,C] (optional) and dstT [C,R] (optional), 32x32 tiles through smem
@@ -570,7 +577,7 @@ adamw_update_kernel(float* __restrict__ p, float* __restrict__ g, float* __restr
 //   phase 1  per-block partial sum of g^2 (fixed order => deterministic)          -- grid barrier --
 //   phase 2  every block re-reduces the partials, forms coef, updates its slice of p/m/v, zeroes g
 //                                                                                  -- grid barrier --
-//   phase 3  re-casts every LoRA factor into the zero-padded 16-bit [16, C] operands the wgmma
+//   phase 3  re-casts every LoRA factor into the zero-padded 16-bit [rows, C] operands the wgmma
 //            kernels read (table walk, same rows as lb_refresh_shadows)
 // The grid is launched with cudaLaunchAttributeCooperative (co-residency guaranteed) and at most
 // one CTA per SM; the barrier is a generation counter in `bar` (2 x uint32, zero-initialised).
@@ -594,7 +601,6 @@ __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int nbl
   __syncthreads();
 }
 
-template <bool PADCOL = false>   // shadow table format as refresh_shadows_kernel
 __global__ void __launch_bounds__(OPT_THREADS)
 optim_step_fused_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
                         float* __restrict__ v, long long n, OptGroups groups,
@@ -660,24 +666,9 @@ optim_step_fused_kernel(float* __restrict__ p, float* __restrict__ g, float* __r
   }
   if (n_entries <= 0) return;
   grid_barrier(bar, nb);
-  // ---- phase 3: work item = (table entry, 256-column block); p is read through L2 (just written)
-  {
-    // one table entry per block iteration (entries have 64 ... 10240 columns: no empty work items)
-    for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb) {
-      const long long* e = table + static_cast<size_t>(e_i) * (PADCOL ? 8 : 7);
-      const long long src_off = __ldg(e), rs = __ldg(e + 1), cs = __ldg(e + 2);
-      const int r = static_cast<int>(__ldg(e + 3)), C = static_cast<int>(__ldg(e + 4));
-      const long long dst_off = __ldg(e + 5), dst_rs = __ldg(e + 6);
-      const int rows = PADCOL ? static_cast<int>(__ldg(e + 7)) : 16;
-      for (int c = threadIdx.x; c < C; c += OPT_THREADS) {
-#pragma unroll 16
-        for (int j = 0; j < rows; ++j) {
-          const float x = (j < r) ? __ldcg(p + src_off + j * rs + c * cs) : 0.f;
-          shadow[dst_off + j * dst_rs + c] = to16(x, fmt);
-        }
-      }
-    }
-  }
+  // ---- phase 3: one table entry per block iteration (entries have 64 ... 10240 columns: no empty work items)
+  for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb)
+    refresh_shadow_entry(p, table + static_cast<size_t>(e_i) * 8, shadow, fmt, threadIdx.x, OPT_THREADS);
 }
 
 // ------------------------------------------------------------------------------- data-parallel optimizer step
@@ -820,23 +811,9 @@ optim_step_dp_kernel(float* __restrict__ p, float* __restrict__ g, float* __rest
     g[i] = 0.f;
   grid_barrier(bar, nb);
   if (blockIdx.x == 0 && threadIdx.x == 0) epoch_dev[0] = epoch;
-  // ---- phase 3: operand shadows
-  if (n_entries > 0) {
-    // one table entry per block iteration (entries have 64 ... 10240 columns: no empty work items)
-    for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb) {
-      const long long* e = table + static_cast<size_t>(e_i) * 7;
-      const long long src_off = __ldg(e), rs = __ldg(e + 1), cs = __ldg(e + 2);
-      const int r = static_cast<int>(__ldg(e + 3)), C = static_cast<int>(__ldg(e + 4));
-      const long long dst_off = __ldg(e + 5), dst_rs = __ldg(e + 6);
-      for (int c = threadIdx.x; c < C; c += OPT_THREADS) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float x = (j < r) ? __ldcg(p + src_off + j * rs + c * cs) : 0.f;
-          shadow[dst_off + j * dst_rs + c] = to16(x, fmt);
-        }
-      }
-    }
-  }
+  // ---- phase 3: operand shadows, one table entry per block iteration
+  for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb)
+    refresh_shadow_entry(p, table + static_cast<size_t>(e_i) * 8, shadow, fmt, threadIdx.x, OPT_THREADS);
 }
 
 // ------------------------------------------------------------------------------- textual inversion step
@@ -908,69 +885,7 @@ int launch_t_from16(const void* gY, int fmt, const void* down, int C, int M, int
 // =============================================================================== C ABI
 using namespace lb;
 
-extern "C" int lb_abi_version(void) { return 5; }
-
-extern "C" int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float scale,
-                                   float* out, long long out_js, long long out_cs, int M, int C,
-                                   int r, int H, int W, int dy, int dx, int in_dtype, void* stream);
-extern "C" int lb_lora_wgrad_masked(const void* S, const float* V, const float* diag, float scale,
-                                    float* out, long long out_js, long long out_cs, int M, int C,
-                                    int r, float drop_p, const void* seed_dev, int in_dtype,
-                                    void* stream);
-static int wgrad_launch(const void* S, const float* V, const float* diag, float scale, float* out,
-                        long long out_js, long long out_cs, int M, int C, int r, int r_pad, int H, int W,
-                        int dy, int dx, float drop_p, const void* seed_dev, int in_dtype,
-                        void* stream);
-
-extern "C" int lb_lora_wgrad(const void* S, const float* V, const float* diag, float scale,
-                             float* out, long long out_js, long long out_cs, int M, int C, int r,
-                             int in_dtype, void* stream) {
-  return lb_lora_wgrad_shift(S, V, diag, scale, out, out_js, out_cs, M, C, r, 0, 0, 0, 0, in_dtype,
-                             stream);
-}
-
-extern "C" int lb_lora_wgrad_shift(const void* S, const float* V, const float* diag, float scale,
-                                   float* out, long long out_js, long long out_cs, int M, int C,
-                                   int r, int H, int W, int dy, int dx, int in_dtype, void* stream) {
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, 16, H, W, dy, dx, 0.f, nullptr,
-                      in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_rp(const void* S, const float* V, const float* diag, float scale,
-                                float* out, long long out_js, long long out_cs, int M, int C, int r,
-                                int r_pad, int in_dtype, void* stream) {
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, 0, 0, 0, 0, 0.f, nullptr,
-                      in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_shift_rp(const void* S, const float* V, const float* diag, float scale,
-                                      float* out, long long out_js, long long out_cs, int M, int C,
-                                      int r, int r_pad, int H, int W, int dy, int dx, int in_dtype,
-                                      void* stream) {
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, H, W, dy, dx, 0.f, nullptr,
-                      in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_masked(const void* S, const float* V, const float* diag, float scale,
-                                    float* out, long long out_js, long long out_cs, int M, int C,
-                                    int r, float drop_p, const void* seed_dev, int in_dtype,
-                                    void* stream) {
-  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, 16, 0, 0, 0, 0, drop_p, seed_dev,
-                      in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_masked_rp(const void* S, const float* V, const float* diag, float scale,
-                                       float* out, long long out_js, long long out_cs, int M, int C,
-                                       int r, int r_pad, float drop_p, const void* seed_dev, int in_dtype,
-                                       void* stream) {
-  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
-  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, 0, 0, 0, 0, drop_p, seed_dev,
-                      in_dtype, stream);
-}
-
-static int prob_pad(const lb_wgrad_problem&) { return 16; }
-static int prob_pad(const lb_wgrad_problem_rp& q) { return q.r_pad; }
+extern "C" int lb_abi_version(void) { return 6; }
 
 static int wgrad_run(WgArgs& a, int in_dtype, void* stream) {
   if (a.M <= 0 || a.n_pr < 1 || a.n_pr > WG_MAXP) return LB_ERR_SHAPE;
@@ -1017,26 +932,38 @@ static int wgrad_run(WgArgs& a, int in_dtype, void* stream) {
 }
 
 static int wgrad_launch(const void* S, const float* V, const float* diag, float scale, float* out,
-                        long long out_js, long long out_cs, int M, int C, int r, int r_pad, int H, int W,
-                        int dy, int dx, float drop_p, const void* seed_dev, int in_dtype,
-                        void* stream) {
-  if (H < 0 || W < 0 || (H > 0) != (W > 0)) return LB_ERR_SHAPE;
-  if (H > 0 && (M % (H * W)) != 0) return LB_ERR_SHAPE;
+                        long long out_js, long long out_cs, int M, int C, int r, int r_pad, float drop_p,
+                        const void* seed_dev, int in_dtype, void* stream) {
   WgArgs a = {};
   a.pr[0].S = reinterpret_cast<const uint2*>(S); a.pr[0].V = V; a.pr[0].out = out;
   a.pr[0].js = out_js; a.pr[0].cs = out_cs; a.pr[0].C = C; a.pr[0].drop_p = drop_p;
   a.pr[0].diag = diag; a.pr[0].scale = scale; a.pr[0].r = r; a.pr[0].vp = r_pad;
   a.n_pr = 1;
   a.seed_dev = reinterpret_cast<const unsigned long long*>(seed_dev);
-  a.M = M; a.pr[0].cH = H; a.pr[0].cW = W; a.pr[0].dy = dy; a.pr[0].dx = dx; a.pr[0].kw = 1; a.pr[0].taps = 1;
+  a.M = M; a.pr[0].kw = 1; a.pr[0].taps = 1;
   return wgrad_run(a, in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad(const void* S, const float* V, const float* diag, float scale,
+                             float* out, long long out_js, long long out_cs, int M, int C, int r,
+                             int r_pad, int in_dtype, void* stream) {
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, 0.f, nullptr, in_dtype, stream);
+}
+
+extern "C" int lb_lora_wgrad_masked(const void* S, const float* V, const float* diag, float scale,
+                                    float* out, long long out_js, long long out_cs, int M, int C,
+                                    int r, int r_pad, float drop_p, const void* seed_dev, int in_dtype,
+                                    void* stream) {
+  if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
+  return wgrad_launch(S, V, diag, scale, out, out_js, out_cs, M, C, r, r_pad, drop_p, seed_dev, in_dtype,
+                      stream);
 }
 
 // All kh*kw taps of a conv down-factor gradient in one launch: tap t reads S shifted by
 // (t/kw - pad_h, t%kw - pad_w) and accumulates into out[j*out_js + c*out_cs + t].
-static int wgrad_conv_impl(const void* S, const float* V, const float* diag, float scale,
-                           float* out, int M, int C, int r, int r_pad, int H, int W, int kh, int kw,
-                           int pad_h, int pad_w, int in_dtype, void* stream) {
+extern "C" int lb_lora_wgrad_conv(const void* S, const float* V, const float* diag, float scale,
+                                  float* out, int M, int C, int r, int r_pad, int H, int W, int kh, int kw,
+                                  int pad_h, int pad_w, int in_dtype, void* stream) {
   if (H <= 0 || W <= 0 || kh <= 0 || kw <= 0 || (M % (H * W)) != 0) return LB_ERR_SHAPE;
   WgArgs a = {};
   const int taps = kh * kw;
@@ -1048,23 +975,11 @@ static int wgrad_conv_impl(const void* S, const float* V, const float* diag, flo
   return wgrad_run(a, in_dtype, stream);
 }
 
-extern "C" int lb_lora_wgrad_conv(const void* S, const float* V, const float* diag, float scale,
-                                  float* out, int M, int C, int r, int H, int W, int kh, int kw,
-                                  int pad_h, int pad_w, int in_dtype, void* stream) {
-  return wgrad_conv_impl(S, V, diag, scale, out, M, C, r, 16, H, W, kh, kw, pad_h, pad_w, in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_conv_rp(const void* S, const float* V, const float* diag, float scale,
-                                     float* out, int M, int C, int r, int r_pad, int H, int W, int kh, int kw,
-                                     int pad_h, int pad_w, int in_dtype, void* stream) {
-  return wgrad_conv_impl(S, V, diag, scale, out, M, C, r, r_pad, H, W, kh, kw, pad_h, pad_w, in_dtype, stream);
-}
-
-static int wgrad_pair_impl(const void* X, const float* dTs, float* dA, long long dA_js,
-                           long long dA_cs, int K, const void* gY, const float* T, float* dB,
-                           long long dB_js, long long dB_cs, int N, const float* diag,
-                           float scale, int M, int r, int r_pad, float drop_p, const void* seed_dev,
-                           int in_dtype, void* stream) {
+extern "C" int lb_lora_wgrad_pair(const void* X, const float* dTs, float* dA, long long dA_js,
+                                  long long dA_cs, int K, const void* gY, const float* T, float* dB,
+                                  long long dB_js, long long dB_cs, int N, const float* diag,
+                                  float scale, int M, int r, int r_pad, float drop_p, const void* seed_dev,
+                                  int in_dtype, void* stream) {
   if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && seed_dev == nullptr)) return LB_ERR_SHAPE;
   WgArgs a = {};
   a.pr[0].S = reinterpret_cast<const uint2*>(X); a.pr[0].V = dTs; a.pr[0].out = dA;
@@ -1076,24 +991,6 @@ static int wgrad_pair_impl(const void* X, const float* dTs, float* dA, long long
   a.seed_dev = reinterpret_cast<const unsigned long long*>(seed_dev);
   a.M = M;
   return wgrad_run(a, in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_pair(const void* X, const float* dTs, float* dA, long long dA_js,
-                                  long long dA_cs, int K, const void* gY, const float* T, float* dB,
-                                  long long dB_js, long long dB_cs, int N, const float* diag,
-                                  float scale, int M, int r, float drop_p, const void* seed_dev,
-                                  int in_dtype, void* stream) {
-  return wgrad_pair_impl(X, dTs, dA, dA_js, dA_cs, K, gY, T, dB, dB_js, dB_cs, N, diag, scale, M, r, 16, drop_p,
-                         seed_dev, in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_pair_rp(const void* X, const float* dTs, float* dA, long long dA_js,
-                                     long long dA_cs, int K, const void* gY, const float* T, float* dB,
-                                     long long dB_js, long long dB_cs, int N, const float* diag,
-                                     float scale, int M, int r, int r_pad, float drop_p, const void* seed_dev,
-                                     int in_dtype, void* stream) {
-  return wgrad_pair_impl(X, dTs, dA, dA_js, dA_cs, K, gY, T, dB, dB_js, dB_cs, N, diag, scale, M, r, r_pad,
-                         drop_p, seed_dev, in_dtype, stream);
 }
 
 // dA and dB of up to 4 sites that share X (a grouped family) in one launch. HOST arrays of length n.
@@ -1123,22 +1020,21 @@ extern "C" int lb_lora_wgrad_multi(int n, const void* X, const float* const* dTs
 // possible (24 problems per launch): the dA / dB of EVERY linear site of a step, queued during
 // backward and flushed once at its end -- they feed only the optimizer, and one launch over
 // hundreds of MB fills the chip where 120-270 launches over a few MB each were latency-bound.
-template <typename Prob>
-static int wgrad_batch_impl(const Prob* probs, int n, int in_dtype, void* stream) {
+extern "C" int lb_lora_wgrad_batch(const lb_wgrad_problem* probs, int n, int in_dtype, void* stream) {
   if (probs == nullptr || n < 1) return LB_ERR_SHAPE;
   for (int base = 0; base < n; base += WG_MAXP) {
     const int cnt = (n - base) < WG_MAXP ? (n - base) : WG_MAXP;
     WgArgs a = {};
     int max_m = 0;
     for (int i = 0; i < cnt; ++i) {
-      const Prob& q = probs[base + i];
+      const lb_wgrad_problem& q = probs[base + i];
       if (q.M <= 0 || !(q.drop_p >= 0.f && q.drop_p < 1.f) || (q.drop_p > 0.f && q.seed_dev == nullptr))
         return LB_ERR_SHAPE;
       WgProblem& w = a.pr[i];
       w.S = reinterpret_cast<const uint2*>(q.S); w.V = q.V; w.out = q.out; w.js = q.out_js; w.cs = q.out_cs;
       w.C = q.C; w.drop_p = q.drop_p; w.diag = q.diag; w.scale = q.scale; w.r = q.r; w.M = q.M;
       w.seed = reinterpret_cast<const unsigned long long*>(q.seed_dev);
-      w.vp = prob_pad(q);
+      w.vp = q.r_pad;
       if (q.conv_H > 0) {       // conv lora_down weight-gradient: all taps of one site as one problem
         if (q.conv_W <= 0 || q.kh <= 0 || q.kw <= 0 || (q.M % (q.conv_H * q.conv_W)) != 0) return LB_ERR_SHAPE;
         w.cH = q.conv_H; w.cW = q.conv_W; w.dy = -q.pad_h; w.dx = -q.pad_w; w.kw = q.kw; w.taps = q.kh * q.kw;
@@ -1153,14 +1049,6 @@ static int wgrad_batch_impl(const Prob* probs, int n, int in_dtype, void* stream
   return LB_OK;
 }
 
-extern "C" int lb_lora_wgrad_batch(const lb_wgrad_problem* probs, int n, int in_dtype, void* stream) {
-  return wgrad_batch_impl(probs, n, in_dtype, stream);
-}
-
-extern "C" int lb_lora_wgrad_batch_rp(const lb_wgrad_problem_rp* probs, int n, int in_dtype, void* stream) {
-  return wgrad_batch_impl(probs, n, in_dtype, stream);
-}
-
 template <int RP>
 static void up_dropout_launch(void* Y, int y_dtype, const float* T, const float* up, long long up_rs,
                               long long up_cs, const float* diag, float scale, float drop_p,
@@ -1171,10 +1059,10 @@ static void up_dropout_launch(void* Y, int y_dtype, const float* T, const float*
     up_dropout_kernel<uint16_t, RP><<<blocks, 256, 0, st>>>(reinterpret_cast<uint16_t*>(Y), y_dtype == LB_BF16, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r);
 }
 
-extern "C" int lb_lora_up_dropout_rp(void* Y, int y_dtype, const float* T, const float* up,
-                                     long long up_rs, long long up_cs, const float* diag, float scale,
-                                     float drop_p, const void* seed_dev, int M, int N, int r, int r_pad,
-                                     void* stream) {
+extern "C" int lb_lora_up_dropout(void* Y, int y_dtype, const float* T, const float* up,
+                                  long long up_rs, long long up_cs, const float* diag, float scale,
+                                  float drop_p, const void* seed_dev, int M, int N, int r, int r_pad,
+                                  void* stream) {
   if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
   if (M <= 0 || N <= 0 || (N % 8) != 0) return LB_ERR_SHAPE;
   if (r < 1 || r > r_pad) return LB_ERR_RANK;
@@ -1191,51 +1079,10 @@ extern "C" int lb_lora_up_dropout_rp(void* Y, int y_dtype, const float* T, const
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
-extern "C" int lb_lora_up_dropout(void* Y, int y_dtype, const float* T, const float* up,
-                                  long long up_rs, long long up_cs, const float* diag, float scale,
-                                  float drop_p, const void* seed_dev, int M, int N, int r,
-                                  void* stream) {
-  if (M <= 0 || N <= 0 || (N % 8) != 0) return LB_ERR_SHAPE;
-  if (r < 1 || r > 16) return LB_ERR_RANK;
-  if (!(drop_p >= 0.f && drop_p < 1.f) || seed_dev == nullptr) return LB_ERR_SHAPE;
-  if (reinterpret_cast<uintptr_t>(Y) & 15) return LB_ERR_ALIGN;
-  const long long threads = static_cast<long long>(M) * (N / 8);
-  const int blocks = static_cast<int>((threads + 255) / 256);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const unsigned long long* sd = reinterpret_cast<const unsigned long long*>(seed_dev);
-  if (y_dtype == LB_F32)
-    up_dropout_kernel<float><<<blocks, 256, 0, st>>>(reinterpret_cast<float*>(Y), 0, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r);
-  else if (y_dtype == LB_BF16 || y_dtype == LB_F16)
-    up_dropout_kernel<uint16_t><<<blocks, 256, 0, st>>>(reinterpret_cast<uint16_t*>(Y), y_dtype == LB_BF16, T, up, up_rs, up_cs, diag, scale, drop_p, sd, M, N, r);
-  else
-    return LB_ERR_DTYPE;
-  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
 extern "C" int lb_lora_dropout_dt(const void* gY, int in_dtype, const float* up, long long up_rs,
                                   long long up_cs, float drop_p, const void* seed_dev, float* dTs,
-                                  int M, int N, int r, void* stream) {
-  if (M <= 0 || N <= 0 || (N % 8) != 0) return LB_ERR_SHAPE;
-  if (r < 1 || r > 16) return LB_ERR_RANK;
-  if (in_dtype != LB_BF16 && in_dtype != LB_F16) return LB_ERR_DTYPE;
-  if (!(drop_p >= 0.f && drop_p < 1.f) || seed_dev == nullptr) return LB_ERR_SHAPE;
-  if (reinterpret_cast<uintptr_t>(gY) & 15) return LB_ERR_ALIGN;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  dim3 grid((N + DT_COLS - 1) / DT_COLS, (M + DT_ROWS - 1) / DT_ROWS);
-  const int use_atomics = grid.x > 1;
-  if (use_atomics && cudaMemsetAsync(dTs, 0, sizeof(float) * static_cast<size_t>(M) * 16, st) != cudaSuccess)
-    return LB_ERR_CUDA;
-  dropout_dt_kernel<<<grid, 256, 0, st>>>(
-      reinterpret_cast<const uint4*>(gY), in_dtype == LB_BF16, up, up_rs, up_cs, drop_p,
-      reinterpret_cast<const unsigned long long*>(seed_dev), dTs, M, N, r, use_atomics);
-  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
-extern "C" int lb_lora_dropout_dt_rp(const void* gY, int in_dtype, const float* up, long long up_rs,
-                                     long long up_cs, float drop_p, const void* seed_dev, float* dTs,
-                                     int M, int N, int r, int r_pad, void* stream) {
+                                  int M, int N, int r, int r_pad, void* stream) {
   if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
-  if (r_pad == 16) return lb_lora_dropout_dt(gY, in_dtype, up, up_rs, up_cs, drop_p, seed_dev, dTs, M, N, r, stream);
   if (M <= 0 || N <= 0 || (N % 8) != 0) return LB_ERR_SHAPE;
   if (r < 1 || r > r_pad) return LB_ERR_RANK;
   if (in_dtype != LB_BF16 && in_dtype != LB_F16) return LB_ERR_DTYPE;
@@ -1246,25 +1093,19 @@ extern "C" int lb_lora_dropout_dt_rp(const void* gY, int in_dtype, const float* 
   const int use_atomics = grid.x > 1;
   if (use_atomics && cudaMemsetAsync(dTs, 0, sizeof(float) * static_cast<size_t>(M) * r_pad, st) != cudaSuccess)
     return LB_ERR_CUDA;
-  dropout_dt_kernel<true><<<grid, 256, 0, st>>>(
-      reinterpret_cast<const uint4*>(gY), in_dtype == LB_BF16, up, up_rs, up_cs, drop_p,
-      reinterpret_cast<const unsigned long long*>(seed_dev), dTs, M, N, r, use_atomics, r_pad);
+  const uint4* g4 = reinterpret_cast<const uint4*>(gY);
+  const unsigned long long* sd = reinterpret_cast<const unsigned long long*>(seed_dev);
+  if (r_pad == 16)
+    dropout_dt_kernel<<<grid, 256, 0, st>>>(g4, in_dtype == LB_BF16, up, up_rs, up_cs, drop_p, sd, dTs, M, N, r,
+                                            use_atomics);
+  else
+    dropout_dt_kernel<true><<<grid, 256, 0, st>>>(g4, in_dtype == LB_BF16, up, up_rs, up_cs, drop_p, sd, dTs, M,
+                                                  N, r, use_atomics, r_pad);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
-extern "C" int lb_cast_rows_pad16(const float* src, long long src_rs, long long src_cs,
-                                  void* dst16, int r, int C, int out_dtype, void* stream) {
-  if (C <= 0) return LB_ERR_SHAPE;
-  if (r < 1 || r > 16) return LB_ERR_RANK;
-  if (out_dtype != LB_BF16 && out_dtype != LB_F16) return LB_ERR_DTYPE;
-  dim3 grid((C + 255) / 256, 16);
-  cast_rows_pad16_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      src, src_rs, src_cs, reinterpret_cast<uint16_t*>(dst16), r, C, out_dtype == LB_BF16);
-  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
-extern "C" int lb_cast_rows_pad16_rp(const float* src, long long src_rs, long long src_cs,
-                                     void* dst16, int r, int r_pad, int C, int out_dtype, void* stream) {
+extern "C" int lb_cast_rows_pad(const float* src, long long src_rs, long long src_cs,
+                                void* dst16, int r, int r_pad, int C, int out_dtype, void* stream) {
   if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
   if (C <= 0) return LB_ERR_SHAPE;
   if (r < 1 || r > r_pad) return LB_ERR_RANK;
@@ -1281,16 +1122,6 @@ extern "C" int lb_refresh_shadows(const float* p, const long long* table, int n_
   if (out_dtype != LB_BF16 && out_dtype != LB_F16) return LB_ERR_DTYPE;
   dim3 grid((max_C + 255) / 256, n_entries);
   refresh_shadows_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      p, table, reinterpret_cast<uint16_t*>(dst16_base), out_dtype == LB_BF16);
-  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
-extern "C" int lb_refresh_shadows_rp(const float* p, const long long* table, int n_entries,
-                                     int max_C, void* dst16_base, int out_dtype, void* stream) {
-  if (n_entries <= 0 || max_C <= 0) return LB_ERR_SHAPE;
-  if (out_dtype != LB_BF16 && out_dtype != LB_F16) return LB_ERR_DTYPE;
-  dim3 grid((max_C + 255) / 256, n_entries);
-  refresh_shadows_kernel<true><<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       p, table, reinterpret_cast<uint16_t*>(dst16_base), out_dtype == LB_BF16);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
@@ -1428,14 +1259,13 @@ extern "C" int lb_adamw_clip_step(float* p, float* g, float* m, float* v, long l
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
-template <bool PADCOL>
-static int optim_step_fused_impl(float* p, float* g, float* m, float* v, long long n,
-                                 const long long* group_off, int n_groups, const float* lr_dev,
-                                 float beta1, float beta2, float eps, float weight_decay,
-                                 float max_norm, float inv_world, int* step_dev, float* partials,
-                                 float* gnorm_out, const long long* table, int n_entries, int max_C,
-                                 void* shadow16, int shadow_dtype, unsigned int* barrier2,
-                                 void* stream) {
+extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
+                                   const long long* group_off, int n_groups, const float* lr_dev,
+                                   float beta1, float beta2, float eps, float weight_decay,
+                                   float max_norm, float inv_world, int* step_dev, float* partials,
+                                   float* gnorm_out, const long long* table, int n_entries, int max_C,
+                                   void* shadow16, int shadow_dtype, unsigned int* barrier2,
+                                   void* stream) {
   if (n <= 0 || n_groups < 1 || n_groups > OPT_MAX_GROUPS) return LB_ERR_SHAPE;
   if (reinterpret_cast<uintptr_t>(g) & 15) return LB_ERR_ALIGN;
   if (n_entries > 0 && (table == nullptr || shadow16 == nullptr || max_C <= 0)) return LB_ERR_SHAPE;
@@ -1464,34 +1294,10 @@ static int optim_step_fused_impl(float* p, float* g, float* m, float* v, long lo
   cfg.numAttrs = 1;
   const int fmt = shadow_dtype == LB_BF16;
   uint16_t* sh = reinterpret_cast<uint16_t*>(shadow16);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, optim_step_fused_kernel<PADCOL>, p, g, m, v, n, groups, lr_dev, beta1,
+  cudaError_t e = cudaLaunchKernelEx(&cfg, optim_step_fused_kernel, p, g, m, v, n, groups, lr_dev, beta1,
                                      beta2, eps, weight_decay, max_norm, inv_world, step_dev, partials, gnorm_out,
                                      table, n_entries, max_C, sh, fmt, barrier2);
   return e == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
-extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
-                                   const long long* group_off, int n_groups, const float* lr_dev,
-                                   float beta1, float beta2, float eps, float weight_decay,
-                                   float max_norm, float inv_world, int* step_dev, float* partials,
-                                   float* gnorm_out, const long long* table, int n_entries, int max_C,
-                                   void* shadow16, int shadow_dtype, unsigned int* barrier2,
-                                   void* stream) {
-  return optim_step_fused_impl<false>(p, g, m, v, n, group_off, n_groups, lr_dev, beta1, beta2, eps, weight_decay,
-                                      max_norm, inv_world, step_dev, partials, gnorm_out, table, n_entries, max_C,
-                                      shadow16, shadow_dtype, barrier2, stream);
-}
-
-extern "C" int lb_optim_step_fused_rp(float* p, float* g, float* m, float* v, long long n,
-                                      const long long* group_off, int n_groups, const float* lr_dev,
-                                      float beta1, float beta2, float eps, float weight_decay,
-                                      float max_norm, float inv_world, int* step_dev, float* partials,
-                                      float* gnorm_out, const long long* table, int n_entries, int max_C,
-                                      void* shadow16, int shadow_dtype, unsigned int* barrier2,
-                                      void* stream) {
-  return optim_step_fused_impl<true>(p, g, m, v, n, group_off, n_groups, lr_dev, beta1, beta2, eps, weight_decay,
-                                     max_norm, inv_world, step_dev, partials, gnorm_out, table, n_entries, max_C,
-                                     shadow16, shadow_dtype, barrier2, stream);
 }
 
 // ------------------------------------------------------------------------------- CUDA IPC helpers

@@ -42,11 +42,7 @@ class _WgProblemC(_ct.Structure):
                 ("M", _ct.c_int), ("C", _ct.c_int), ("r", _ct.c_int), ("scale", _ct.c_float),
                 ("diag", _ct.c_void_p), ("drop_p", _ct.c_float), ("seed_dev", _ct.c_void_p),
                 ("conv_H", _ct.c_int), ("conv_W", _ct.c_int), ("kh", _ct.c_int), ("kw", _ct.c_int),
-                ("pad_h", _ct.c_int), ("pad_w", _ct.c_int)]
-
-
-class _WgProblemRpC(_ct.Structure):
-    _fields_ = _WgProblemC._fields_ + [("r_pad", _ct.c_int)]
+                ("pad_h", _ct.c_int), ("pad_w", _ct.c_int), ("r_pad", _ct.c_int)]
 
 
 _WG_QUEUE = None      # None: launch immediately; dict dtype -> [(_WgProblemC fields, keepalive)]
@@ -64,14 +60,9 @@ def wgrad_defer_cancel():
 
 
 def _wgrad_launch(dtype, items):
-    if all(it[0][-1] == R_PAD for it in items):
-        arr = (_WgProblemC * len(items))(*[_WgProblemC(*it[0][:-1]) for it in items])
-        check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
-    else:
-        arr = (_WgProblemRpC * len(items))(*[_WgProblemRpC(*it[0]) for it in items])
-        check(_C.lib.lb_lora_wgrad_batch_rp(arr, len(items), dtype_code(dtype), stream_ptr()),
-              "lb_lora_wgrad_batch_rp")
-    n = (len(items) + WG_BATCH - 1) // WG_BATCH
+    arr = (_WgProblemC * len(items))(*[_WgProblemC(*it[0]) for it in items])
+    check(_C.lib.lb_lora_wgrad_batch(arr, len(items), dtype_code(dtype), stream_ptr()), "lb_lora_wgrad_batch")
+    n =(len(items) + WG_BATCH - 1) // WG_BATCH
     _count(n)
     return n
 
@@ -104,16 +95,12 @@ def _req_cuda(*ts):
 
 
 def cast_rows_pad16(src: torch.Tensor, rs: int, cs: int, r: int, C: int, dtype) -> torch.Tensor:
-    """fp32 factor -> zero-padded 16-bit [rank_pad(r), C] operand (see lb_cast_rows_pad16[_rp])."""
+    """fp32 factor -> zero-padded 16-bit [rank_pad(r), C] operand (see lb_cast_rows_pad)."""
     _req_cuda(src)
     rp = rank_pad(r) if r >= 1 else R_PAD
     out = torch.empty((rp, C), device=src.device, dtype=dtype)
-    if rp == R_PAD:
-        check(_C.lib.lb_cast_rows_pad16(ptr(src), rs, cs, ptr(out), r, C, dtype_code(dtype),
-                                        stream_ptr()), "lb_cast_rows_pad16")
-    else:
-        check(_C.lib.lb_cast_rows_pad16_rp(ptr(src), rs, cs, ptr(out), r, rp, C, dtype_code(dtype),
-                                           stream_ptr()), "lb_cast_rows_pad16_rp")
+    check(_C.lib.lb_cast_rows_pad(ptr(src), rs, cs, ptr(out), r, rp, C, dtype_code(dtype), stream_ptr()),
+          "lb_cast_rows_pad")
     _count()
     return out
 
@@ -200,35 +187,19 @@ def fused_linear(x2d: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tens
     assert x2d.is_contiguous() and down16.is_contiguous()
     y = torch.empty((M, N), device=x2d.device, dtype=out_dtype)
     t = torch.empty((M, rp), device=x2d.device, dtype=torch.float32) if want_t else None
-    if rp != R_PAD:
-        assert t_in is None or t_in.shape == (M, rp)
-        if drop_p > 0.0:
-            assert t_in is None and seed is not None and seed.dtype == torch.int64 and seed.is_cuda
-            check(_C.lib.lb_lora_linear_fwd_dropout_rp(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up), up_rs, up_cs,
-                                                       ptr(diag), float(scale), ptr(y), ptr(t), M, K, N, r, rp,
-                                                       dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype),
-                                                       float(drop_p), ptr(seed), stream_ptr()),
-                  "lb_lora_linear_fwd_dropout_rp")
-        else:
-            check(_C.lib.lb_lora_linear_fwd_rp(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up), up_rs, up_cs, ptr(diag),
-                                               float(scale), ptr(y), ptr(t), ptr(t_in), M, K, N, r, rp,
-                                               dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype), stream_ptr()),
-                  "lb_lora_linear_fwd_rp")
-        _count()
-        return y, t
+    assert t_in is None or t_in.shape == (M, rp)
     if drop_p > 0.0:
         assert t_in is None and seed is not None and seed.dtype == torch.int64 and seed.is_cuda
         check(_C.lib.lb_lora_linear_fwd_dropout(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up),
                                                 up_rs, up_cs, ptr(diag), float(scale), ptr(y), ptr(t),
-                                                M, K, N, r, dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype),
-                                                float(drop_p), ptr(seed), stream_ptr()),
+                                                M, K, N, r, rp, dtype_code(x2d.dtype) | wflag,
+                                                dtype_code(out_dtype), float(drop_p), ptr(seed), stream_ptr()),
               "lb_lora_linear_fwd_dropout")
-        _count()
-        return y, t
-    check(_C.lib.lb_lora_linear_fwd(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up),
-                                    up_rs, up_cs, ptr(diag), float(scale), ptr(y), ptr(t), ptr(t_in),
-                                    M, K, N, r, dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype),
-                                    stream_ptr()), "lb_lora_linear_fwd")
+    else:
+        check(_C.lib.lb_lora_linear_fwd(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up),
+                                        up_rs, up_cs, ptr(diag), float(scale), ptr(y), ptr(t), ptr(t_in),
+                                        M, K, N, r, rp, dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype),
+                                        stream_ptr()), "lb_lora_linear_fwd")
     _count()
     return y, t
 
@@ -244,12 +215,8 @@ def wgrad(S: torch.Tensor, V: torch.Tensor, diag: Optional[torch.Tensor], scale:
     if _WG_QUEUE is not None and deferrable:
         _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag)
         return
-    if rp == R_PAD:
-        check(_C.lib.lb_lora_wgrad(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
-                                   M, C, r, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad")
-    else:
-        check(_C.lib.lb_lora_wgrad_rp(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
-                                      M, C, r, rp, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad_rp")
+    check(_C.lib.lb_lora_wgrad(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js, out_cs,
+                               M, C, r, rp, dtype_code(S.dtype), stream_ptr()), "lb_lora_wgrad")
     _count()
 
 
@@ -279,16 +246,15 @@ def conv_down16(a4d: torch.Tensor, dtype, table_cache: dict) -> torch.Tensor:
     key = (r, cin, taps, a4d.device)
     tab = table_cache.get(key)
     if tab is None:
-        rows = [(t, cin * taps, taps, r, cin, t * cin, taps * cin) + ((rp,) if rp != R_PAD else ())
-                for t in range(taps)]
+        rows = [(t, cin * taps, taps, r, cin, t * cin, taps * cin, rp) for t in range(taps)]
         tab = torch.tensor(rows, device=a4d.device, dtype=torch.int64)
         table_cache[key] = tab
     src = a4d.detach()
     if src.dtype != torch.float32 or not src.is_contiguous():
         src = src.float().contiguous()
     out = torch.empty((rp, taps * cin), device=a4d.device, dtype=dtype)
-    refresh = _C.lib.lb_refresh_shadows if rp == R_PAD else _C.lib.lb_refresh_shadows_rp
-    check(refresh(ptr(src), ptr(tab), taps, cin, ptr(out), dtype_code(dtype), stream_ptr()), "lb_refresh_shadows")
+    check(_C.lib.lb_refresh_shadows(ptr(src), ptr(tab), taps, cin, ptr(out), dtype_code(dtype), stream_ptr()),
+          "lb_refresh_shadows")
     _count()
     return out
 
@@ -311,53 +277,21 @@ def fused_conv2d(x_nhwc: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.T
     t = torch.empty((n * h * w, rp), device=x_nhwc.device, dtype=torch.float32) if want_t else None
     import ctypes
     up_ptr = ctypes.c_void_p(up.data_ptr() + 4 * up_off)
-    if rp != R_PAD:
-        if drop_p > 0.0:
-            assert t_in is None and not per_tap and up_gs == 0 and seed is not None and seed.dtype == torch.int64
-            check(_C.lib.lb_lora_conv2d_fwd_dropout_rp(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
-                                                       up_cs, ptr(diag), float(scale), ptr(y), ptr(t), n, h, w, cin,
-                                                       cout, kh, kw, pad_h, pad_w, r, rp, dtype_code(x_nhwc.dtype),
-                                                       dtype_code(out_dtype), float(drop_p), ptr(seed), stream_ptr()),
-                  "lb_lora_conv2d_fwd_dropout_rp")
-        else:
-            check(_C.lib.lb_lora_conv2d_fwd_rp(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs, up_cs,
-                                               up_gs, ptr(diag), float(scale), ptr(y), ptr(t), ptr(t_in), n, h, w,
-                                               cin, cout, kh, kw, pad_h, pad_w, r, rp, 1 if per_tap else 0,
-                                               dtype_code(x_nhwc.dtype), dtype_code(out_dtype), stream_ptr()),
-                  "lb_lora_conv2d_fwd_rp")
-        _count()
-        return y, t
     if drop_p > 0.0:     # forward with nn.Dropout on the branch: masked in the drain, one launch
         assert t_in is None and not per_tap and up_gs == 0 and seed is not None and seed.dtype == torch.int64
         check(_C.lib.lb_lora_conv2d_fwd_dropout(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
                                                 up_cs, ptr(diag), float(scale), ptr(y), ptr(t), n, h, w,
-                                                cin, cout, kh, kw, pad_h, pad_w, r, dtype_code(x_nhwc.dtype),
+                                                cin, cout, kh, kw, pad_h, pad_w, r, rp, dtype_code(x_nhwc.dtype),
                                                 dtype_code(out_dtype), float(drop_p), ptr(seed), stream_ptr()),
               "lb_lora_conv2d_fwd_dropout")
-        _count()
-        return y, t
-    check(_C.lib.lb_lora_conv2d_fwd(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
-                                    up_cs, up_gs, ptr(diag), float(scale), ptr(y), ptr(t), ptr(t_in),
-                                    n, h, w,
-                                    cin, cout, kh, kw, pad_h, pad_w, r, 1 if per_tap else 0,
-                                    dtype_code(x_nhwc.dtype), dtype_code(out_dtype), stream_ptr()),
-          "lb_lora_conv2d_fwd")
+    else:
+        check(_C.lib.lb_lora_conv2d_fwd(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
+                                        up_cs, up_gs, ptr(diag), float(scale), ptr(y), ptr(t), ptr(t_in),
+                                        n, h, w, cin, cout, kh, kw, pad_h, pad_w, r, rp, 1 if per_tap else 0,
+                                        dtype_code(x_nhwc.dtype), dtype_code(out_dtype), stream_ptr()),
+              "lb_lora_conv2d_fwd")
     _count()
     return y, t
-
-
-def wgrad_shift(S_rows: torch.Tensor, V: torch.Tensor, diag, scale: float, out: torch.Tensor,
-                out_off: int, out_js: int, out_cs: int, r: int, C: int, H: int, W: int, dy: int,
-                dx: int):
-    """Conv tap of the weight-gradient reduction (see lb_lora_wgrad_shift). S_rows: NHWC bytes."""
-    _req_cuda(S_rows, V, out)
-    M = V.shape[0]
-    import ctypes
-    out_ptr = ctypes.c_void_p(out.data_ptr() + 4 * out_off)
-    check(_C.lib.lb_lora_wgrad_shift(ptr(S_rows), ptr(V), ptr(diag), float(scale), out_ptr, out_js,
-                                     out_cs, M, C, r, H, W, dy, dx, dtype_code(S_rows.dtype),
-                                     stream_ptr()), "lb_lora_wgrad_shift")
-    _count()
 
 
 # ------------------------------------------------------------------------------------ dropout
@@ -368,14 +302,9 @@ def up_dropout_(y2d: torch.Tensor, T: torch.Tensor, up: torch.Tensor, up_rs: int
     M, N = y2d.shape
     rp = T.shape[1]
     assert y2d.is_contiguous() and seed.dtype == torch.int64
-    if rp == R_PAD:
-        check(_C.lib.lb_lora_up_dropout(ptr(y2d), dtype_code(y2d.dtype), ptr(T), ptr(up), up_rs, up_cs,
-                                        ptr(diag), float(scale), float(p), ptr(seed), M, N, r,
-                                        stream_ptr()), "lb_lora_up_dropout")
-    else:
-        check(_C.lib.lb_lora_up_dropout_rp(ptr(y2d), dtype_code(y2d.dtype), ptr(T), ptr(up), up_rs, up_cs,
-                                           ptr(diag), float(scale), float(p), ptr(seed), M, N, r, rp,
-                                           stream_ptr()), "lb_lora_up_dropout_rp")
+    check(_C.lib.lb_lora_up_dropout(ptr(y2d), dtype_code(y2d.dtype), ptr(T), ptr(up), up_rs, up_cs,
+                                    ptr(diag), float(scale), float(p), ptr(seed), M, N, r, rp,
+                                    stream_ptr()), "lb_lora_up_dropout")
     _count()
 
 
@@ -386,14 +315,9 @@ def dropout_dt(gy2d: torch.Tensor, up: torch.Tensor, up_rs: int, up_cs: int, p: 
     M, N = gy2d.shape
     rp = rank_pad(r)
     out = torch.empty((M, rp), device=gy2d.device, dtype=torch.float32)
-    if rp == R_PAD:
-        check(_C.lib.lb_lora_dropout_dt(ptr(gy2d), dtype_code(gy2d.dtype), ptr(up), up_rs, up_cs,
-                                        float(p), ptr(seed), ptr(out), M, N, r, stream_ptr()),
-              "lb_lora_dropout_dt")
-    else:
-        check(_C.lib.lb_lora_dropout_dt_rp(ptr(gy2d), dtype_code(gy2d.dtype), ptr(up), up_rs, up_cs,
-                                           float(p), ptr(seed), ptr(out), M, N, r, rp, stream_ptr()),
-              "lb_lora_dropout_dt_rp")
+    check(_C.lib.lb_lora_dropout_dt(ptr(gy2d), dtype_code(gy2d.dtype), ptr(up), up_rs, up_cs,
+                                    float(p), ptr(seed), ptr(out), M, N, r, rp, stream_ptr()),
+          "lb_lora_dropout_dt")
     _count()
     return out
 
@@ -406,14 +330,9 @@ def wgrad_masked(S: torch.Tensor, V: torch.Tensor, diag, scale: float, out: torc
         _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag, p, seed)
         return
     rp = V.shape[1]
-    if rp == R_PAD:
-        check(_C.lib.lb_lora_wgrad_masked(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
-                                          out_cs, M, C, r, float(p), ptr(seed), dtype_code(S.dtype),
-                                          stream_ptr()), "lb_lora_wgrad_masked")
-    else:
-        check(_C.lib.lb_lora_wgrad_masked_rp(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
-                                             out_cs, M, C, r, rp, float(p), ptr(seed), dtype_code(S.dtype),
-                                             stream_ptr()), "lb_lora_wgrad_masked_rp")
+    check(_C.lib.lb_lora_wgrad_masked(ptr(S), ptr(V), ptr(diag), float(scale), ptr(out), out_js,
+                                      out_cs, M, C, r, rp, float(p), ptr(seed), dtype_code(S.dtype),
+                                      stream_ptr()), "lb_lora_wgrad_masked")
     _count()
 
 
@@ -431,14 +350,9 @@ def wgrad_pair(x2d: torch.Tensor, dTs: torch.Tensor, dA: torch.Tensor, gy2d: tor
         return
     rp = dTs.shape[1]
     assert T.shape[1] == rp
-    if rp == R_PAD:
-        check(_C.lib.lb_lora_wgrad_pair(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
-                                        1, r, N, ptr(diag), float(scale), M, r, float(p), ptr(seed),
-                                        dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair")
-    else:
-        check(_C.lib.lb_lora_wgrad_pair_rp(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
-                                           1, r, N, ptr(diag), float(scale), M, r, rp, float(p), ptr(seed),
-                                           dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair_rp")
+    check(_C.lib.lb_lora_wgrad_pair(ptr(x2d), ptr(dTs), ptr(dA), K, 1, K, ptr(gy2d), ptr(T), ptr(dB),
+                                    1, r, N, ptr(diag), float(scale), M, r, rp, float(p), ptr(seed),
+                                    dtype_code(x2d.dtype), stream_ptr()), "lb_lora_wgrad_pair")
     _count()
 
 
@@ -537,12 +451,7 @@ def wgrad_conv(x_nhwc_rows: torch.Tensor, V: torch.Tensor, diag, scale: float, o
                        conv=(H, W, kh, kw, pad_h, pad_w))
         return
     rp = V.shape[1]
-    if rp == R_PAD:
-        check(_C.lib.lb_lora_wgrad_conv(ptr(x_nhwc_rows), ptr(V), ptr(diag), float(scale), ptr(out), M, C, r,
-                                        H, W, kh, kw, pad_h, pad_w, dtype_code(x_nhwc_rows.dtype), stream_ptr()),
-              "lb_lora_wgrad_conv")
-    else:
-        check(_C.lib.lb_lora_wgrad_conv_rp(ptr(x_nhwc_rows), ptr(V), ptr(diag), float(scale), ptr(out), M, C, r,
-                                           rp, H, W, kh, kw, pad_h, pad_w, dtype_code(x_nhwc_rows.dtype),
-                                           stream_ptr()), "lb_lora_wgrad_conv_rp")
+    check(_C.lib.lb_lora_wgrad_conv(ptr(x_nhwc_rows), ptr(V), ptr(diag), float(scale), ptr(out), M, C, r,
+                                    rp, H, W, kh, kw, pad_h, pad_w, dtype_code(x_nhwc_rows.dtype), stream_ptr()),
+          "lb_lora_wgrad_conv")
     _count()

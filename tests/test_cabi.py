@@ -32,21 +32,21 @@ def test_every_declared_symbol_is_exported():
         assert hasattr(lib, n), f"{n} declared in include/lora_b200.h but not exported"
 
 
-def test_argument_validation_without_gpu():
+def test_rank_padded_argument_validation_without_gpu():
     from lora_b200 import _C
     L = _C.lib
     buf = ctypes.create_string_buffer(4096)
     base = (ctypes.addressof(buf) + 255) & ~255
     p = ctypes.c_void_p(base)
     # rank out of range, bad dtype, misaligned K / pointer: refused before any CUDA call
-    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 64, 64, 17, 0, 0, None) == -2
-    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 64, 64, 4, 2, 0, None) == -3
-    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 60, 64, 4, 0, 0, None) == -1
+    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 64, 64, 17, 16, 0, 0, None) == -2
+    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 64, 64, 4, 16, 2, 0, None) == -3
+    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 60, 64, 4, 16, 0, 0, None) == -1
     assert L.lb_lora_linear_fwd(ctypes.c_void_p(base + 2), p, None, p, p, 4, 1, None, 1.0, p, None, None,
-                                8, 64, 64, 4, 0, 0, None) == -4
-    assert L.lb_lora_wgrad(p, p, None, 1.0, p, 1, 1, 8, 60, 4, 0, None) == -1
-    assert L.lb_lora_wgrad(p, p, None, 1.0, p, 1, 1, 8, 64, 0, 0, None) == -2
-    assert L.lb_cast_rows_pad16(p, 1, 1, p, 4, 64, 2, None) == -3
+                                8, 64, 64, 4, 16, 0, 0, None) == -4
+    assert L.lb_lora_wgrad(p, p, None, 1.0, p, 1, 1, 8, 60, 4, 16, 0, None) == -1
+    assert L.lb_lora_wgrad(p, p, None, 1.0, p, 1, 1, 8, 64, 0, 16, 0, None) == -2
+    assert L.lb_cast_rows_pad(p, 1, 1, p, 4, 16, 64, 2, None) == -3
     # frozen-weight block layout: host-side size query and refusals of the tiler
     assert L.lb_tiled_weight_elems(320, 768) == 5 * 12 * 64 * 64
     assert L.lb_tiled_weight_elems(1000, 136) == 16 * 3 * 64 * 64
@@ -55,7 +55,7 @@ def test_argument_validation_without_gpu():
     assert L.lb_tile_weight(p, 0, 64, 1, 64, 64, p, 2, None) == -3         # fp32 is not a 16-bit operand type
     assert L.lb_tile_weight(p, 0, 64, 1, 64, 64, ctypes.c_void_p(base + 2), 0, None) == -4
     # the LB_W_TILED flag does not hide a bad dtype
-    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 64, 64, 4, 0x100 | 2, 0, None) == -3
+    assert L.lb_lora_linear_fwd(p, p, None, p, p, 4, 1, None, 1.0, p, None, None, 8, 64, 64, 4, 16, 0x100 | 2, 0, None) == -3
 
 
 def test_missing_library_fails_loudly(tmp_path, monkeypatch):

@@ -66,33 +66,61 @@ def test_masked_mse_and_its_gradient(fmt, dtype, variant):
     assert p1.grad.stride() == p1.stride()
 
 
-def test_one_launch_optimizer_equals_three_launches():
-    """lb_optim_step_fused (cooperative: norm, grid barrier, AdamW + zero_grad, grid barrier, shadows)
-    against lb_adamw_clip_step (2 kernels) + lb_refresh_shadows: the same parameters, moments and shadows."""
+def _optimizer_run(sites_spec, mode):
+    """Three optimizer steps of a LoraArena over the same seeded gradients (the second one large
+    enough to clip). sites_spec: [("linear" | "conv", r)]; mode: "fused" (lb_optim_step_fused),
+    "split" (lb_adamw_clip_step + lb_refresh_shadows) or "dp" (lb_optim_step_dp at world = 1, with the
+    arena's own gradient buffer and a zeroed flag array as the only peer)."""
+    import ctypes
     import torch.nn as nn
     import lora_b200 as L
     from lora_b200.arena import LoraArena
-    results = []
-    for fused in (True, False):
-        torch.manual_seed(0)
-        sites = nn.ModuleList([L.LoraInjectedLinear(320, 640, r=4, dropout_p=0.0) for _ in range(5)] +
-                              [L.LoraInjectedConv2d(64, 96, 3, 1, 1, r=8, dropout_p=0.0)]).to(DEV)
-        for s in sites:
-            s.lora_up.weight.data.normal_(0, 0.1)
-        arena = LoraArena([(sites, 1e-3)])
-        arena.fused_step = fused
-        g = torch.Generator(device=DEV).manual_seed(5)
-        for step in range(3):
-            arena.g.copy_(torch.randn(arena.n, device=DEV, generator=g) * (2.0 if step == 1 else 0.01))
-            arena.step(0.9, 0.999, 1e-8, 1e-2, 1.0, world_size=1)
-        torch.cuda.synchronize()
-        assert float(arena.g.abs().max()) == 0.0 and int(arena.step_dev) == 3
-        results.append((arena.p.clone(), arena.m.clone(), arena.v.clone(), arena.shadow.clone(), float(arena.gnorm)))
+    torch.manual_seed(0)
+    sites = nn.ModuleList([L.LoraInjectedLinear(320, 640, r=r, dropout_p=0.0) if kind == "linear" else
+                           L.LoraInjectedConv2d(64, 96, 3, 1, 1, r=r, dropout_p=0.0)
+                           for kind, r in sites_spec]).to(DEV)
+    for s in sites:
+        s.lora_up.weight.data.normal_(0, 0.1)
+    arena = LoraArena([(sites, 1e-3)])
+    arena.fused_step = mode != "split"
+    if mode == "dp":
+        arena._dp_flags = torch.zeros(2, device=DEV, dtype=torch.int32)
+        arena._dp_epoch = torch.zeros(1, device=DEV, dtype=torch.int32)
+        arena.gsum = torch.zeros_like(arena.g)
+        one = ctypes.c_void_p * 1
+        arena._dp = (one(arena.g.data_ptr()), one(arena._dp_flags.data_ptr()), 1, 0)
+    g = torch.Generator(device=DEV).manual_seed(5)
+    for step in range(3):
+        arena.g.copy_(torch.randn(arena.n, device=DEV, generator=g) * (2.0 if step == 1 else 0.01))
+        arena.step(0.9, 0.999, 1e-8, 1e-2, 1.0, world_size=1)
+    torch.cuda.synchronize()
+    assert float(arena.g.abs().max()) == 0.0 and int(arena.step_dev) == 3
+    return arena.p.clone(), arena.m.clone(), arena.v.clone(), arena.shadow.clone(), float(arena.gnorm)
+
+
+def _assert_same_step(got, want):
     # same arithmetic; only the block partition of the sum of squares differs (fp32 order noise in
     # the clip coefficient), so parameters agree to ~1e-7 and the 16-bit shadows to one ulp
-    for a, b in zip(results[0][:3], results[1][:3]):
+    for a, b in zip(got[:3], want[:3]):
         assert float((a - b).norm() / (b.norm() + 1e-30)) < 2e-6
-    sa, sb = results[0][3].float(), results[1][3].float()
+    sa, sb = got[3].float(), want[3].float()
     assert float((sa - sb).abs().max()) <= 2.0 ** -7 * float(sb.abs().max())
     assert float((sa != sb).float().mean()) < 1e-3
-    assert abs(results[0][4] - results[1][4]) <= 1e-6 * abs(results[1][4])
+    assert abs(got[4] - want[4]) <= 1e-6 * abs(want[4])
+
+
+def test_one_launch_optimizer_equals_three_launches():
+    """lb_optim_step_fused (cooperative: norm, grid barrier, AdamW + zero_grad, grid barrier, shadows)
+    against lb_adamw_clip_step (2 kernels) + lb_refresh_shadows: the same parameters, moments and shadows,
+    with 16-row shadow slots only and with 32-row ones (r = 32 linear and conv sites)."""
+    for spec in ([("linear", 4)] * 5 + [("conv", 8)],
+                 [("linear", 4)] * 4 + [("linear", 32), ("conv", 32)]):
+        _assert_same_step(_optimizer_run(spec, "fused"), _optimizer_run(spec, "split"))
+
+
+def test_data_parallel_optimizer_at_world_one_equals_one_launch():
+    """lb_optim_step_dp with a single rank (its all-reduce reads only its own gradients) against
+    lb_optim_step_fused on an identical arena with an r = 4 and an r = 32 site: the same parameters,
+    moments and shadows."""
+    spec = [("linear", 4), ("conv", 32)]
+    _assert_same_step(_optimizer_run(spec, "dp"), _optimizer_run(spec, "fused"))

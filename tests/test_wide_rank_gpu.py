@@ -296,11 +296,11 @@ def _tiny_models(seed=0):
     return unet, text
 
 
-def test_extended_training_step_r32_matches_reference_step_tiny():
+def test_extended_training_step_r32_padded_shadow_table_matches_reference_step_tiny():
     """--use_extended_lora shape of the step at r = 32 (Linear + ResnetBlock2D Conv2d sites, rank pad
-    32, 8-column shadow table) vs the oracle's reference step, as the r = 4 test in
+    32, 32-row shadow slots) vs the oracle's reference step, as the r = 4 test in
     test_modules_gpu.py. The first-step factor gradients go through the deferred reduction queue
-    (lb_lora_wgrad_batch_rp) that LoraTrainStep runs; then two optimizer steps: losses, and every LoRA
+    (lb_lora_wgrad_batch) that LoraTrainStep runs; then two optimizer steps: losses, and every LoRA
     factor afterwards. Dropout is 0 on both sides (mask streams differ by design)."""
     import lora_b200 as L
     from lora_b200 import ops
@@ -329,7 +329,7 @@ def test_extended_training_step_r32_matches_reference_step_tiny():
         rs.down.data.copy_(o.lora_down.weight.data)
     cfg = StepConfig(use_cuda_graph=False, autocast_dtype=torch.bfloat16)
     tr = LoraTrainStep(unet, text, cfg, latent_shape=(1, 4, 16, 16), seq_len=77, device=DEV)
-    assert tr.arena.wide
+    assert int(tr.arena.table[:, 7].max()) == 32
     ref = RefDreamboothStep(unet_r, text_r, DDPMNoiser(device=DEV), us, ts, autocast_dtype=torch.bfloat16)
     lat = torch.randn(1, 4, 16, 16, device=DEV) * 0.18215
     ids = torch.randint(0, 1000, (1, 77), device=DEV)
