@@ -245,6 +245,44 @@ int lb_ti_embed_step(float* rows, float* grad, float* m, float* v, const long lo
                      float eps, float weight_decay, int* step_dev, int clip_decay, float target_norm,
                      void* stream);
 
+/* ---- sparse, exact AdamW over the token-embedding table (pivotal tuning's `continue_inversion`,
+ * train_lora_w_ti.py). The claimed rows are one more param-group of the LoRA arena: `master` and
+ * `slot_grad` are that group's [capacity, D] fp32 slices of the arena's p and g, and the unchanged
+ * lb_optim_step_fused launch clips and updates them with the LoRA factors. Device-resident state:
+ *   slot_of  int32 [V] (token -> slot, -1 = unclaimed), slot_tok int32 [capacity] (slot -> token),
+ *   state    int32 [4] {claimed, claimed after this step's scatter, flush ticket (zero), flags},
+ *            flags bit 0 = a token found no free slot (sticky; its gradient was dropped),
+ *            bit 1 = an id outside [0, V) was skipped,
+ *   decay    fp64  [1] product of the per-step decay factors fl32(1 - lr*wd) since the last flush.
+ * An unclaimed row's stored value times `decay` is what dense AdamW would hold in it (its gradient
+ * and moments are zero, so only the decoupled weight decay has moved it). */
+
+/* Backward of the embedding lookup, one launch (replaces the dense [V, D] gradient autograd builds
+ * for text_encoder.get_input_embeddings().weight, cli_lora_pti.py:596-606 / train_lora_w_ti.py:1052):
+ * ids int64 [n_tok] (n_tok = B*S <= 2048), grad [n_tok, D] of grad_dtype (LB_F32/LB_BF16/LB_F16).
+ * For every distinct token, the gradient rows of its positions are summed in position order (fp32,
+ * no atomics: bitwise deterministic) and ADDED to slot_grad[slot]. A token without a slot claims the
+ * next one, in first-occurrence order, and its master becomes table[tok] * decay (table_dtype).
+ * Reads state[0], writes state[1] (lb_embed_rows_write_back commits it). Past capacity, flag bit 0 is
+ * set and that token's gradient is dropped; nothing is written out of bounds. */
+int lb_embed_rows_scatter(const long long* ids, const void* grad, int grad_dtype, int n_tok, int D, int V,
+                          int* slot_of, int* slot_tok, int capacity, int* state, const void* table,
+                          int table_dtype, const double* decay, float* master, float* slot_grad, void* stream);
+
+/* After the optimizer launch, one launch: table[slot_tok[s]] = master[s] (cast to table_dtype) for the
+ * first n_write claimed slots (n_write < 0: every claimed slot), state[0] = state[1], and, when decay
+ * and lr_dev are given, decay *= (double) fl32(1 - lr_dev[lr_index] * weight_decay) -- the factor the
+ * optimizer applied to every row this step. Writing back only the placeholder slots (claimed first)
+ * leaves every other row bit-identical, which is train_lora_w_ti.py:1070-1075's restore. */
+int lb_embed_rows_write_back(const float* master, const int* slot_tok, int capacity, int* state, int n_write,
+                             void* table, int table_dtype, int D, int V, double* decay, const float* lr_dev,
+                             int lr_index, float weight_decay, void* stream);
+
+/* One launch over the table: table[row] *= decay for every unclaimed row, then decay = 1. Makes the
+ * whole table what dense AdamW (cli_lora_pti.py:958-997, every row decays every step) would hold. */
+int lb_embed_rows_flush(void* table, int table_dtype, int V, int D, const int* slot_of, double* decay, int* state,
+                        void* stream);
+
 /* Fold a LoRA into its frozen weight: out[n,k] = W[n,k] + alpha * sum_j up[n,j]*down[j,k]
  * (W, out: LB_F32/LB_BF16/LB_F16 [N,K]; conv weights flattened to [Cout, Cin*kh*kw]; out may alias W;
  * 1 <= r <= 64).

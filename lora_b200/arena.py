@@ -42,7 +42,10 @@ class LoraArena:
     the reference builds them (unet first, then text encoder: train_lora_dreambooth.py:659-669)."""
 
     def __init__(self, groups: Sequence[Tuple[object, float]], compute_dtype=torch.bfloat16,
-                 device: Optional[torch.device] = None):
+                 device: Optional[torch.device] = None, rows: Optional[Tuple[int, int, float]] = None):
+        """rows: (capacity, D, lr) appends one more param-group of `capacity` fp32 rows of width D
+        after the LoRA groups -- the claimed token-embedding rows of lora_b200.embed_rows, clipped
+        and updated by the same optimizer launch (`rows_group`, `rows_master`, `rows_grad`)."""
         self.compute_dtype = compute_dtype
         site_groups: List[List[nn.Module]] = []
         for model, _ in groups:
@@ -66,6 +69,16 @@ class LoraArena:
                     self.entries.append((s, which, holder, off, w.numel()))
                     off = _round_up(off + w.numel(), _ALIGN)
             self.group_off.append(off)
+        lrs = [float(lr) for _, lr in groups]
+        self.rows_group = None
+        if rows is not None:
+            cap, width, rows_lr = int(rows[0]), int(rows[1]), float(rows[2])
+            if cap <= 0 or width <= 0:
+                raise _C.LoraB200Error(f"LoraArena: rows=(capacity={cap}, D={width}) must be positive")
+            self.rows_group, self.rows_shape = len(lrs), (cap, width)
+            off = _round_up(off + cap * width, _ALIGN)
+            self.group_off.append(off)
+            lrs.append(rows_lr)
         self.n = off
         self.n_params = sum(e[4] for e in self.entries)
         dev = self.device
@@ -73,8 +86,8 @@ class LoraArena:
         self.g = torch.zeros_like(self.p)
         self.m = torch.zeros_like(self.p)
         self.v = torch.zeros_like(self.p)
-        self.lr = torch.tensor([float(lr) for _, lr in groups], device=dev, dtype=torch.float32)
-        self.base_lr = [float(lr) for _, lr in groups]
+        self.lr = torch.tensor(lrs, device=dev, dtype=torch.float32)
+        self.base_lr = lrs
         self.step_dev = torch.zeros(1, device=dev, dtype=torch.int32)
         self.partials = torch.zeros(1024, device=dev, dtype=torch.float32)
         self.gnorm = torch.zeros(1, device=dev, dtype=torch.float32)
@@ -215,6 +228,14 @@ class LoraArena:
             if s is site and w == which:
                 return o
         raise KeyError
+
+    def rows_view(self, buf: torch.Tensor) -> torch.Tensor:
+        """[capacity, D] view of the rows group inside one of the flat buffers (p, g, m or v)."""
+        if self.rows_group is None:
+            raise _C.LoraB200Error("LoraArena was built without rows=")
+        o = self.group_off[self.rows_group]
+        cap, width = self.rows_shape
+        return buf[o:o + cap * width].view(cap, width)
 
     def _gview(self, site, which):
         for s, w, holder, o, n in self.entries:

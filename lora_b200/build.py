@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "liblora_b200.so")
 STAMP = os.path.join(HERE, ".liblora_b200.stamp")
 
-SOURCES = ["fused_linear.cu", "fused_conv.cu", "lora_aux.cu", "svd.cu", "svd_batched.cu", "step_glue.cu"]
+SOURCES = ["fused_linear.cu", "fused_conv.cu", "lora_aux.cu", "svd.cu", "svd_batched.cu", "step_glue.cu", "embed_rows.cu"]
 # every header under csrc/ takes part in the rebuild digest (a stale .so after a header edit is silent)
 HEADERS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [
     os.path.join(ROOT, "include", "lora_b200.h")]

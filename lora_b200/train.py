@@ -88,6 +88,11 @@ class StepConfig:
 class LoraTrainStep:
     """One data-parallel replica of the LoRA fine-tuning step (bs = latents.shape[0] per GPU)."""
 
+    # run the text encoder with gradients even when it has no trained LoRA factors
+    _text_encoder_grad = False
+    # LoraArena's rows= argument (capacity, D, lr) of a step that trains embedding rows too
+    _arena_rows = None
+
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, cfg: StepConfig,
                  latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
         self.cfg = cfg
@@ -98,7 +103,8 @@ class LoraTrainStep:
         groups = [(unet, cfg.learning_rate)]
         if cfg.train_text_encoder:
             groups.append((text_encoder, cfg.learning_rate_text))
-        self.arena = LoraArena(groups, compute_dtype=cfg.compute_dtype, device=self.device)
+        self.arena = LoraArena(groups, compute_dtype=cfg.compute_dtype, device=self.device,
+                               rows=self._arena_rows)
         self.noiser = DDPMNoiser(device=self.device)
         self.model_dtype = next(unet.parameters()).dtype
         # static step I/O (graph-stable addresses)
@@ -172,7 +178,7 @@ class LoraTrainStep:
         ac = (torch.autocast("cuda", dtype=cfg.autocast_dtype) if cfg.autocast_dtype is not None
               else torch.autocast("cuda", enabled=False))
         with ac:
-            if cfg.train_text_encoder:
+            if cfg.train_text_encoder or self._text_encoder_grad:
                 ehs = self.text_encoder(self.input_ids)[0]
             else:
                 with torch.no_grad():
@@ -330,12 +336,16 @@ class LoraTrainStep:
                        float(max(1, cfg.max_train_steps - cfg.lr_warmup_steps)))
         return 1.0
 
-    def step_device(self) -> torch.Tensor:
-        """One step on inputs already resident in self.latents / self.input_ids."""
+    def _set_step_lr(self):
+        """Per-group learning rates of the step about to run (iteration self.global_step)."""
         if self.cfg.lr_scheduler != "constant":
             k = self.global_step + (1 if self.cfg.lr_step_first else 0)
             mult = self.lr_multiplier(k)                     # host-side schedule, tiny async H2D copy
             self.arena.set_lr([b * mult for b in self.arena.base_lr])
+
+    def step_device(self) -> torch.Tensor:
+        """One step on inputs already resident in self.latents / self.input_ids."""
+        self._set_step_lr()
         self.global_step += 1
         if self.graph is not None:
             self.graph.replay()
@@ -433,3 +443,128 @@ class TextualInversionStep(LoraTrainStep):
         for prm in self._frozen:
             prm.requires_grad_(True)
         self._frozen = []
+
+
+class LoraEmbeddingStep(LoraTrainStep):
+    """The LoRA step with the CLIP token-embedding table trained by the same AdamW and clipped by the
+    same clip_grad_norm_ as the factors -- the reference's two joint configurations:
+
+      mode="table"         cli_lora_pti.py phase 2 with `--continue_inversion` (:958-997 optimizer,
+                           :545-620 loop): lr_scheduler.step() first, loss_step(t_mutliplier=0.8),
+                           backward, clip over UNet + text encoder, AdamW(weight_decay_lora) over
+                           [unet LoRA, table (+ text LoRA)]; every row decays every step, nothing
+                           is restored.
+          LoraEmbeddingStep(unet, text_encoder, placeholder_ids,
+                            StepConfig(learning_rate=unet_lr, learning_rate_text=text_encoder_lr,
+                                       train_text_encoder=train_text_encoder,
+                                       adam_weight_decay=weight_decay_lora, t_multiplier=0.8,
+                                       lr_step_first=True, lr_scheduler="linear", ...),
+                            lr_embedding=continue_inversion_lr or ti_lr, mode="table")
+
+      mode="placeholders"  train_lora_w_ti.py (:830-853 optimizer, :986-1075 loop): before
+                           iteration k < unfreeze_lora_step the LoRA groups get lr 0 (moments still
+                           move, gradients still enter the norm) and the table runs at
+                           lr_ti * lambda(k); from then on the LoRA groups run at their base lr
+                           (unscheduled) and the table at 0. clip, AdamW, lr_scheduler.step(); every
+                           row except the placeholders is restored.
+          LoraEmbeddingStep(unet, text_encoder, [placeholder_token_id],
+                            StepConfig(learning_rate=learning_rate, learning_rate_text=learning_rate_text,
+                                       train_text_encoder=True, adam_weight_decay=adam_weight_decay,
+                                       lr_scheduler=lr_scheduler, lr_warmup_steps=..., max_train_steps=...),
+                            lr_embedding=learning_rate_ti, mode="placeholders",
+                            unfreeze_lora_step=unfreeze_lora_step)
+
+    The table keeps requires_grad=False; the rows that get a gradient are claimed into
+    `row_capacity` slots of the arena (lora_b200/embed_rows.py). Per step this adds two launches
+    to the plain step: the gradient scatter (in backward) and the write-back (after the optimizer).
+    Mode "table" leaves the decay of unseen rows pending: call `flush()` before reading the table
+    outside the step (validation, saving a full text encoder); `release()` flushes too. Single
+    process only (each rank would claim its own slots)."""
+
+    _text_encoder_grad = True
+
+    def __init__(self, unet: nn.Module, text_encoder: nn.Module, placeholder_token_ids, cfg: StepConfig,
+                 lr_embedding: float, mode: str = "table", unfreeze_lora_step: Optional[int] = None,
+                 row_capacity: int = 1024, latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
+        from .embed_rows import MODES, EmbeddingRows
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise ValueError("LoraEmbeddingStep runs in one process: data-parallel ranks would claim "
+                             "different embedding rows")
+        if mode not in MODES:
+            raise ValueError(f"mode {mode!r}: one of {MODES}")
+        if mode == "placeholders" and not cfg.train_text_encoder:
+            raise ValueError("mode='placeholders' (train_lora_w_ti.py) needs StepConfig.train_text_encoder=True: "
+                             "without it the script clips the UNet factors only but updates the table too")
+        if mode == "table" and unfreeze_lora_step is not None:
+            raise ValueError("unfreeze_lora_step belongs to mode='placeholders'")
+        self.mode = mode
+        self.unfreeze_lora_step = (500 if unfreeze_lora_step is None else int(unfreeze_lora_step)) \
+            if mode == "placeholders" else None        # train_lora_w_ti.py:570-574 default
+        D = text_encoder.get_input_embeddings().weight.shape[1]
+        self._arena_rows = (int(row_capacity), int(D), float(lr_embedding))
+        super().__init__(unet, text_encoder, cfg, latent_shape=latent_shape, seq_len=seq_len, device=device)
+        self.rows = EmbeddingRows(text_encoder, self.arena, placeholder_token_ids, mode=mode,
+                                  weight_decay=cfg.adam_weight_decay)
+        # overflow flag of the last two step_host calls (pinned, copied without a synchronise)
+        self._h_flags = [torch.zeros(1, dtype=torch.int32).pin_memory() for _ in range(2)]
+        self._flag_events = [None, None]
+        self._host_calls = 0
+
+    def _set_step_lr(self):
+        if self.mode == "table":
+            return super()._set_step_lr()
+        cfg = self.cfg
+        k = self.global_step
+        mult = 1.0
+        if cfg.lr_scheduler != "constant":
+            mult = self.lr_multiplier(k + (1 if cfg.lr_step_first else 0))
+        base, rg = self.arena.base_lr, self.arena.rows_group
+        if k < self.unfreeze_lora_step:          # train_lora_w_ti.py:988-991
+            lrs = [0.0] * len(base)
+            lrs[rg] = base[rg] * mult
+        else:                                    # :992-995: LoRA at its base lr, table frozen
+            lrs = list(base)
+            lrs[rg] = 0.0
+        self.arena.set_lr(lrs)
+
+    def _update(self):
+        super()._update()
+        self.rows.write_back()
+
+    def _snapshot(self):
+        snap = super()._snapshot()
+        snap["rows"] = self.rows.snapshot()
+        return snap
+
+    def _restore(self, snap):
+        self.rows.restore(snap["rows"])
+        super()._restore(snap)
+
+    def step_host(self, latents_cpu: torch.Tensor, input_ids_cpu: torch.Tensor) -> torch.Tensor:
+        """LoraTrainStep.step_host; an overflow of the row slots in this step raises no later than the
+        next call (the flag is copied to pinned memory behind the step and read one call later)."""
+        out = super().step_host(latents_cpu, input_ids_cpu)
+        i = self._host_calls % 2
+        self._h_flags[i].copy_(self.rows.state[3:4], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._flag_events[i] = ev
+        self._host_calls += 1
+        prev = self._flag_events[1 - i]
+        if prev is not None:                     # the previous step: finished or about to (this one is queued)
+            prev.synchronize()
+            self.rows.raise_for_flags(int(self._h_flags[1 - i][0]))
+        return out
+
+    def flush(self):
+        """Apply the pending decay to the rows no gradient has touched yet (mode "table") and check
+        for an overflow of the row slots: the table then holds what dense AdamW would."""
+        self.rows.flush()
+
+    def release(self):
+        """End of training: flush, then drop the lookup hook."""
+        try:
+            self.flush()
+        finally:
+            self.rows.remove()

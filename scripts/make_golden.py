@@ -17,6 +17,10 @@ Outputs (all small, committed):
   golden/pti_loss_step.pt               cli_lora_pti.loss_step losses (plain / t_mult / masked / inpainting)
   golden/ti_train_inversion.pt          cli_lora_pti.train_inversion: 3 real steps (grads, lr, rows after)
   golden/pti_perform_tuning.pt          cli_lora_pti.perform_tuning: 3 real steps (losses, lrs, all factors after)
+  golden/pti_continue_inversion.pt      the same loop with continue_inversion: 3 real steps (losses, lrs,
+                                        the whole token-embedding table after each)
+
+`python scripts/make_golden.py continue_inversion` regenerates one file only.
 """
 import hashlib
 import importlib.util
@@ -464,16 +468,103 @@ def gen_tuning(R):
     print("tuning", [(r["loss"], r["lrs"]) for r in rec], len(sites))
 
 
+def gen_continue_inversion(R):
+    """LoRA-tuning phase with `continue_inversion=True`: the reference's own `perform_tuning` loop
+    (cli_lora_pti.py:545-620) for 3 steps, CPU fp32, with the param groups and requires_grad flags
+    built as at :958-997 -- [unet LoRA (1e-4), the whole token-embedding table (continue_inversion_lr
+    5e-3), text LoRA (1e-5)], one AdamW(weight_decay_lora=1e-3), encoder / final layer norm /
+    position embedding frozen -- and a LambdaLR linear decay. Recorded: per-step loss and per-group
+    lr, and the full table after every step."""
+    from lora_b200.host.clip import build_text_encoder
+    from lora_b200.host.ddpm import DDPMNoiser
+    from lora_b200.host.unet_sd15 import UNet2DConditionModel, UNetConfig
+    P = load_ref_pti(R)
+    noiser = DDPMNoiser(device="cpu")
+
+    class Sched:
+        config = types.SimpleNamespace(num_train_timesteps=noiser.num_train_timesteps, prediction_type="epsilon")
+        add_noise = staticmethod(noiser.add_noise)
+
+    torch.manual_seed(0)
+    unet = UNet2DConditionModel(UNetConfig.tiny())
+    text = build_text_encoder(tiny=True)
+    unet.requires_grad_(False)
+    up, _ = R.inject_trainable_lora(unet, r=4)
+    params = [{"params": itertools.chain(*up), "lr": 1e-4}]
+    text.requires_grad_(False)
+    params.append({"params": text.get_input_embeddings().parameters(), "lr": 5e-3})      # :962-971
+    text.requires_grad_(True)
+    for prm in itertools.chain(text.text_model.encoder.parameters(), text.text_model.final_layer_norm.parameters(),
+                               text.text_model.embeddings.position_embedding.parameters()):
+        prm.requires_grad = False
+    tp, _ = R.inject_trainable_lora(text, target_replace_module={"CLIPAttention"}, r=4)
+    params.append({"params": itertools.chain(*tp), "lr": 1e-5})
+    gg = torch.Generator().manual_seed(6)
+    sites = [m for m in list(unet.modules()) + list(text.modules()) if type(m).__name__ == "LoraInjectedLinear"]
+    for m in sites:
+        m.lora_down.weight.data.normal_(0, 0.25, generator=gg)
+        m.lora_up.weight.data.normal_(0, 0.05, generator=gg)
+    opt = torch.optim.AdamW(params, weight_decay=1e-3)
+    sched = torch.optim.lr_scheduler.LambdaLR(opt, lambda k: max(0.0, 1.0 - k / 6))
+    emb = text.get_input_embeddings()
+    V = emb.weight.shape[0]
+    tok = [V - 2, V - 1]
+    g = torch.Generator().manual_seed(23)
+    batches = []
+    for _ in range(3):
+        ids = torch.randint(0, V - 2, (2, 77), generator=g)
+        ids[0, 4], ids[1, 6] = tok[0], tok[1]
+        batches.append({"pixel_values": torch.randn(2, 4, 8, 8, generator=g) * 0.18215, "input_ids": ids})
+    table0 = emb.weight.detach().clone()
+    rec = []
+
+    class Recording:                    # lr_scheduler_lora: stepped first, snapshots the table it finds
+        def step(self_inner):
+            if rec:
+                rec[-1]["table_after"] = emb.weight.detach().clone()
+            sched.step()
+            rec.append(dict(lrs=[grp["lr"] for grp in opt.param_groups]))
+
+        def get_last_lr(self_inner):
+            return sched.get_last_lr()
+
+    real_loss_step = P.loss_step
+
+    def spy(*a, **k):
+        out = real_loss_step(*a, **k)
+        rec[-1]["loss"] = float(out.detach())
+        rec[-1]["kwargs"] = {kk: vv for kk, vv in k.items() if isinstance(vv, (int, float, bool))}
+        return out
+
+    P.loss_step = spy
+    torch.manual_seed(1001)
+    import contextlib, io
+    try:
+        with contextlib.redirect_stdout(io.StringIO()):
+            P.perform_tuning(unet, None, text, batches, 3, Sched, opt, 10 ** 9, tok, ["<a>", "<b>"], "/nonexistent",
+                             Recording(), {"CrossAttention", "Attention", "GEGLU"}, {"CLIPAttention"}, 1.0,
+                             "out", None, "/nonexistent", True)
+    finally:
+        P.loss_step = real_loss_step
+    rec[-1]["table_after"] = emb.weight.detach().clone()
+    assert len(rec) == 3 and rec[0]["kwargs"]["t_mutliplier"] == 0.8
+    assert not torch.equal(rec[0]["table_after"], table0)
+    torch.save(dict(model_seed=0, factor_seed=6, step_seed=1001, n_unet_sites=len(up) // 2, token_ids=tok,
+                    lrs0=[1e-4, 5e-3, 1e-5], weight_decay=1e-3, table0=table0, batches=batches, steps=rec),
+               f"{OUT}/pti_continue_inversion.pt")
+    print("continue_inversion", [(r["loss"], r["lrs"]) for r in rec])
+
+
+GENERATORS = {"ops": gen_ops, "ctor_rng": gen_ctor_rng, "inject": gen_inject, "manifest": gen_manifest,
+              "svd": gen_svd, "adamw": gen_adamw, "loss_step": gen_loss_step, "ti": gen_ti, "tuning": gen_tuning,
+              "continue_inversion": gen_continue_inversion}
+
+
 if __name__ == "__main__":
+    # `python scripts/make_golden.py [name ...]` regenerates only the named files
     R = load_ref_lora()
-    gen_ops(R)
-    gen_ctor_rng(R)
-    gen_inject(R)
-    gen_manifest(R)
-    gen_svd(R)
-    gen_adamw()
-    gen_loss_step(R)
-    gen_ti(R)
-    gen_tuning(R)
+    for name in (sys.argv[1:] or list(GENERATORS)):
+        fn = GENERATORS[name]
+        fn() if fn is gen_adamw else fn(R)
     for fn in sorted(os.listdir(OUT)):
         print(fn, os.path.getsize(f"{OUT}/{fn}"))
