@@ -1,7 +1,9 @@
 """ORACLE (test infrastructure only -- never imported by the product path).
 
 CPU restatement of the arithmetic of the reference's LoRA hot path, written as explicit matrix
-formulas in float64 (torch CPU tensors used as plain ndarrays; no autograd, no nn.Module).
+formulas in float64 (torch CPU tensors used as plain ndarrays; no autograd, no nn.Module). The
+forward / backward restatements take `device=`: the same float64 formulas on another device, for the
+kernel tests at full SD1.5 conv sizes, where CPU float64 convolutions would dominate the run time.
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import
 this package.
 
@@ -18,19 +20,19 @@ import torch
 F64 = torch.float64
 
 
-def _f(x):
-    return None if x is None else x.detach().to("cpu", F64)
+def _f(x, device="cpu"):
+    return None if x is None else x.detach().to(device, F64)
 
 
-def selector_matrix(diag: Optional[torch.Tensor], r: int) -> torch.Tensor:
+def selector_matrix(diag: Optional[torch.Tensor], r: int, device="cpu") -> torch.Tensor:
     """lora_diffusion/lora.py:63-70 -- selector is Identity or a Linear whose weight is diag(d)."""
     if diag is None:
-        return torch.eye(r, dtype=F64)
-    return torch.diag(_f(diag))
+        return torch.eye(r, dtype=F64, device=device)
+    return torch.diag(_f(diag, device))
 
 
 def lora_linear_forward(x, W, bias, A, B, scale: float, diag=None, keep_mask=None,
-                        dropout_p: float = 0.0):
+                        dropout_p: float = 0.0, device="cpu"):
     """lora_diffusion/lora.py:53-58.
 
         y = x W^T (+ b) + dropout( ((x A^T) S^T) B^T ) * scale
@@ -38,10 +40,11 @@ def lora_linear_forward(x, W, bias, A, B, scale: float, diag=None, keep_mask=Non
     x: [M,K]; W: [N,K]; A = lora_down.weight [r,K]; B = lora_up.weight [N,r]; S = selector weight.
     dropout (lora.py:45,56): keep_mask in {0,1}^[M,N] applied to the LoRA branch and rescaled by
     1/(1-p); None means eval mode or p == 0.
+    device: where the float64 arithmetic runs (the result lives there too).
     """
-    x, W, A, B, bias = _f(x), _f(W), _f(A), _f(B), _f(bias)
+    x, W, A, B, bias = (_f(t, device) for t in (x, W, A, B, bias))
     r = A.shape[0]
-    S = selector_matrix(diag, r)
+    S = selector_matrix(diag, r, device)
     base = x @ W.T
     if bias is not None:
         base = base + bias
@@ -49,12 +52,12 @@ def lora_linear_forward(x, W, bias, A, B, scale: float, diag=None, keep_mask=Non
     t = t @ S.T                      # selector (nn.Linear: y = t S^T)
     u = t @ B.T                      # lora_up
     if keep_mask is not None:
-        u = u * _f(keep_mask) / (1.0 - dropout_p)
+        u = u * _f(keep_mask, device) / (1.0 - dropout_p)
     return base + u * scale
 
 
 def lora_linear_backward(gy, x, W, A, B, scale: float, diag=None, keep_mask=None,
-                         dropout_p: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                         dropout_p: float = 0.0, device="cpu") -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Autograd of lora.py:53-58 with W, b frozen (train_lora_dreambooth.py:595): returns
     (dX, dA, dB). No dW.
 
@@ -62,12 +65,12 @@ def lora_linear_backward(gy, x, W, A, B, scale: float, diag=None, keep_mask=None
         dT = gU B S                         dA = dT^T x
         dX = gY W + dT A
     """
-    gy, x, W, A, B = _f(gy), _f(x), _f(W), _f(A), _f(B)
+    gy, x, W, A, B = (_f(t, device) for t in (gy, x, W, A, B))
     r = A.shape[0]
-    S = selector_matrix(diag, r)
+    S = selector_matrix(diag, r, device)
     gu = gy * scale
     if keep_mask is not None:
-        gu = gu * _f(keep_mask) / (1.0 - dropout_p)
+        gu = gu * _f(keep_mask, device) / (1.0 - dropout_p)
     t_sel = (x @ A.T) @ S.T
     dB = gu.T @ t_sel
     dT = (gu @ B) @ S
@@ -83,24 +86,25 @@ def _conv2d_naive(x, w, stride, padding, dilation):
 
 
 def lora_conv2d_forward(x, W, bias, A, B, scale: float, stride=1, padding=0, dilation=1,
-                        diag=None, keep_mask=None, dropout_p: float = 0.0):
+                        diag=None, keep_mask=None, dropout_p: float = 0.0, device="cpu"):
     """lora_diffusion/lora.py:130-135.
 
     x: [N,Cin,H,W]; W: [Cout,Cin,kh,kw]; A = lora_down.weight [r,Cin,kh,kw] (same stride/padding/
     dilation as the base conv, lora.py:105-114); B = lora_up.weight [Cout,r,1,1] (1x1, lora.py:116-123).
     The selector, when set, is a 1x1 conv with weight diag(d) (lora.py:140-156).
+    device: where the float64 arithmetic runs (the result lives there too).
     """
-    x, W, A, B, bias = _f(x), _f(W), _f(A), _f(B), _f(bias)
+    x, W, A, B, bias = (_f(t, device) for t in (x, W, A, B, bias))
     r = A.shape[0]
     base = _conv2d_naive(x, W, stride, padding, dilation)
     if bias is not None:
         base = base + bias.view(1, -1, 1, 1)
     t = _conv2d_naive(x, A, stride, padding, dilation)           # [N,r,Ho,Wo]
-    S = selector_matrix(diag, r)
+    S = selector_matrix(diag, r, device)
     t = torch.einsum("nchw,dc->ndhw", t, S)
     u = torch.einsum("nrhw,or->nohw", t, B.reshape(B.shape[0], r))
     if keep_mask is not None:
-        u = u * _f(keep_mask) / (1.0 - dropout_p)
+        u = u * _f(keep_mask, device) / (1.0 - dropout_p)
     return base + u * scale
 
 
@@ -148,7 +152,7 @@ def collapse_delta(A, B, alpha: float = 1.0):
 
 
 def lora_conv2d_backward(gy, x, W, A, B, scale: float, stride=1, padding=0, dilation=1, diag=None,
-                         keep_mask=None, dropout_p: float = 0.0):
+                         keep_mask=None, dropout_p: float = 0.0, device="cpu"):
     """Autograd of lora.py:130-135 with the base conv frozen: returns (dX, dA, dB), written with
     the explicit transposed-convolution / weight-gradient operators (float64, no autograd graph).
 
@@ -157,14 +161,14 @@ def lora_conv2d_backward(gy, x, W, A, B, scale: float, stride=1, padding=0, dila
         dA = conv_weight_grad(x, dT) ;  dX = conv_input_grad(gY, W) + conv_input_grad(dT, A)
     """
     from torch.nn import grad as G
-    gy, x, W, A, B = _f(gy), _f(x), _f(W), _f(A), _f(B)
+    gy, x, W, A, B = (_f(t, device) for t in (gy, x, W, A, B))
     r = A.shape[0]
-    S = selector_matrix(diag, r)
+    S = selector_matrix(diag, r, device)
     t = _conv2d_naive(x, A, stride, padding, dilation)
     t_sel = torch.einsum("nchw,dc->ndhw", t, S)
     gu = gy * scale
     if keep_mask is not None:                 # nn.Dropout on the branch (lora.py:115,133): same mask
-        gu = gu * _f(keep_mask) / (1.0 - dropout_p)
+        gu = gu * _f(keep_mask, device) / (1.0 - dropout_p)
     B2 = B.reshape(B.shape[0], r)
     dB = torch.einsum("nohw,njhw->oj", gu, t_sel).reshape(B.shape)
     dT = torch.einsum("nohw,oj->njhw", gu, B2)
