@@ -424,6 +424,16 @@ int lb_step_prologue(const float* latents, const float* noise, const long long* 
                      const float* inpaint_mask, const float* masked_latents, void* out, int out_dtype,
                      int B, int C, int H, int W, void* stream);
 
+/* lb_step_prologue plus the v-prediction target of the same timesteps (cli_lora_pti.py:333-338,
+ * diffusers' DDPMScheduler.get_velocity), in the same launch:
+ *   velocity[b, c, h, w] = sqrt_acp[t_b] * noise[b, c, h, w] - sqrt_one_minus_acp[t_b] * latents[b, c, h, w]
+ * fp32 NCHW (the target layout lb_masked_mse_fwd_bwd reads), two rounded products and one rounded
+ * difference: equal to torch's evaluation bit for bit. velocity NULL: LB_ERR_SHAPE. */
+int lb_step_prologue_v(const float* latents, const float* noise, const long long* timesteps,
+                       const float* sqrt_acp, const float* sqrt_one_minus_acp, int n_timesteps,
+                       const float* inpaint_mask, const float* masked_latents, void* out, int out_dtype,
+                       float* velocity, int B, int C, int H, int W, void* stream);
+
 /* Loss epilogue, one launch (cli_lora_pti.py:340-370, train_lora_dreambooth.py:855-875):
  *   loss = sum_b weights[b] * mean_{c,h,w} (mask[b,h,w] * (pred - target))^2      (weights NULL: 1/B)
  *   grad = d loss / d pred = 2 weights[b] mask^2 (pred - target) / (C H W)        (pred's dtype/layout)

@@ -1,6 +1,8 @@
 // The two ends of a training step, either side of the UNet call:
 //   lb_step_prologue      scheduler.add_noise + cast + NCHW -> NHWC (+ the inpainting concat)
 //                         cli_lora_pti.py:295-313, train_lora_dreambooth.py:822-840
+//   lb_step_prologue_v    the same, plus the v-prediction target scheduler.get_velocity
+//                         cli_lora_pti.py:333-338, train_lora_dreambooth.py:846-853
 //   lb_masked_mse_fwd_bwd the (mask-weighted) MSE of cli_lora_pti.py:340-370 /
 //                         train_lora_dreambooth.py:855-875 and its gradient w.r.t. the prediction,
 //                         in one pass (the loss is a scalar: its backward is known in the forward)
@@ -28,11 +30,12 @@ __device__ __forceinline__ void st_any(void* p, long long i, int dt, float x) {
 
 // out[b, p, c] (NHWC, C_out = C or C + 1 + C) = sqrt_acp[t_b] * x0[b, c, p] + sqrt_1m[t_b] * eps[b, c, p]
 // for c < C; channel C = inpaint mask[b, p]; channels C+1.. = masked-image latents[b, c', p].
+// velocity (optional, fp32 NCHW like x0): v[b, c, p] = sqrt_acp[t_b] * eps[b, c, p] - sqrt_1m[t_b] * x0[b, c, p].
 __global__ void __launch_bounds__(256)
 prologue_kernel(const float* __restrict__ x0, const float* __restrict__ eps, const long long* __restrict__ t,
                 const float* __restrict__ sqrt_acp, const float* __restrict__ sqrt_1m,
                 const float* __restrict__ inp_mask, const float* __restrict__ masked_lat, void* __restrict__ out,
-                int out_dt, int B, int C, int P, int T) {
+                int out_dt, float* __restrict__ velocity, int B, int C, int P, int T) {
   const long long i = blockIdx.x * 256ll + threadIdx.x;
   if (i >= static_cast<long long>(B) * P) return;
   const int b = static_cast<int>(i / P), px = static_cast<int>(i % P);
@@ -43,8 +46,11 @@ prologue_kernel(const float* __restrict__ x0, const float* __restrict__ eps, con
   const long long obase = i * c_out;
   for (int c = 0; c < C; ++c) {
     const long long src = (static_cast<long long>(b) * C + c) * P + px;
-    // two rounded products and one rounded sum, as torch evaluates add_noise (no FMA contraction)
-    st_any(out, obase + c, out_dt, __fadd_rn(__fmul_rn(a, x0[src]), __fmul_rn(s, eps[src])));
+    const float x = x0[src], e = eps[src];
+    // two rounded products and one rounded sum (difference), as torch evaluates add_noise and
+    // get_velocity (no FMA contraction): both equal torch's result bit for bit
+    st_any(out, obase + c, out_dt, __fadd_rn(__fmul_rn(a, x), __fmul_rn(s, e)));
+    if (velocity) velocity[src] = __fsub_rn(__fmul_rn(a, e), __fmul_rn(s, x));   // consecutive px: coalesced
   }
   if (inp_mask) {
     st_any(out, obase + C, out_dt, inp_mask[static_cast<long long>(b) * P + px]);
@@ -104,18 +110,35 @@ masked_mse_kernel(const void* __restrict__ pred, int pred_dt, long long sb, long
 
 using namespace lbglue;
 
-extern "C" int lb_step_prologue(const float* latents, const float* noise, const long long* timesteps,
-                                const float* sqrt_acp, const float* sqrt_one_minus_acp, int n_timesteps,
-                                const float* inpaint_mask, const float* masked_latents, void* out,
-                                int out_dtype, int B, int C, int H, int W, void* stream) {
+static int launch_prologue(const float* latents, const float* noise, const long long* timesteps,
+                           const float* sqrt_acp, const float* sqrt_one_minus_acp, int n_timesteps,
+                           const float* inpaint_mask, const float* masked_latents, void* out, int out_dtype,
+                           float* velocity, int B, int C, int H, int W, void* stream) {
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || n_timesteps <= 0) return LB_ERR_SHAPE;
   if (out_dtype != LB_BF16 && out_dtype != LB_F16 && out_dtype != LB_F32) return LB_ERR_DTYPE;
   if ((inpaint_mask == nullptr) != (masked_latents == nullptr)) return LB_ERR_SHAPE;
   const long long n = static_cast<long long>(B) * H * W;
   prologue_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      latents, noise, timesteps, sqrt_acp, sqrt_one_minus_acp, inpaint_mask, masked_latents, out, out_dtype, B,
-      C, H * W, n_timesteps);
+      latents, noise, timesteps, sqrt_acp, sqrt_one_minus_acp, inpaint_mask, masked_latents, out, out_dtype,
+      velocity, B, C, H * W, n_timesteps);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_step_prologue(const float* latents, const float* noise, const long long* timesteps,
+                                const float* sqrt_acp, const float* sqrt_one_minus_acp, int n_timesteps,
+                                const float* inpaint_mask, const float* masked_latents, void* out,
+                                int out_dtype, int B, int C, int H, int W, void* stream) {
+  return launch_prologue(latents, noise, timesteps, sqrt_acp, sqrt_one_minus_acp, n_timesteps, inpaint_mask,
+                         masked_latents, out, out_dtype, nullptr, B, C, H, W, stream);
+}
+
+extern "C" int lb_step_prologue_v(const float* latents, const float* noise, const long long* timesteps,
+                                  const float* sqrt_acp, const float* sqrt_one_minus_acp, int n_timesteps,
+                                  const float* inpaint_mask, const float* masked_latents, void* out,
+                                  int out_dtype, float* velocity, int B, int C, int H, int W, void* stream) {
+  if (velocity == nullptr) return LB_ERR_SHAPE;
+  return launch_prologue(latents, noise, timesteps, sqrt_acp, sqrt_one_minus_acp, n_timesteps, inpaint_mask,
+                         masked_latents, out, out_dtype, velocity, B, C, H, W, stream);
 }
 
 extern "C" int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long stride_b, long long stride_c,

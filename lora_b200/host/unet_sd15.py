@@ -1,4 +1,4 @@
-"""SD1.5-shaped UNet *host model* (plain PyTorch; stands in for diffusers' UNet2DConditionModel).
+"""SD1.5- and SD2.x-shaped UNet *host model* (plain PyTorch; stands in for diffusers' UNet2DConditionModel).
 
 diffusers is not installed in this image and no SD weights exist offline, so the caller side of
 the LoRA hot path is restated here: an architecture with the SD1.5 hyper-parameters
@@ -14,10 +14,18 @@ the one the reference relies on (lora_diffusion/lora.py:159-165, 208-212):
     site order of the reference's fixture files (example_loras/*.safetensors: 144 UNet sites,
     per-block channel sequence [320,320,640,640,1280,1280 | 1280x3,640x3,320x3 | 1280];
     checked in tests/test_site_census.py).
+
+SD 2.x (`UNetConfig.sd21()`, the topology of both stable-diffusion-2-1 768-v and 2-1-base) differs in
+three hyper-parameters only: per-block head counts (5, 10, 20, 20) -- head dim 64 everywhere --,
+cross-attention dim 1024 (OpenCLIP-H text encoder, host/clip.py) and `nn.Linear` proj_in / proj_out
+(`use_linear_projection`). proj_in / proj_out sit in Transformer2DModel, outside every target set, so
+the SD2 UNet has the same 144 default sites. diffusers' `upcast_attention` (softmax in fp32 for the
+768-v model) is not restated: F.scaled_dot_product_attention already keeps its softmax in fp32 under
+bf16 / fp16, and attention scores are not a LoRA site.
 """
 import math
 from dataclasses import dataclass, field
-from typing import Optional, Tuple
+from typing import Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
@@ -30,15 +38,35 @@ class UNetConfig:
     out_channels: int = 4
     block_out_channels: Tuple[int, ...] = (320, 640, 1280, 1280)
     layers_per_block: int = 2
-    attention_head_dim: int = 8          # SD1.5: this is the NUMBER of heads
+    # diffusers' meaning: the NUMBER of heads (dim_head = channels // heads); one int for every block
+    # (SD1.5: 8) or one per down block (SD2.x: (5, 10, 20, 20)) -- up blocks take the tuple reversed,
+    # the mid block its last entry
+    attention_head_dim: Union[int, Tuple[int, ...]] = 8
     cross_attention_dim: int = 768
     norm_num_groups: int = 32
     # which down blocks carry cross-attention (SD1.5: first three)
     down_has_attn: Tuple[bool, ...] = (True, True, True, False)
+    # Transformer2DModel proj_in / proj_out as nn.Linear on NHWC tokens (SD2.x) instead of 1x1 convs
+    use_linear_projection: bool = False
 
     @staticmethod
     def sd15() -> "UNetConfig":
         return UNetConfig()
+
+    @staticmethod
+    def sd21() -> "UNetConfig":
+        """stable-diffusion-2-1 (768-v, 96x96 latents) and 2-1-base (512, 64x64): same topology."""
+        return UNetConfig(attention_head_dim=(5, 10, 20, 20), cross_attention_dim=1024,
+                          use_linear_projection=True)
+
+    @staticmethod
+    def sd2_tiny() -> "UNetConfig":
+        """SD2 features at toy widths (CPU tests): per-block heads, linear projection, and a
+        cross-attention width (64, host/clip.py's tiny SD2 encoder) unlike the UNet's."""
+        return UNetConfig(block_out_channels=(32, 64, 64), attention_head_dim=(2, 4, 4),
+                          cross_attention_dim=64, norm_num_groups=8,
+                          down_has_attn=(True, True, False), layers_per_block=1,
+                          use_linear_projection=True)
 
     @staticmethod
     def tiny() -> "UNetConfig":
@@ -114,23 +142,33 @@ class BasicTransformerBlock(nn.Module):
 
 
 class Transformer2DModel(nn.Module):
-    def __init__(self, channels: int, heads: int, cross_attention_dim: int, groups: int):
+    def __init__(self, channels: int, heads: int, cross_attention_dim: int, groups: int, linear: bool = False):
         super().__init__()
+        self.linear = linear
+        proj = (lambda: nn.Linear(channels, channels)) if linear else (lambda: nn.Conv2d(channels, channels, 1))
         self.norm = nn.GroupNorm(groups, channels, eps=1e-6)
-        self.proj_in = nn.Conv2d(channels, channels, 1)
+        self.proj_in = proj()
         self.transformer_blocks = nn.ModuleList(
             [BasicTransformerBlock(channels, heads, channels // heads, cross_attention_dim)])
-        self.proj_out = nn.Conv2d(channels, channels, 1)
+        self.proj_out = proj()
 
     def forward(self, x, context):
         B, C, H, W = x.shape
         res = x
-        h = self.proj_in(self.norm(x))
+        h = self.norm(x)
+        if not self.linear:
+            h = self.proj_in(h)
         h = h.permute(0, 2, 3, 1).reshape(B, H * W, C)
+        if self.linear:                      # diffusers' order: reshape to tokens, then proj_in
+            h = self.proj_in(h)
         for blk in self.transformer_blocks:
             h = blk(h, context)
+        if self.linear:
+            h = self.proj_out(h)
         h = h.reshape(B, H, W, C).permute(0, 3, 1, 2)
-        return self.proj_out(h) + res
+        if not self.linear:
+            h = self.proj_out(h)
+        return h + res
 
 
 class ResnetBlock2D(nn.Module):
@@ -175,11 +213,11 @@ class Upsample2D(nn.Module):
 class DownBlock(nn.Module):
     """CrossAttnDownBlock2D / DownBlock2D."""
 
-    def __init__(self, cin, cout, temb, layers, has_attn, heads, ctx_dim, groups, add_down):
+    def __init__(self, cin, cout, temb, layers, has_attn, heads, ctx_dim, groups, add_down, linear=False):
         super().__init__()
         if has_attn:
             self.attentions = nn.ModuleList(
-                [Transformer2DModel(cout, heads, ctx_dim, groups) for _ in range(layers)])
+                [Transformer2DModel(cout, heads, ctx_dim, groups, linear) for _ in range(layers)])
         self.resnets = nn.ModuleList(
             [ResnetBlock2D(cin if i == 0 else cout, cout, temb, groups) for i in range(layers)])
         self.downsamplers = nn.ModuleList([Downsample2D(cout)]) if add_down else None
@@ -201,11 +239,11 @@ class DownBlock(nn.Module):
 class UpBlock(nn.Module):
     """CrossAttnUpBlock2D / UpBlock2D."""
 
-    def __init__(self, cin, cout, cprev, temb, layers, has_attn, heads, ctx_dim, groups, add_up):
+    def __init__(self, cin, cout, cprev, temb, layers, has_attn, heads, ctx_dim, groups, add_up, linear=False):
         super().__init__()
         if has_attn:
             self.attentions = nn.ModuleList(
-                [Transformer2DModel(cout, heads, ctx_dim, groups) for _ in range(layers)])
+                [Transformer2DModel(cout, heads, ctx_dim, groups, linear) for _ in range(layers)])
         resnets = []
         for i in range(layers):
             skip = cin if i == layers - 1 else cout
@@ -229,9 +267,9 @@ class UpBlock(nn.Module):
 class MidBlock(nn.Module):
     """UNetMidBlock2DCrossAttn: resnet, attention, resnet."""
 
-    def __init__(self, ch, temb, heads, ctx_dim, groups):
+    def __init__(self, ch, temb, heads, ctx_dim, groups, linear=False):
         super().__init__()
-        self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, ctx_dim, groups)])
+        self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, ctx_dim, groups, linear)])
         self.resnets = nn.ModuleList([ResnetBlock2D(ch, ch, temb, groups) for _ in range(2)])
 
     def forward(self, x, temb, context):
@@ -273,6 +311,11 @@ class UNet2DConditionModel(nn.Module):
         temb = ch[0] * 4
         g = cfg.norm_num_groups
         heads = cfg.attention_head_dim
+        if isinstance(heads, int):
+            heads = (heads,) * len(ch)
+        if len(heads) != len(ch):
+            raise ValueError(f"attention_head_dim {heads}: one head count per block {ch}")
+        lin = cfg.use_linear_projection
         self.conv_in = nn.Conv2d(cfg.in_channels, ch[0], 3, padding=1)
         self.time_embedding = TimestepEmbedding(ch[0], temb)
         self.down_blocks = nn.ModuleList()
@@ -283,19 +326,20 @@ class UNet2DConditionModel(nn.Module):
             cin, cout = cout, c
             last = i == len(ch) - 1
             self.down_blocks.append(DownBlock(cin, cout, temb, cfg.layers_per_block,
-                                              cfg.down_has_attn[i], heads, cfg.cross_attention_dim,
-                                              g, add_down=not last))
+                                              cfg.down_has_attn[i], heads[i], cfg.cross_attention_dim,
+                                              g, add_down=not last, linear=lin))
         rev = list(reversed(ch))
         rev_attn = list(reversed(cfg.down_has_attn))
+        rev_heads = list(reversed(heads))
         cout = rev[0]
         for i, c in enumerate(rev):
             cprev, cout = cout, c
             cin = rev[min(i + 1, len(ch) - 1)]
             last = i == len(ch) - 1
             self.up_blocks.append(UpBlock(cin, cout, cprev, temb, cfg.layers_per_block + 1,
-                                          rev_attn[i], heads, cfg.cross_attention_dim, g,
-                                          add_up=not last))
-        self.mid_block = MidBlock(ch[-1], temb, heads, cfg.cross_attention_dim, g)
+                                          rev_attn[i], rev_heads[i], cfg.cross_attention_dim, g,
+                                          add_up=not last, linear=lin))
+        self.mid_block = MidBlock(ch[-1], temb, heads[-1], cfg.cross_attention_dim, g, linear=lin)
         self.conv_norm_out = nn.GroupNorm(g, ch[0], eps=1e-5)
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
 

@@ -2,6 +2,7 @@
 
   step_prologue     scheduler.add_noise + cast to the model dtype + NCHW -> channels_last
                     (+ the 9-channel inpainting concat)   cli_lora_pti.py:295-313
+                    (+ the v-prediction target scheduler.get_velocity, cli_lora_pti.py:333-338)
   fused_masked_mse  (mask-weighted) MSE and its gradient w.r.t. the prediction in one pass
                     cli_lora_pti.py:340-370, train_lora_dreambooth.py:855-875
 
@@ -18,8 +19,10 @@ from ._C import check, dtype_code, ptr, stream_ptr
 
 def step_prologue(latents: torch.Tensor, noise: torch.Tensor, timesteps: torch.Tensor, noiser,
                   out_dtype: torch.dtype, inpaint_mask: Optional[torch.Tensor] = None,
-                  masked_latents: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """noisy (+ inpainting channels) as a channels_last [B, C', H, W] tensor of `out_dtype`."""
+                  masked_latents: Optional[torch.Tensor] = None, velocity: bool = False):
+    """noisy (+ inpainting channels) as a channels_last [B, C', H, W] tensor of `out_dtype`.
+    velocity=True: `(noisy, v)`, v = sqrt_acp[t] * noise - sqrt_one_minus_acp[t] * latents as an fp32
+    NCHW tensor (the v-prediction target), written by the same launch."""
     if not latents.is_cuda:
         raise _C.LoraB200Error("step_prologue needs CUDA tensors (no CPU path)")
     B, C, H, W = latents.shape
@@ -31,11 +34,15 @@ def step_prologue(latents: torch.Tensor, noise: torch.Tensor, timesteps: torch.T
                       memory_format=torch.channels_last)
     im = None if inpaint_mask is None else inpaint_mask.float().contiguous()
     ml = None if masked_latents is None else masked_latents.float().contiguous()
-    check(_C.lib.lb_step_prologue(ptr(lat), ptr(eps), ptr(t), ptr(noiser.sqrt_acp), ptr(noiser.sqrt_one_minus_acp),
-                                  int(noiser.num_train_timesteps), ptr(im), ptr(ml), ptr(out),
-                                  dtype_code(out_dtype), B, C, H, W, stream_ptr()), "lb_step_prologue")
+    args = (ptr(lat), ptr(eps), ptr(t), ptr(noiser.sqrt_acp), ptr(noiser.sqrt_one_minus_acp),
+            int(noiser.num_train_timesteps), ptr(im), ptr(ml), ptr(out), dtype_code(out_dtype))
+    if velocity:
+        v = torch.empty((B, C, H, W), device=latents.device, dtype=torch.float32)
+        check(_C.lib.lb_step_prologue_v(*args, ptr(v), B, C, H, W, stream_ptr()), "lb_step_prologue_v")
+    else:
+        check(_C.lib.lb_step_prologue(*args, B, C, H, W, stream_ptr()), "lb_step_prologue")
     ops._count()
-    return out
+    return (out, v) if velocity else out
 
 
 class _MaskedMSE(torch.autograd.Function):

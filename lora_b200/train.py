@@ -83,6 +83,19 @@ class StepConfig:
     # queue the dA / dB reductions of all linear sites (and the conv sites' dB) during backward and
     # run them in ceil(n/24) launches at its end (ops.wgrad_flush / lb_lora_wgrad_batch)
     defer_wgrad: bool = True
+    # the regression target, as the reference's trainers read it from scheduler.config.prediction_type
+    # (cli_lora_pti.py:333-338, train_lora_dreambooth.py:846-853): "epsilon" (SD 1.x, SD 2.x base)
+    # regresses the noise, "v_prediction" (SD 2.x 768-v) the velocity
+    # sqrt_acp[t] * noise - sqrt(1 - acp[t]) * latents
+    prediction_type: str = "epsilon"
+
+
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+
+
+def _check_prediction_type(cfg: StepConfig):
+    if cfg.prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"Unknown prediction type {cfg.prediction_type}")
 
 
 class LoraTrainStep:
@@ -95,6 +108,7 @@ class LoraTrainStep:
 
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, cfg: StepConfig,
                  latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
+        _check_prediction_type(cfg)
         self.cfg = cfg
         self.unet, self.text_encoder = unet, text_encoder
         self.device = torch.device(device or "cuda")
@@ -166,13 +180,19 @@ class LoraTrainStep:
             t_max = int(self.noiser.num_train_timesteps * cfg.t_multiplier)
             timesteps = torch.randint(0, t_max, (bsz,), device=lat.device).long()
         fused = cfg.fused_glue and lat.is_cuda
+        v_pred = cfg.prediction_type == "v_prediction"
+        target = noise
         if fused:
             from .step_ops import step_prologue
             noisy = step_prologue(lat, noise, timesteps, self.noiser, self.model_dtype,
                                   self.inpaint_mask if cfg.train_inpainting else None,
-                                  self.masked_latents if cfg.train_inpainting else None)
+                                  self.masked_latents if cfg.train_inpainting else None, velocity=v_pred)
+            if v_pred:
+                noisy, target = noisy
         else:
             noisy = self.noiser.add_noise(lat, noise, timesteps)
+            if v_pred:
+                target = self.noiser.get_velocity(lat, noise, timesteps)
             if cfg.train_inpainting:
                 noisy = torch.cat([noisy, self.inpaint_mask.to(noisy.dtype), self.masked_latents.to(noisy.dtype)], dim=1)
         ac = (torch.autocast("cuda", dtype=cfg.autocast_dtype) if cfg.autocast_dtype is not None
@@ -186,7 +206,6 @@ class LoraTrainStep:
             if not fused:
                 noisy = noisy.to(self.model_dtype).contiguous(memory_format=torch.channels_last)
             pred = self.unet(noisy, timesteps, ehs.to(self.model_dtype)).sample
-        target = noise
         m = None
         if cfg.use_mask:
             m = (self.mask.float() + 0.01).pow(cfg.mask_temperature)
@@ -391,6 +410,7 @@ class TextualInversionStep(LoraTrainStep):
                  lr: float = 5e-4, weight_decay: float = 0.0, clip_ti_decay: bool = True,
                  latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
         from .ti import TextualInversionRows
+        _check_prediction_type(cfg)
         self.cfg = cfg
         self.unet, self.text_encoder = unet, text_encoder
         self.device = torch.device(device or "cuda")

@@ -15,6 +15,7 @@ Outputs (all small, committed):
   golden/svd_distill.pt                 cli_svd.overwrite_base outputs on small matrices
   golden/adamw_clip.pt                  clip_grad_norm_ + torch.optim.AdamW trajectories
   golden/pti_loss_step.pt               cli_lora_pti.loss_step losses (plain / t_mult / masked / inpainting)
+  golden/pti_loss_step_v.pt             the same with prediction_type "v_prediction" (+ one SD2 tiny case)
   golden/ti_train_inversion.pt          cli_lora_pti.train_inversion: 3 real steps (grads, lr, rows after)
   golden/pti_perform_tuning.pt          cli_lora_pti.perform_tuning: 3 real steps (losses, lrs, all factors after)
   golden/pti_continue_inversion.pt      the same loop with continue_inversion: 3 real steps (losses, lrs,
@@ -322,6 +323,80 @@ def gen_loss_step(R):
     print({c["name"]: c["loss"] for c in cases})
 
 
+def gen_loss_step_v(R):
+    """`loss_step` (cli_lora_pti.py:260-370) with the scheduler's prediction_type = "v_prediction", so
+    that its :333-338 branch regresses `scheduler.get_velocity(latents, noise, timesteps)`: plain,
+    t_mutliplier 0.8, masked, inpainting on the tiny SD1.5 models, and plain on the tiny SD2 models
+    (UNetConfig.sd2_tiny + the tiny SD2 text encoder). CPU fp32, cached latents."""
+    from lora_b200.host.clip import build_text_encoder
+    from lora_b200.host.ddpm import DDPMNoiser
+    from lora_b200.host.unet_sd15 import UNet2DConditionModel, UNetConfig
+    P = load_ref_pti(R)
+    noiser = DDPMNoiser(device="cpu")
+
+    class Sched:                      # what loss_step reads from a diffusers DDPMScheduler
+        config = types.SimpleNamespace(num_train_timesteps=noiser.num_train_timesteps,
+                                       prediction_type="v_prediction")
+        add_noise = staticmethod(noiser.add_noise)
+        # a restatement of diffusers' DDPMScheduler.get_velocity (scaled_linear betas 0.00085 -> 0.012):
+        # sqrt(acp[t]) * noise - sqrt(1 - acp[t]) * sample, computed from alphas_cumprod like diffusers
+        alphas_cumprod = torch.cumprod(1.0 - torch.linspace(0.00085 ** 0.5, 0.012 ** 0.5, 1000,
+                                                            dtype=torch.float32) ** 2, dim=0)
+
+        @staticmethod
+        def get_velocity(sample, noise, timesteps):
+            acp = Sched.alphas_cumprod.to(device=sample.device, dtype=sample.dtype)
+            sqrt_alpha_prod = (acp[timesteps] ** 0.5).flatten()
+            while len(sqrt_alpha_prod.shape) < len(sample.shape):
+                sqrt_alpha_prod = sqrt_alpha_prod.unsqueeze(-1)
+            sqrt_one_minus_alpha_prod = ((1 - acp[timesteps]) ** 0.5).flatten()
+            while len(sqrt_one_minus_alpha_prod.shape) < len(sample.shape):
+                sqrt_one_minus_alpha_prod = sqrt_one_minus_alpha_prod.unsqueeze(-1)
+            return sqrt_alpha_prod * noise - sqrt_one_minus_alpha_prod * sample
+
+    g = torch.Generator().manual_seed(78)
+    lat = torch.randn(2, 4, 8, 8, generator=g) * 0.18215
+    ids = torch.randint(0, 1000, (2, 77), generator=g)
+    loss_mask = (torch.rand(2, 1, 64, 64, generator=g) > 0.4).float()
+    inp_mask = (torch.rand(2, 1, 8, 8, generator=g) > 0.5).float()
+    inp_lat = torch.randn(2, 4, 8, 8, generator=g) * 0.18215
+    cases = []
+    for name, model, in_ch, kw, with_mask in [
+            ("plain", "sd15_tiny", 4, dict(), False),
+            ("t_mult_0.8", "sd15_tiny", 4, dict(t_mutliplier=0.8), False),
+            ("masked_T1", "sd15_tiny", 4, dict(mask_temperature=1.0), True),
+            ("inpaint", "sd15_tiny", 9, dict(train_inpainting=True), False),
+            ("sd2_plain", "sd2_tiny", 4, dict(), False)]:
+        torch.manual_seed(0)
+        sd2 = model == "sd2_tiny"
+        cfg = UNetConfig.sd2_tiny() if sd2 else UNetConfig.tiny()
+        cfg.in_channels = in_ch
+        unet = UNet2DConditionModel(cfg)
+        text = build_text_encoder(tiny=True, sd2=sd2)
+        R.inject_trainable_lora(unet, r=4)
+        gg = torch.Generator().manual_seed(5)
+        for m in unet.modules():
+            if type(m).__name__ == "LoraInjectedLinear":
+                m.lora_down.weight.data.normal_(0, 0.25, generator=gg)
+                m.lora_up.weight.data.normal_(0, 0.05, generator=gg)
+                m.dropout.p = 0.0
+        batch = {"pixel_values": lat, "input_ids": ids}
+        if in_ch == 9:
+            batch.update(masked_image_latents=inp_lat, mask_values=inp_mask)
+        if with_mask:
+            batch["mask"] = loss_mask
+        text.train(False), unet.train(False)
+        torch.manual_seed(1235)
+        loss = P.loss_step(batch, unet, None, text, Sched, cached_latents=True, **kw)
+        cases.append(dict(name=name, model=model, in_channels=in_ch, kwargs=kw, with_mask=with_mask,
+                          loss=float(loss)))
+    torch.save(dict(latents=lat, input_ids=ids, loss_mask=loss_mask, inpaint_mask=inp_mask,
+                    masked_latents=inp_lat, model_seed=0, up_seed=5, step_seed=1235,
+                    prediction_type="v_prediction", cases=cases),
+               f"{OUT}/pti_loss_step_v.pt")
+    print({c["name"]: c["loss"] for c in cases})
+
+
 def gen_ti(R):
     """Textual-inversion phase: the reference's own `train_inversion` loop (cli_lora_pti.py:373-542)
     run for 3 steps on the tiny models, CPU fp32, with torch.optim.AdamW over the embedding table
@@ -556,7 +631,7 @@ def gen_continue_inversion(R):
 
 
 GENERATORS = {"ops": gen_ops, "ctor_rng": gen_ctor_rng, "inject": gen_inject, "manifest": gen_manifest,
-              "svd": gen_svd, "adamw": gen_adamw, "loss_step": gen_loss_step, "ti": gen_ti, "tuning": gen_tuning,
+              "svd": gen_svd, "adamw": gen_adamw, "loss_step": gen_loss_step, "loss_step_v": gen_loss_step_v, "ti": gen_ti, "tuning": gen_tuning,
               "continue_inversion": gen_continue_inversion}
 
 
