@@ -269,6 +269,28 @@ int lb_embed_rows_scatter(const long long* ids, const void* grad, int grad_dtype
                           int* slot_of, int* slot_tok, int capacity, int* state, const void* table,
                           int table_dtype, const double* decay, float* master, float* slot_grad, void* stream);
 
+/* lb_embed_rows_scatter for `world` data-parallel replicas (1 <= world <= 16, 0 <= rank < world), one
+ * launch. ids_by_rank: HOST array of `world` device pointers, rank r's ids int64 [n_per_rank]
+ * (world * n_per_rank <= 2048); grad [n_per_rank, D] holds this rank's positions only. Slots are
+ * claimed over the concatenation [ids of rank 0; ids of rank 1; ...] -- the order of one process
+ * running the concatenated batch -- so every rank claims the same slots for the same tokens, tokens
+ * seen only on other ranks included (master = table[tok] * decay, no local gradient); only this
+ * rank's positions add into slot_grad (the arena's all-reduce sums the ranks). Flag bits are raised
+ * identically on every rank (the union is what overflows the capacity).
+ * Handshake, for ids that peers write while this launch runs (the other ranks' entries of
+ * ids_by_rank are CUDA-IPC mappings): flags_by_rank, a HOST array of `world` device pointers to each
+ * rank's one-word uint32 flag (zeroed once; this rank's own entry included), and epoch_dev, two
+ * zero-initialised uint32 {epoch, ticket} of this rank. The launch publishes epoch + 1 in its own
+ * flag (system-scope release) and waits for every peer's flag to reach it before reading that peer's
+ * ids; every rank must launch it the same number of times. Waits are bounded (~20 s) and trap.
+ * flags_by_rank = epoch_dev = NULL: the ids are stable for the launch (e.g. all-gathered by NCCL
+ * into one buffer beforehand). world = 1 without flags is lb_embed_rows_scatter. */
+int lb_embed_rows_scatter_dp(const long long* const* ids_by_rank, int world, int rank, int n_per_rank,
+                             const void* grad, int grad_dtype, int D, int V, int* slot_of, int* slot_tok,
+                             int capacity, int* state, const void* table, int table_dtype, const double* decay,
+                             float* master, float* slot_grad, const unsigned int* const* flags_by_rank,
+                             unsigned int* epoch_dev, void* stream);
+
 /* After the optimizer launch, one launch: table[slot_tok[s]] = master[s] (cast to table_dtype) for the
  * first n_write claimed slots (n_write < 0: every claimed slot), state[0] = state[1], and, when decay
  * and lr_dev are given, decay *= (double) fl32(1 - lr_dev[lr_index] * weight_decay) -- the factor the

@@ -73,6 +73,8 @@ def _load():
                                         i32, i32, vp], i32),
         "lb_ti_embed_step": ([vp, vp, vp, vp, vp, vp, i32, i32, i32, vp, f32, f32, f32, f32, vp, i32, f32, vp], i32),
         "lb_embed_rows_scatter": ([vp, vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, vp, vp, vp, vp], i32),
+        "lb_embed_rows_scatter_dp": ([vp, i32, i32, i32, vp, i32, i32, i32, vp, vp, i32, vp, vp, i32, vp, vp, vp,
+                                      vp, vp, vp], i32),
         "lb_embed_rows_write_back": ([vp, vp, i32, vp, i32, vp, i32, i32, i32, vp, vp, i32, f32, vp], i32),
         "lb_embed_rows_flush": ([vp, i32, i32, i32, vp, vp, vp, vp], i32),
         "lb_lora_merge": ([vp, i32, vp, vp, f32, vp, i32, i32, i32, vp], i32),
@@ -132,7 +134,7 @@ EXPORTED = [n for n in ("lb_abi_version", "lb_lora_linear_fwd", "lb_lora_wgrad",
                         "lb_cast_conv_weight", "lb_lora_up_dropout", "lb_lora_dropout_dt",
                         "lb_lora_wgrad_masked", "lb_lora_wgrad_pair", "lb_svd_mul", "lb_svd_gram",
                         "lb_svd_chol_inv", "lb_svd_apply", "lb_svd_jacobi", "lb_svd_randn", "lb_split_bf16x3", "lb_lora_merge", "lb_ti_embed_step",
-                        "lb_embed_rows_scatter", "lb_embed_rows_write_back", "lb_embed_rows_flush", "lb_lora_linear_fwd_grouped", "lb_lora_wgrad_multi", "lb_lora_wgrad_conv",
+                        "lb_embed_rows_scatter", "lb_embed_rows_scatter_dp", "lb_embed_rows_write_back", "lb_embed_rows_flush", "lb_lora_linear_fwd_grouped", "lb_lora_wgrad_multi", "lb_lora_wgrad_conv",
                         "lb_lora_linear_fwd_dropout", "lb_lora_conv2d_fwd_dropout", "lb_debug_set_pdl", "lb_svd_workspace_bytes", "lb_svd_truncated_batched",
                         "lb_optim_step_fused", "lb_step_prologue", "lb_step_prologue_v", "lb_masked_mse_fwd_bwd",
                         "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight")]

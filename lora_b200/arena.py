@@ -27,6 +27,8 @@ from ._C import check, dtype_code, ptr, stream_ptr
 
 _ALIGN = 8  # elements; keeps every factor 32-byte aligned inside the arena
 _LORA_CLASS_NAMES = ("LoraInjectedLinear", "LoraInjectedConv2d")
+# peer memory blocks this process has opened over CUDA IPC: handle -> base address
+_IPC_OPENED: Dict[bytes, int] = {}
 
 
 def lora_sites(model: nn.Module) -> List[nn.Module]:
@@ -178,7 +180,21 @@ class LoraArena:
         self._dp_flags = torch.zeros(2 * world, device=dev, dtype=torch.int32)
         self._dp_epoch = torch.zeros(1, device=dev, dtype=torch.int32)
         self.gsum = torch.zeros_like(self.g)
-        torch.cuda.synchronize(dev)
+        g_ptrs, f_ptrs = self.map_peer_tensors([self.g, self._dp_flags])
+        VP = ctypes.c_void_p * world
+        self._dp = (VP(*g_ptrs), VP(*f_ptrs), world, rank)
+        return True
+
+    def map_peer_tensors(self, tensors: Sequence[torch.Tensor]) -> List[List[int]]:
+        """Collective over the process group (every rank passes its own tensors of the same list):
+        exports each device tensor over CUDA IPC, all-gathers the handles and opens the peers' ones.
+        Returns, per tensor, the `world` device addresses of every rank's copy in rank order (this
+        rank's own included), usable by kernels of this process. All ranks must be on one node; the
+        tensors must outlive every launch that reads them. Ends in a barrier: on return every rank
+        has mapped every tensor."""
+        import torch.distributed as dist
+        world, rank = dist.get_world_size(), dist.get_rank()
+        torch.cuda.synchronize(self.device)
 
         def export(t):
             h = ctypes.create_string_buffer(64)
@@ -186,28 +202,22 @@ class LoraArena:
             check(_C.lib.lb_ipc_export(ptr(t), h, ctypes.byref(off)), "lb_ipc_export")
             return bytes(h.raw), int(off.value)
 
-        mine = (export(self.g), export(self._dp_flags))
+        mine = [export(t) for t in tensors]
         everyone = [None] * world
         dist.all_gather_object(everyone, mine)
-        opened = {}
 
         def open_(handle, off):
-            if handle not in opened:
+            if handle not in _IPC_OPENED:     # a block is opened once per process
                 base = ctypes.c_void_p()
                 check(_C.lib.lb_ipc_open(ctypes.create_string_buffer(handle, 64), ctypes.byref(base)), "lb_ipc_open")
-                opened[handle] = int(base.value)
-            return opened[handle] + off
+                _IPC_OPENED[handle] = int(base.value)
+            return _IPC_OPENED[handle] + off
 
-        g_ptrs, f_ptrs = [], []
-        for r, ((hg, og), (hf, of)) in enumerate(everyone):
-            if r == rank:
-                g_ptrs.append(self.g.data_ptr()); f_ptrs.append(self._dp_flags.data_ptr())
-            else:
-                g_ptrs.append(open_(hg, og)); f_ptrs.append(open_(hf, of))
-        VP = ctypes.c_void_p * world
-        self._dp = (VP(*g_ptrs), VP(*f_ptrs), world, rank)
+        out = []
+        for i, t in enumerate(tensors):
+            out.append([t.data_ptr() if r == rank else open_(*everyone[r][i]) for r in range(world)])
         dist.barrier()            # every rank has mapped every buffer before anybody launches
-        return True
+        return out
 
     def sync_replicas(self, src: int = 0):
         """Broadcast rank `src`'s LoRA factors and optimizer state (p, m, v, Adam's t) to every

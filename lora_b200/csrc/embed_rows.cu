@@ -1,7 +1,10 @@
 // Sparse, exact AdamW over the token-embedding table: the gradient scatter that replaces the dense
 // embedding backward, the write-back of the trained rows, and the lazy weight decay of the rows no
 // gradient has touched yet. The AdamW update itself is the arena's optimizer launch: the claimed
-// rows are one more param-group of the LoRA arena (see lora_b200/embed_rows.py).
+// rows are one more param-group of the LoRA arena (see lora_b200/embed_rows.py). Under data
+// parallelism the scatter claims slots over the union of every rank's ids (lb_embed_rows_scatter_dp),
+// so the ranks' rows groups hold the same tokens in the same slots and the arena's all-reduce can sum
+// them.
 //
 // Row state (all device memory, owned by the caller):
 //   slot_of  int32 [V]         token -> slot, -1 = unclaimed
@@ -17,11 +20,12 @@
 #include <stdint.h>
 
 #include "lora_b200.h"
+#include "ptx.cuh"
 
 namespace lb_embed {
 
 constexpr int THREADS = 256;
-constexpr int MAX_TOKENS = 2048;        // B * S per scatter launch (shared-memory bookkeeping)
+constexpr int MAX_TOKENS = 2048;        // world * B * S per scatter launch (shared-memory bookkeeping)
 constexpr int MAX_CTAS = 264;
 
 __device__ __forceinline__ float load_elem(const void* base, size_t i, int dtype) {
@@ -41,15 +45,42 @@ __device__ __forceinline__ void store_elem(void* base, size_t i, int dtype, floa
   }
 }
 
+constexpr int MAX_WORLD = 16;
+
+// Every rank's id buffer, in rank order (this rank's own one included), and for the peer handshake
+// every rank's one-word flag. Passed by value: the launch needs no device-side pointer table.
+struct RankIds {
+  const long long* ids[MAX_WORLD];
+  const unsigned int* flags[MAX_WORLD];
+};
+
 // Every CTA redoes the (cheap, shared-memory) bookkeeping of the whole batch, so that it knows
 // every distinct token's slot without a second launch; CTA b then owns the distinct tokens
 // b, b + grid, ... in first-occurrence order. A slot claimed by this launch has an index >= the
 // committed count state[0], which this launch never writes: whether another CTA has already
 // published a new token's slot or not, every CTA classifies that token as "new" and computes the
 // same slot for it.
+//
+// Data parallel (world > 1): the "whole batch" is the concatenation [ids of rank 0; ids of rank 1;
+// ...] of n_per_rank positions each, so every rank claims the same slots for the same tokens in the
+// same order as one process running the concatenated batch -- tokens that occur only on other ranks
+// included (master = stored row * decay, no local gradient). Only this rank's positions
+// [rank * n_per_rank, (rank + 1) * n_per_rank) add into slot_grad (grad holds just those rows); the
+// arena's all-reduce sums the ranks.
+//
+// Handshake (flags given): CTA 0 publishes this rank's epoch in its own flag with a system-scope
+// release (the ids were written before this launch, in stream order); every CTA then waits until
+// every peer's flag has reached the epoch before it reads that peer's ids. epoch_dev = {epoch of the
+// last scatter, CTA ticket}: every CTA reads the epoch before taking its ticket, the last CTA to
+// finish advances it, so the counter moves once per launch on every rank and is never restored.
+// Buffer lifetime: a peer's ids buffer is not rewritten while this rank may still read it. Rank r
+// writes its next step's ids only after its lb_optim_step_dp of this step has returned; that launch
+// waits for every rank's barrier-2 signal, and each rank signals barrier 2 from its own
+// lb_optim_step_dp, which its stream runs after its scatter has finished reading every rank's ids.
 __global__ void __launch_bounds__(THREADS)
-embed_rows_scatter_kernel(const long long* __restrict__ ids, const void* __restrict__ grad, int grad_dtype,
-                          int n_tok, int D, int V, int* __restrict__ slot_of, int* __restrict__ slot_tok,
+embed_rows_scatter_kernel(RankIds src, int world, int rank, int n_per_rank, unsigned int* __restrict__ my_flag,
+                          unsigned int* __restrict__ epoch_dev, const void* __restrict__ grad, int grad_dtype,
+                          int D, int V, int* __restrict__ slot_of, int* __restrict__ slot_tok,
                           int capacity, int* __restrict__ state, const void* __restrict__ table,
                           int table_dtype, const double* __restrict__ decay, float* __restrict__ master,
                           float* __restrict__ slot_grad) {
@@ -61,10 +92,26 @@ embed_rows_scatter_kernel(const long long* __restrict__ ids, const void* __restr
   __shared__ int s_scan[THREADS];
   const int tid = threadIdx.x;
   const int claimed0 = state[0];
+  const int n_tok = world * n_per_rank;
+  const int lo_local = rank * n_per_rank, hi_local = lo_local + n_per_rank;
+  unsigned int epoch = 0;
+  if (my_flag != nullptr) {
+    epoch = epoch_dev[0] + 1u;
+    if (blockIdx.x == 0 && tid == 0) {
+      __threadfence_system();
+      lb::st_release_sys(my_flag, epoch);
+    }
+    if (tid < world && tid != rank) lb::wait_flag_reached(src.flags[tid], epoch);
+    __syncthreads();
+  }
 
-  for (int i = tid; i < n_tok; i += THREADS) {
-    const long long t = ids[i];
-    s_id[i] = (t >= 0 && t < V) ? static_cast<int>(t) : -1;
+  for (int r = 0; r < world; ++r) {
+    // volatile: a peer's buffer may have been rewritten since an earlier launch, never cache it
+    const volatile long long* ids = src.ids[r];
+    for (int i = tid; i < n_per_rank; i += THREADS) {
+      const long long t = ids[i];
+      s_id[r * n_per_rank + i] = (t >= 0 && t < V) ? static_cast<int>(t) : -1;
+    }
   }
   __syncthreads();
   // first occurrence / next occurrence, per position (early exits keep repeated tokens cheap)
@@ -140,10 +187,25 @@ embed_rows_scatter_kernel(const long long* __restrict__ ids, const void* __restr
       for (int c = tid; c < D; c += THREADS)
         mrow[c] = static_cast<float>(static_cast<double>(load_elem(table, static_cast<size_t>(tok) * D + c, table_dtype)) * dk);
     }
+    // this rank's positions of the token: a contiguous run of its position chain (ranks in order)
+    int pl = p0;
+    while (pl >= 0 && pl < lo_local) pl = s_next[pl];
+    if (pl < 0 || pl >= hi_local) continue;  // the token occurs on other ranks only
     for (int c = tid; c < D; c += THREADS) {
       float acc = 0.f;
-      for (int p = p0; p >= 0; p = s_next[p]) acc += load_elem(grad, static_cast<size_t>(p) * D + c, grad_dtype);
+      for (int p = pl; p >= 0 && p < hi_local; p = s_next[p])
+        acc += load_elem(grad, static_cast<size_t>(p - lo_local) * D + c, grad_dtype);
       grow[c] += acc;
+    }
+  }
+  if (my_flag != nullptr) {
+    __syncthreads();
+    if (tid == 0) {
+      __threadfence();
+      if (atomicAdd(epoch_dev + 1, 1u) == gridDim.x - 1) {
+        epoch_dev[0] = epoch;                // every CTA has read the old epoch before taking its ticket
+        epoch_dev[1] = 0u;
+      }
     }
   }
 }
@@ -197,20 +259,46 @@ inline bool dtype_ok(int t) { return t == LB_F32 || t == LB_BF16 || t == LB_F16;
 
 using namespace lb_embed;
 
+extern "C" int lb_embed_rows_scatter_dp(const long long* const* ids_by_rank, int world, int rank, int n_per_rank,
+                                        const void* grad, int grad_dtype, int D, int V, int* slot_of, int* slot_tok,
+                                        int capacity, int* state, const void* table, int table_dtype,
+                                        const double* decay, float* master, float* slot_grad,
+                                        const unsigned int* const* flags_by_rank, unsigned int* epoch_dev,
+                                        void* stream) {
+  if (ids_by_rank == nullptr || grad == nullptr || slot_of == nullptr || slot_tok == nullptr ||
+      state == nullptr || table == nullptr || decay == nullptr || master == nullptr || slot_grad == nullptr)
+    return LB_ERR_SHAPE;
+  if (world < 1 || world > MAX_WORLD || rank < 0 || rank >= world) return LB_ERR_SHAPE;
+  if (n_per_rank <= 0 || n_per_rank > MAX_TOKENS / world || D <= 0 || V <= 0 || capacity <= 0)
+    return LB_ERR_SHAPE;
+  if ((flags_by_rank == nullptr) != (epoch_dev == nullptr)) return LB_ERR_SHAPE;
+  if (!dtype_ok(grad_dtype) || !dtype_ok(table_dtype)) return LB_ERR_DTYPE;
+  RankIds src = {};
+  for (int r = 0; r < world; ++r) {
+    if (ids_by_rank[r] == nullptr) return LB_ERR_SHAPE;
+    src.ids[r] = ids_by_rank[r];
+    if (flags_by_rank != nullptr) {
+      if (flags_by_rank[r] == nullptr) return LB_ERR_SHAPE;
+      src.flags[r] = flags_by_rank[r];
+    }
+  }
+  unsigned int* my_flag = flags_by_rank ? const_cast<unsigned int*>(flags_by_rank[rank]) : nullptr;
+  const int n_tok = world * n_per_rank;
+  const int grid = n_tok < MAX_CTAS ? n_tok : MAX_CTAS;
+  embed_rows_scatter_kernel<<<grid, THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      src, world, rank, n_per_rank, my_flag, epoch_dev, grad, grad_dtype, D, V, slot_of, slot_tok, capacity, state,
+      table, table_dtype, decay, master, slot_grad);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
 extern "C" int lb_embed_rows_scatter(const long long* ids, const void* grad, int grad_dtype, int n_tok, int D, int V,
                                      int* slot_of, int* slot_tok, int capacity, int* state, const void* table,
                                      int table_dtype, const double* decay, float* master, float* slot_grad,
                                      void* stream) {
-  if (ids == nullptr || grad == nullptr || slot_of == nullptr || slot_tok == nullptr || state == nullptr ||
-      table == nullptr || decay == nullptr || master == nullptr || slot_grad == nullptr)
-    return LB_ERR_SHAPE;
-  if (n_tok <= 0 || n_tok > MAX_TOKENS || D <= 0 || V <= 0 || capacity <= 0) return LB_ERR_SHAPE;
-  if (!dtype_ok(grad_dtype) || !dtype_ok(table_dtype)) return LB_ERR_DTYPE;
-  const int grid = n_tok < MAX_CTAS ? n_tok : MAX_CTAS;
-  embed_rows_scatter_kernel<<<grid, THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      ids, grad, grad_dtype, n_tok, D, V, slot_of, slot_tok, capacity, state, table, table_dtype, decay, master,
-      slot_grad);
-  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+  if (ids == nullptr) return LB_ERR_SHAPE;
+  const long long* one[1] = {ids};
+  return lb_embed_rows_scatter_dp(one, 1, 0, n_tok, grad, grad_dtype, D, V, slot_of, slot_tok, capacity, state, table,
+                                  table_dtype, decay, master, slot_grad, nullptr, nullptr, stream);
 }
 
 extern "C" int lb_embed_rows_write_back(const float* master, const int* slot_tok, int capacity, int* state,

@@ -11,6 +11,7 @@
 
 #include "dropmask.cuh"
 #include "lora_b200.h"
+#include "ptx.cuh"
 #include "tmap.h"
 
 namespace lb {
@@ -692,14 +693,6 @@ struct DpPeers {
   unsigned int* flags[DP_MAX_WORLD];  // flag arrays in rank order (own one included)
 };
 
-__device__ __forceinline__ void st_release_sys(unsigned int* p, unsigned int v) {
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned int ld_acquire_sys(const unsigned int* p) {
-  unsigned int v;
-  asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ float4 ld_peer16(const float* p) {
   float4 v;
   asm volatile("ld.volatile.global.v4.f32 {%0,%1,%2,%3}, [%4];"
@@ -708,13 +701,7 @@ __device__ __forceinline__ float4 ld_peer16(const float* p) {
 }
 // all ranks have written `epoch` into this rank's flags[b*world + r]
 __device__ __forceinline__ void dp_wait_all(const unsigned int* flags, int b, int world, unsigned int epoch) {
-  if (threadIdx.x < world) {
-    const unsigned int* f = flags + b * world + threadIdx.x;
-    const long long t0 = clock64();
-    while (static_cast<int>(ld_acquire_sys(f) - epoch) < 0) {
-      if (clock64() - t0 > 40000000000ll) __trap();
-    }
-  }
+  if (threadIdx.x < world) wait_flag_reached(flags + b * world + threadIdx.x, epoch);
   __syncthreads();
 }
 

@@ -1,5 +1,6 @@
 // Thin inline-PTX wrappers for the sm_90a features the LoRA kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (descriptors, fence / commit / wait), proxy fences.
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (descriptors, fence / commit / wait), proxy fences,
+// system-scope flags between the GPUs of a node.
 // Everything here is device-only and header-only.
 #pragma once
 #include <cuda.h>
@@ -132,6 +133,27 @@ __device__ __forceinline__ void reg_fence(float* r) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
+
+// ---------------------------------------------------------------- cross-GPU flags
+// System-scope release store / acquire load of a uint32 flag that another GPU of the node reads or
+// writes through a CUDA-IPC mapping: the writer's earlier global writes are visible to a reader
+// whose acquire load returns the stored value.
+__device__ __forceinline__ void st_release_sys(unsigned int* p, unsigned int v) {
+  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ unsigned int ld_acquire_sys(const unsigned int* p) {
+  unsigned int v;
+  asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+// Spin until *f has reached `epoch` (wrap-around safe). Bounded (~20 s): a peer that never arrives
+// traps (a CUDA error on the host) instead of hanging the device.
+__device__ __forceinline__ void wait_flag_reached(const unsigned int* f, unsigned int epoch) {
+  const long long t0 = clock64();
+  while (static_cast<int>(ld_acquire_sys(f) - epoch) < 0) {
+    if (clock64() - t0 > 40000000000ll) __trap();
+  }
 }
 
 // ---------------------------------------------------------------- small helpers

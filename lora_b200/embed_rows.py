@@ -14,6 +14,8 @@ gradient), so the arena's single optimizer launch clips and updates them with th
             itself keeps requires_grad=False
   backward  lb_embed_rows_scatter sums each distinct token's gradient rows into its slot and claims
             slots for tokens seen for the first time (master = stored row * pending decay)
+            (data parallel: lb_embed_rows_scatter_dp claims over the union of every rank's ids, in
+            rank order, so that every rank's slots hold the same tokens; see enable_data_parallel)
   update    the arena's optimizer launch (unchanged)
   after     lb_embed_rows_write_back copies the claimed masters (mode "placeholders": the
             placeholder slots only) into the table and advances the pending decay
@@ -26,6 +28,7 @@ step where a token is seen for the first time, the forward reads its stored row,
 the pending decay (a relative difference of 1 - decay, about steps * lr * wd); its master, and so
 every later step, starts from the decayed value.
 """
+import ctypes
 from typing import Sequence
 
 import torch
@@ -35,6 +38,8 @@ from . import _C, ops
 from ._C import check, dtype_code, ptr, stream_ptr
 
 MODES = ("table", "placeholders")
+# tokens one scatter launch can take: B * S, times the world size under data parallelism
+MAX_SCATTER_TOKENS = 2048
 
 
 class _Lookup(torch.autograd.Function):
@@ -100,7 +105,73 @@ class EmbeddingRows:
             return out
         return _Lookup.apply(self._anchor, out, inputs[0], self)
 
+    # ------------------------------------------------------------------ data parallel
+    def sync_replicas(self, src: int = 0):
+        """Broadcast rank `src`'s table and row state (slot map, slot list, counters, pending decay,
+        the rows' masters) to every rank: the common starting point DDP's parameter broadcast gives
+        the reference. A no-op outside torch.distributed."""
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+            return
+        a = self.arena
+        for buf in (self.emb[0].weight.data, self.slot_of, self.slot_tok, self.state, self.decay, a.rows_view(a.p)):
+            dist.broadcast(buf, src=src)
+
+    def enable_data_parallel(self, ids: torch.Tensor, peer: bool) -> bool:
+        """Collective: from now on the scatter claims slots over the union of every rank's `ids`
+        (the step's static [B, S] input buffer; the embedding must see exactly that buffer), in rank
+        order, so every rank's rows group holds the same tokens in the same slots.
+        peer=True: the peers' id buffers and a one-word flag per rank are mapped over CUDA IPC
+        (arena.map_peer_tensors) and read inside the scatter launch, after a flag handshake.
+        Otherwise, or when a mapping fails on any rank: `gather_ids()` (one NCCL all-gather into a
+        static [world * B, S] buffer) must run before each step's backward. Returns whether the peer
+        path is in use (the same on every rank)."""
+        import torch.distributed as dist
+        world, rank = dist.get_world_size(), dist.get_rank()
+        n = ids.numel()
+        if ids.dtype != torch.int64 or not ids.is_contiguous():
+            raise _C.LoraB200Error("EmbeddingRows.enable_data_parallel: ids must be a contiguous int64 buffer")
+        if world * n > MAX_SCATTER_TOKENS:
+            raise _C.LoraB200Error(f"EmbeddingRows: {world} ranks x {n} tokens exceed the scatter's limit of "
+                                   f"{MAX_SCATTER_TOKENS} tokens per step")
+        dev = ids.device
+        VP = ctypes.c_void_p * world
+        self._gathered = None
+        ok = False
+        if peer:
+            self._flag = torch.zeros(1, device=dev, dtype=torch.int32)
+            self._epoch = torch.zeros(2, device=dev, dtype=torch.int32)
+            try:
+                id_ptrs, flag_ptrs = self.arena.map_peer_tensors([ids, self._flag])
+                ok = True
+            except Exception as e:           # e.g. ranks on different nodes: all-gather the ids instead
+                self.peer_error = f"{type(e).__name__}: {e}"
+            agree = torch.tensor([1.0 if ok else 0.0], device=dev)
+            dist.all_reduce(agree, op=dist.ReduceOp.MIN)
+            ok = float(agree) == 1.0
+        if ok:
+            self._dp_ids, self._dp_flags = VP(*id_ptrs), VP(*flag_ptrs)
+        else:
+            self._flag = self._epoch = self._dp_flags = None
+            self._gathered = torch.zeros((world,) + tuple(ids.shape), device=dev, dtype=torch.int64)
+            base, nbytes = self._gathered.data_ptr(), n * self._gathered.element_size()
+            self._dp_ids = VP(*[base + r * nbytes for r in range(world)])
+        self._dp_local = ids
+        self._dp = (world, rank, n)
+        return ok
+
+    @property
+    def gathers_ids(self) -> bool:
+        """True on the NCCL path: gather_ids() must run before each backward."""
+        return getattr(self, "_gathered", None) is not None
+
+    def gather_ids(self):
+        import torch.distributed as dist
+        dist.all_gather_into_tensor(self._gathered, self._dp_local)
+
     def _scatter(self, ids: torch.Tensor, grad_out: torch.Tensor):
+        if getattr(self, "_dp", None) is not None:
+            return self._scatter_dp(ids, grad_out)
         a = self.arena
         ids = ids.reshape(-1)
         if ids.dtype != torch.int64:
@@ -112,6 +183,23 @@ class EmbeddingRows:
                                            ptr(self.state), ptr(table.data), dtype_code(table.dtype),
                                            ptr(self.decay), ptr(a.rows_view(a.p)), ptr(a.rows_view(a.g)),
                                            stream_ptr()), "lb_embed_rows_scatter")
+        ops._count(1)
+
+    def _scatter_dp(self, ids: torch.Tensor, grad_out: torch.Tensor):
+        a = self.arena
+        world, rank, n = self._dp
+        local = self._dp_local
+        if ids.data_ptr() != local.data_ptr() or ids.numel() != n:
+            raise _C.LoraB200Error("EmbeddingRows: under data parallelism the embedding must look up the step's "
+                                   "input_ids buffer (the peers read it)")
+        g = grad_out.reshape(-1, self.D).contiguous()
+        table = self.emb[0].weight
+        check(_C.lib.lb_embed_rows_scatter_dp(self._dp_ids, world, rank, n, ptr(g), dtype_code(g.dtype), self.D,
+                                              self.V, ptr(self.slot_of), ptr(self.slot_tok), self.capacity,
+                                              ptr(self.state), ptr(table.data), dtype_code(table.dtype),
+                                              ptr(self.decay), ptr(a.rows_view(a.p)), ptr(a.rows_view(a.g)),
+                                              self._dp_flags, ptr(self._epoch), stream_ptr()),
+              "lb_embed_rows_scatter_dp")
         ops._count(1)
 
     def write_back(self):

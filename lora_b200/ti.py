@@ -45,6 +45,19 @@ class TextualInversionRows(nn.Module):
             out = torch.where(hit, self.rows[j].to(out.dtype), out)
         return out
 
+    @torch.no_grad()
+    def sync_replicas(self, src: int = 0):
+        """Broadcast rank `src`'s trained rows, and the table rows they were taken from, to every
+        rank (DDP's parameter broadcast). A no-op outside torch.distributed."""
+        import torch.distributed as dist
+        if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+            return
+        table = self.emb[0].weight
+        src_rows = table.detach()[self.token_ids].contiguous()
+        dist.broadcast(src_rows, src=src)
+        table.data[self.token_ids] = src_rows
+        dist.broadcast(self.rows.data, src=src)
+
     def set_lr(self, lr: float):
         self.lr.fill_(float(lr))
 

@@ -98,6 +98,17 @@ def _check_prediction_type(cfg: StepConfig):
         raise ValueError(f"Unknown prediction type {cfg.prediction_type}")
 
 
+def _check_ranks_agree(what: str, **fields):
+    """Collective: raise ValueError on every rank unless every rank passed the same fields."""
+    import torch.distributed as dist
+    everyone = [None] * dist.get_world_size()
+    dist.all_gather_object(everyone, fields)
+    bad = sorted(k for k in fields if any(e[k] != everyone[0][k] for e in everyone))
+    if bad:
+        raise ValueError(f"{what}: the data-parallel ranks disagree on " +
+                         ", ".join(f"{k} ({[e[k] for e in everyone]})" for k in bad))
+
+
 class LoraTrainStep:
     """One data-parallel replica of the LoRA fine-tuning step (bs = latents.shape[0] per GPU)."""
 
@@ -426,13 +437,20 @@ class TextualInversionStep(LoraTrainStep):
         if cfg.train_inpainting:
             self.inpaint_mask = torch.zeros((latent_shape[0], 1, latent_shape[2], latent_shape[3]), device=self.device)
             self.masked_latents = torch.zeros(latent_shape, device=self.device, dtype=torch.float32)
-        self._world = 1
+        from .dist import world_info
+        _, self._world = world_info()
+        if self._world > 1:
+            _check_ranks_agree("TextualInversionStep", placeholder_token_ids=[int(t) for t in placeholder_token_ids],
+                               table=tuple(text_encoder.get_input_embeddings().weight.shape),
+                               latent_shape=tuple(int(s) for s in latent_shape), seq_len=int(seq_len))
         self.global_step = 0
         self.graph = self.graph_update = None
         self.graph_error = None
         self.base_lr = float(lr)
         self.ti = TextualInversionRows(text_encoder, placeholder_token_ids, lr=lr, weight_decay=weight_decay,
                                        clip_ti_decay=clip_ti_decay)
+        if self._world > 1:
+            self.ti.sync_replicas()        # rank 0's placeholder rows, in the rows and in the table
         self._frozen = []
         for m in list(unet.modules()) + list(text_encoder.modules()):
             if type(m).__name__ in ("LoraInjectedLinear", "LoraInjectedConv2d"):
@@ -454,6 +472,11 @@ class TextualInversionStep(LoraTrainStep):
         if not cfg.train_text_encoder:
             raise ValueError("TextualInversionStep needs StepConfig.train_text_encoder=True")
         self._fwd_bwd()                # rows.grad <- d loss / d placeholder rows
+        if self._world > 1:            # DDP's mean over the ranks: pre-divide, one all-reduce(sum)
+            import torch.distributed as dist
+            g = self.ti.rows.grad
+            g.mul_(1.0 / self._world)
+            dist.all_reduce(g, op=dist.ReduceOp.SUM)
         self.ti.step()                 # AdamW + norm decay + write-back + zero_grad, one kernel
         return self.loss
 
@@ -498,19 +521,24 @@ class LoraEmbeddingStep(LoraTrainStep):
     `row_capacity` slots of the arena (lora_b200/embed_rows.py). Per step this adds two launches
     to the plain step: the gradient scatter (in backward) and the write-back (after the optimizer).
     Mode "table" leaves the decay of unseen rows pending: call `flush()` before reading the table
-    outside the step (validation, saving a full text encoder); `release()` flushes too. Single
-    process only (each rank would claim its own slots)."""
+    outside the step (validation, saving a full text encoder); `release()` flushes too.
+
+    Data parallel (torch.distributed, one process per GPU of one node): the scatter claims slots over
+    the union of every rank's input_ids in rank order -- the slots one process would claim for the
+    concatenated batch -- so the rows group is summed, clipped and updated by the arena's all-reduce
+    and optimizer launch like the factors. The peers' ids are read inside the scatter launch over
+    CUDA IPC (peer_allreduce, the whole step stays one graph) or all-gathered by NCCL before the
+    backward. world * B * seq_len must not exceed 2048; ranks must agree on the placeholders,
+    row_capacity, mode and shapes (checked at construction); rank 0's table is broadcast."""
 
     _text_encoder_grad = True
 
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, placeholder_token_ids, cfg: StepConfig,
                  lr_embedding: float, mode: str = "table", unfreeze_lora_step: Optional[int] = None,
                  row_capacity: int = 1024, latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
-        from .embed_rows import MODES, EmbeddingRows
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            raise ValueError("LoraEmbeddingStep runs in one process: data-parallel ranks would claim "
-                             "different embedding rows")
+        from ._C import LoraB200Error
+        from .embed_rows import MAX_SCATTER_TOKENS, MODES, EmbeddingRows
+        from .dist import world_info
         if mode not in MODES:
             raise ValueError(f"mode {mode!r}: one of {MODES}")
         if mode == "placeholders" and not cfg.train_text_encoder:
@@ -521,11 +549,30 @@ class LoraEmbeddingStep(LoraTrainStep):
         self.mode = mode
         self.unfreeze_lora_step = (500 if unfreeze_lora_step is None else int(unfreeze_lora_step)) \
             if mode == "placeholders" else None        # train_lora_w_ti.py:570-574 default
-        D = text_encoder.get_input_embeddings().weight.shape[1]
+        table = text_encoder.get_input_embeddings().weight
+        D = table.shape[1]
+        _, world = world_info()
+        n_tok = world * int(latent_shape[0]) * int(seq_len)
+        if n_tok > MAX_SCATTER_TOKENS:
+            raise LoraB200Error(f"LoraEmbeddingStep: {world} rank(s) x batch {latent_shape[0]} x {seq_len} tokens = "
+                                f"{n_tok} exceed the gradient scatter's limit of {MAX_SCATTER_TOKENS} tokens per step")
+        if world > 1:
+            if cfg.capture_collective:
+                raise ValueError("LoraEmbeddingStep: capture_collective is not supported with data parallelism")
+            # ranks that disagree would enter incompatible graphs: refuse on every rank, before anything runs
+            _check_ranks_agree("LoraEmbeddingStep", placeholder_token_ids=[int(t) for t in placeholder_token_ids],
+                               row_capacity=int(row_capacity), D=int(D), vocab=int(table.shape[0]), mode=mode,
+                               latent_shape=tuple(int(s) for s in latent_shape), seq_len=int(seq_len))
         self._arena_rows = (int(row_capacity), int(D), float(lr_embedding))
         super().__init__(unet, text_encoder, cfg, latent_shape=latent_shape, seq_len=seq_len, device=device)
         self.rows = EmbeddingRows(text_encoder, self.arena, placeholder_token_ids, mode=mode,
                                   weight_decay=cfg.adam_weight_decay)
+        if self._world > 1:
+            self.rows.sync_replicas()            # rank 0's table and row state everywhere
+            if not self.rows.enable_data_parallel(self.input_ids, peer=self.peer_allreduce) and self.peer_allreduce:
+                # a rank could not map the peers' ids: the whole step takes the NCCL path
+                self.peer_allreduce = False
+                self.arena._dp = None
         # overflow flag of the last two step_host calls (pinned, copied without a synchronise)
         self._h_flags = [torch.zeros(1, dtype=torch.int32).pin_memory() for _ in range(2)]
         self._flag_events = [None, None]
@@ -547,6 +594,16 @@ class LoraEmbeddingStep(LoraTrainStep):
             lrs = list(base)
             lrs[rg] = 0.0
         self.arena.set_lr(lrs)
+
+    def _body(self):
+        if self.rows.gathers_ids:                # NCCL path: every rank's ids before the backward
+            self.rows.gather_ids()
+        super()._body()
+
+    def step_device(self) -> torch.Tensor:
+        if self.graph is not None and self.graph_update is not None and self.rows.gathers_ids:
+            self.rows.gather_ids()               # outside graph 1, like the gradient all-reduce
+        return super().step_device()
 
     def _update(self):
         super()._update()
