@@ -332,21 +332,6 @@ int lb_tile_weight(const void* src, int src_dtype, long long src_rs, long long s
 int lb_cast_weight(const void* src, int src_dtype, void* dst16, void* dstT16, int R, int C,
                    int out_dtype, void* stream);
 
-/* Global-norm clip + AdamW over one flat fp32 arena, two launches, no host sync.
- *   total = inv_world * ||g||_2 ; coef = min(1, max_norm / (total + 1e-6))  (max_norm <= 0: no clip)
- *   g' = g * inv_world * coef ; decoupled weight decay ; Adam moments ; bias correction with
- *   t = ++(*step_dev) ; g is zeroed for the next step ; *gnorm_out = total.
- * Elements [group_off[i], group_off[i+1]) use lr_dev[i]; group_off is a HOST array of
- * n_groups+1 offsets (n_groups <= 8), lr_dev a DEVICE array (so a captured graph sees scheduler
- * updates), step_dev a DEVICE int. partials: device scratch of >= 1024 floats.
- * Replaces clip_grad_norm_ + torch.optim.AdamW.step + zero_grad,
- * training_scripts/train_lora_dreambooth.py:878-888 and lora_diffusion/cli_lora_pti.py:606-609.
- */
-int lb_adamw_clip_step(float* p, float* g, float* m, float* v, long long n,
-                       const long long* group_off, int n_groups, const float* lr_dev, float beta1,
-                       float beta2, float eps, float weight_decay, float max_norm, float inv_world,
-                       int* step_dev, float* partials, float* gnorm_out, void* stream);
-
 /* fp16 mixed precision: torch.amp.GradScaler's dynamic loss scaling and the LR schedule, run inside
  * the optimizer launch (accelerate's `--mixed_precision fp16`: scaled backward, unscale_ +
  * clip_grad_norm_, scaler.step / scaler.update, and a scheduler step only after an applied step).
@@ -390,11 +375,21 @@ typedef struct lb_grad_scaler {
   int* applied;               /* int32 [1] optimizer steps applied (the schedule's step count) */
 } lb_grad_scaler;
 
-/* The whole optimizer step in ONE cooperative launch: lb_adamw_clip_step's two passes plus
- * lb_refresh_shadows (the re-cast of every LoRA factor into the 16-bit [rows, C] operands of the
- * fused kernels; `table` = the rows lb_refresh_shadows walks, n_entries may be 0), separated by
- * grid barriers on `barrier2` (2 x uint32 of device memory, zero-initialised once by the caller).
- * train_lora_dreambooth.py:878-888 (clip_grad_norm_, optimizer.step, zero_grad).
+/* The whole optimizer step over one flat fp32 arena in ONE cooperative launch, no host sync:
+ * global-norm clip + AdamW + zero_grad, then the refresh of the 16-bit operand shadows.
+ *   total = inv_world * ||g||_2 ; coef = min(1, max_norm / (total + 1e-6))  (max_norm <= 0: no clip)
+ *   g' = g * inv_world * coef ; decoupled weight decay ; Adam moments ; bias correction with
+ *   t = ++(*step_dev) ; g is zeroed for the next step ; *gnorm_out = total (gnorm_out may be NULL).
+ * inv_world: 1 / the number of data-parallel replicas whose gradients `g` already sums (1.0 alone).
+ * Elements [group_off[i], group_off[i+1]) use lr_dev[i]; group_off is a HOST array of n_groups+1
+ * offsets (n_groups <= 8), lr_dev a DEVICE array (so a captured graph sees scheduler updates),
+ * step_dev a DEVICE int. partials: device scratch of >= 1024 floats. g must be 16-byte aligned.
+ * Then every LoRA factor is re-cast into the 16-bit [rows, C] operands of the fused kernels, as
+ * lb_refresh_shadows does (`table`, n_entries, max_C: its arguments, n_entries may be 0;
+ * shadow16 / shadow_dtype: its dst16_base / out_dtype). The phases are separated by grid barriers
+ * on `barrier2` (2 x uint32 of device memory, zero-initialised once by the caller).
+ * Replaces clip_grad_norm_ + torch.optim.AdamW.step + zero_grad,
+ * training_scripts/train_lora_dreambooth.py:878-888 and lora_diffusion/cli_lora_pti.py:606-609.
  * scaler: NULL, or the fp16 loss-scaling mode above (HOST pointer to the struct). */
 int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
                         const long long* group_off, int n_groups, const float* lr_dev, float beta1,

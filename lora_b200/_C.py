@@ -66,8 +66,6 @@ def _load():
         "lb_lora_wgrad": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, i32, vp], i32),
         "lb_cast_rows_pad": ([vp, ll, ll, vp, i32, i32, i32, i32, vp], i32),
         "lb_cast_weight": ([vp, i32, vp, vp, i32, i32, i32, vp], i32),
-        "lb_adamw_clip_step": ([vp, vp, vp, vp, ll, ctypes.POINTER(ll), i32, vp, f32, f32, f32,
-                                f32, f32, f32, vp, vp, vp, vp], i32),
         "lb_optim_step_fused": ([vp, vp, vp, vp, ll, ctypes.POINTER(ll), i32, vp, f32, f32, f32,
                                  f32, f32, f32, vp, vp, vp, vp, i32, i32, vp, i32, vp, vp, vp], i32),
         "lb_step_prologue": ([vp, vp, vp, vp, vp, i32, vp, vp, vp, i32, i32, i32, i32, i32, vp], i32),
@@ -144,7 +142,7 @@ lib = _LazyLib()
 def is_loaded() -> bool:
     return _LazyLib._lib is not None
 EXPORTED = [n for n in ("lb_abi_version", "lb_lora_linear_fwd", "lb_lora_wgrad",
-                        "lb_cast_rows_pad", "lb_cast_weight", "lb_adamw_clip_step",
+                        "lb_cast_rows_pad", "lb_cast_weight",
                         "lb_refresh_shadows", "lb_lora_conv2d_fwd",
                         "lb_cast_conv_weight", "lb_lora_up_dropout", "lb_lora_dropout_dt",
                         "lb_lora_wgrad_masked", "lb_lora_wgrad_pair", "lb_svd_mul", "lb_svd_gram",

@@ -9,10 +9,12 @@ lora_diffusion/cli_lora_pti.py:997, 606-609):
     Parameters become views; Parameter object identity is preserved so the generators returned
     by inject_trainable_lora stay valid) with sibling buffers g, m, v;
   * backward kernels accumulate dA/dB straight into `g` (no autograd accumulation kernels);
-  * data parallel: ONE NCCL all-reduce(sum) over `g` per step; the 1/world average, the
-    global-norm clip coefficient, AdamW, gradient zeroing are one fused pass
-    (lb_adamw_clip_step), followed by one batched refresh of the 16-bit operand copies the
-    wgmma kernels read (lb_refresh_shadows);
+  * one cooperative launch per step (lb_optim_step_fused) computes the global-norm clip
+    coefficient, runs AdamW, zeroes the gradients and refreshes the 16-bit operand copies the
+    wgmma kernels read (with fp16 loss scaling: also unscale, skip and the scale update);
+  * data parallel: with enable_peer_allreduce() the gradient sum over the ranks happens inside
+    that launch by peer reads over NVLink (lb_optim_step_dp, no NCCL call); otherwise ONE NCCL
+    all-reduce(sum) over `g` precedes it and the launch folds in the 1/world average;
   * nothing here synchronises the host, so a whole training step can be captured in a CUDA graph
     (learning rates and the step counter live in device memory).
 """
@@ -107,11 +109,7 @@ class LoraArena:
         self.step_dev = torch.zeros(1, device=dev, dtype=torch.int32)
         self.partials = torch.zeros(1024, device=dev, dtype=torch.float32)
         self.gnorm = torch.zeros(1, device=dev, dtype=torch.float32)
-        self._grid_bar = torch.zeros(2, device=dev, dtype=torch.int32)   # lb_optim_step_fused's grid barrier
-        # one cooperative launch for clip + AdamW + zero_grad + shadow refresh; LB_OPT_SPLIT=1 keeps
-        # the three separate launches (lb_adamw_clip_step x2 kernels + lb_refresh_shadows)
-        import os as _os
-        self.fused_step = _os.environ.get("LB_OPT_SPLIT", "0") != "1"
+        self._grid_bar = torch.zeros(2, device=dev, dtype=torch.int32)   # the optimizer launch's grid barrier
         self._group_off_c = (ctypes.c_longlong * len(self.group_off))(*self.group_off)
 
         # ---- adopt: Parameters become views of p; .grad views of g
@@ -309,8 +307,6 @@ class LoraArena:
         a host round trip. The caller's backward must be seeded with `loss_scale` (the device
         tensor below) times the loss gradient, e.g. `(loss * arena.loss_scale).backward()` or
         step_ops.fused_masked_mse(..., grad_scale=arena.loss_scale)."""
-        if not self.fused_step:
-            raise _C.LoraB200Error("loss scaling runs in the one-launch optimizer step only (unset LB_OPT_SPLIT)")
         if not init_scale > 0.0:
             raise ValueError("enable_loss_scaling: need init_scale > 0")
         self._set_scaler_consts(growth_factor, backoff_factor, growth_interval)
@@ -394,13 +390,11 @@ class LoraArena:
     def step(self, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=1e-2, max_norm=1.0,
              world_size: int = 1, schedule: Optional[LrSchedule] = None):
         """clip_grad_norm_(max_norm) + AdamW + zero_grad on the (already summed) gradients, then the
-        16-bit operand shadows -- one cooperative launch (lb_optim_step_fused). After
-        enable_loss_scaling(): unscale, skip on inf / NaN, scale update and `schedule` in the same
-        launch."""
+        16-bit operand shadows -- one cooperative launch (lb_optim_step_fused; lb_optim_step_dp, which
+        also sums the ranks' gradients, after enable_peer_allreduce()). After enable_loss_scaling():
+        unscale, skip on inf / NaN, scale update and `schedule` in the same launch."""
         scaler = None
         if self.loss_scaling:
-            if not self.fused_step:
-                raise _C.LoraB200Error("loss scaling runs in the one-launch optimizer step only (unset LB_OPT_SPLIT)")
             scaler = self._scaler(schedule)
         elif schedule is not None:
             raise _C.LoraB200Error("step(schedule=...) needs enable_loss_scaling(); otherwise use set_lr")
@@ -415,10 +409,7 @@ class LoraArena:
                                           ptr(self.shadow), dtype_code(self.compute_dtype), ptr(self._grid_bar),
                                           dp[0], dp[1], dp[2], dp[3], ptr(self._dp_epoch), scaler, stream_ptr()),
                   "lb_optim_step_dp")
-            ops._count(1)
-            self._publish_shadows()
-            return
-        if self.fused_step:
+        else:
             check(_C.lib.lb_optim_step_fused(ptr(self.p), ptr(self.g), ptr(self.m), ptr(self.v), self.n,
                                              self._group_off_c, len(self.group_off) - 1, ptr(self.lr),
                                              beta1, beta2, eps, weight_decay,
@@ -427,17 +418,7 @@ class LoraArena:
                                              ptr(self.table), self.table.shape[0], self.table_max_c,
                                              ptr(self.shadow), dtype_code(self.compute_dtype),
                                              ptr(self._grid_bar), scaler, stream_ptr()), "lb_optim_step_fused")
-            ops._count(1)
-            self._publish_shadows()
-            return
-        check(_C.lib.lb_adamw_clip_step(ptr(self.p), ptr(self.g), ptr(self.m), ptr(self.v),
-                                        self.n, self._group_off_c, len(self.group_off) - 1,
-                                        ptr(self.lr), beta1, beta2, eps, weight_decay,
-                                        float(max_norm if max_norm else 0.0), 1.0 / world_size,
-                                        ptr(self.step_dev), ptr(self.partials), ptr(self.gnorm),
-                                        stream_ptr()), "lb_adamw_clip_step")
-        ops._count(2)
-        self.refresh_shadows()
+        ops._count(1)
         # re-validate the per-site operand caches: if torch-side code edited a factor in place since
         # the last step (version bump -> the site fell back to a private re-cast), point it back at
         # the arena's shadow buffer, which the launch above has just refreshed

@@ -506,72 +506,6 @@ __device__ __forceinline__ float block_sum(float x, float* sh) {
   return rsum;
 }
 
-// pass 1: per-block partial sums of g^2 (fixed summation order => run-to-run deterministic)
-__global__ void __launch_bounds__(OPT_THREADS)
-sqnorm_partial_kernel(const float* __restrict__ g, long long n, float* __restrict__ partials,
-                      int* __restrict__ step_dev) {
-  __shared__ float sh[OPT_THREADS / 32];
-  float s = 0.f;
-  const long long n4 = n >> 2;
-  const float4* g4 = reinterpret_cast<const float4*>(g);
-  for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n4;
-       i += static_cast<long long>(gridDim.x) * OPT_THREADS) {
-    const float4 x = g4[i];
-    s += x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w;
-  }
-  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
-    const float x = g[(n4 << 2) + threadIdx.x];
-    s += x * x;
-  }
-  const float tot = block_sum(s, sh);
-  if (threadIdx.x == 0) {
-    partials[blockIdx.x] = tot;
-    if (blockIdx.x == 0) step_dev[0] += 1;  // t for the update pass that follows on the stream
-  }
-}
-
-// pass 2: every block re-reduces the partials (same order everywhere), then updates its slice
-__global__ void __launch_bounds__(OPT_THREADS)
-adamw_update_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
-                    float* __restrict__ v, long long n, OptGroups groups,
-                    const float* __restrict__ lr_dev, float beta1, float beta2, float eps,
-                    float wd, float max_norm, float inv_world, const int* __restrict__ step_dev,
-                    const float* __restrict__ partials, int n_partials,
-                    float* __restrict__ gnorm_out) {
-  __shared__ float sh[OPT_THREADS / 32];
-  float s = 0.f;
-  for (int i = threadIdx.x; i < n_partials; i += OPT_THREADS) s += partials[i];
-  const float sq = block_sum(s, sh);
-  const float total = sqrtf(sq) * inv_world;
-  float coef = inv_world;
-  if (max_norm > 0.f) coef *= fminf(1.f, max_norm / (total + 1e-6f));
-  if (blockIdx.x == 0 && threadIdx.x == 0 && gnorm_out) gnorm_out[0] = total;
-
-  const int t = step_dev[0];
-  const float bc1 = static_cast<float>(1.0 - pow(static_cast<double>(beta1), static_cast<double>(t)));
-  const float bc2_sqrt = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(beta2), static_cast<double>(t))));
-
-  for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n;
-       i += static_cast<long long>(gridDim.x) * OPT_THREADS) {
-    int gi = 0;
-#pragma unroll
-    for (int k = 1; k < OPT_MAX_GROUPS; ++k)
-      if (k < groups.n && i >= groups.off[k]) gi = k;
-    const float lr = lr_dev[gi];
-    const float gg = g[i] * coef;
-    float pp = p[i];
-    pp *= (1.f - lr * wd);
-    const float mm = beta1 * m[i] + (1.f - beta1) * gg;
-    const float vv = beta2 * v[i] + (1.f - beta2) * gg * gg;
-    const float denom = sqrtf(vv) / bc2_sqrt + eps;
-    pp -= (lr / bc1) * (mm / denom);
-    p[i] = pp;
-    m[i] = mm;
-    v[i] = vv;
-    g[i] = 0.f;
-  }
-}
-
 // ------------------------------------------------------------------------------- one-launch optimizer step
 // clip_grad_norm_ + AdamW + zero_grad + refresh of the 16-bit operand shadows in ONE cooperative
 // launch (train_lora_dreambooth.py:878-888 is ~10 foreach launches over hundreds of tiny tensors):
@@ -629,12 +563,14 @@ __device__ __forceinline__ int scaler_found_inf(const float* partials, unsigned 
   return __syncthreads_or(f);
 }
 
-// this step's per-group lrs into shared memory (lr_dev, or fl32(base_lr * lambda(applied)))
-__device__ __forceinline__ void scaler_group_lrs(const lb_grad_scaler& sc, const OptGroups& groups,
-                                                 const float* lr_dev, int applied, float* sh_lr) {
+// this step's per-group lrs into shared memory: lr_dev, or in scaled mode for the scheduled groups
+// fl32(base_lr * lambda(applied))
+template <bool SCALED>
+__device__ __forceinline__ void stage_group_lrs(const lb_grad_scaler& sc, const OptGroups& groups,
+                                                const float* lr_dev, int applied, float* sh_lr) {
   if (threadIdx.x < groups.n) {
     float lr = lr_dev[threadIdx.x];
-    if ((sc.scheduled_groups >> threadIdx.x) & 1u)
+    if (SCALED && ((sc.scheduled_groups >> threadIdx.x) & 1u))
       lr = __double2float_rn(sc.base_lr[threadIdx.x] * sched_lambda(sc, applied));
     sh_lr[threadIdx.x] = lr;
   }
@@ -663,7 +599,7 @@ __device__ __forceinline__ void scaler_commit(const lb_grad_scaler& sc, int foun
   }
 }
 
-// One AdamW element update (the arithmetic of adamw_update_kernel, unchanged)
+// One AdamW element update
 __device__ __forceinline__ void adamw_elem(float* p, float* m, float* v, long long i, float gg, float lr,
                                            float beta1, float beta2, float eps, float wd, float bc1,
                                            float bc2_sqrt) {
@@ -678,122 +614,10 @@ __device__ __forceinline__ void adamw_elem(float* p, float* m, float* v, long lo
   v[i] = vv;
 }
 
-template <bool SCALED>
-__global__ void __launch_bounds__(OPT_THREADS)
-optim_step_fused_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
-                        float* __restrict__ v, long long n, OptGroups groups,
-                        const float* __restrict__ lr_dev, float beta1, float beta2, float eps, float wd,
-                        float max_norm, float inv_world, int* __restrict__ step_dev,
-                        float* __restrict__ partials, float* __restrict__ gnorm_out,
-                        const long long* __restrict__ table, int n_entries, int max_c,
-                        uint16_t* __restrict__ shadow, int fmt, unsigned int* __restrict__ bar,
-                        lb_grad_scaler sc) {
-  __shared__ float sh[OPT_THREADS / 32];
-  __shared__ float sh_lr[OPT_MAX_GROUPS];
-  const unsigned int nb = gridDim.x;
-  // scaled mode: the state every block needs, read before block 0 rewrites it (after the barrier)
-  float scale = 1.f, inv_scale = 1.f;
-  int t0 = 0, applied = 0;
-  if constexpr (SCALED) {
-    scale = sc.scale[0];
-    inv_scale = __double2float_rn(1.0 / static_cast<double>(scale));
-    t0 = step_dev[0];
-    applied = sc.applied[0];
-  }
-  // ---- phase 1
-  {
-    float s = 0.f;
-    int bad = 0;
-    const long long n4 = n >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(g);
-    for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n4;
-         i += static_cast<long long>(nb) * OPT_THREADS) {
-      float4 x = g4[i];
-      if constexpr (SCALED) {
-        x.x *= inv_scale; x.y *= inv_scale; x.z *= inv_scale; x.w *= inv_scale;
-        bad |= !all_finite4(x);
-      }
-      s += x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w;
-    }
-    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
-      float x = g[(n4 << 2) + threadIdx.x];
-      if constexpr (SCALED) {
-        x *= inv_scale;
-        bad |= !isfinite(x);
-      }
-      s += x * x;
-    }
-    if constexpr (SCALED) bad = __syncthreads_or(bad);
-    const float tot = block_sum(s, sh);
-    if (threadIdx.x == 0) {
-      partials[blockIdx.x] = tot;
-      if constexpr (SCALED) partials[nb + blockIdx.x] = bad ? 1.f : 0.f;
-      else if (blockIdx.x == 0) step_dev[0] += 1;
-    }
-  }
-  grid_barrier(bar, nb);
-  // ---- phase 2
-  int skip = 0;
-  {
-    if constexpr (SCALED) {
-      skip = scaler_found_inf(partials, nb);
-      scaler_group_lrs(sc, groups, lr_dev, applied, sh_lr);
-      scaler_commit(sc, skip, scale, t0, applied, step_dev);
-    }
-    float s = 0.f;
-    for (unsigned int i = threadIdx.x; i < nb; i += OPT_THREADS) s += __ldcg(partials + i);
-    const float sq = block_sum(s, sh);
-    const float total = sqrtf(sq) * inv_world;
-    float coef = inv_world;
-    if (max_norm > 0.f) coef *= fminf(1.f, max_norm / (total + 1e-6f));
-    if (blockIdx.x == 0 && threadIdx.x == 0 && gnorm_out) gnorm_out[0] = total;
-    int t;
-    if constexpr (SCALED) t = t0 + 1;
-    else t = __ldcg(step_dev);
-    const float bc1 = static_cast<float>(1.0 - pow(static_cast<double>(beta1), static_cast<double>(t)));
-    const float bc2_sqrt = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(beta2), static_cast<double>(t))));
-    for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n;
-         i += static_cast<long long>(nb) * OPT_THREADS) {
-      if constexpr (SCALED) {
-        if (!skip) {
-          int gi = 0;
-#pragma unroll
-          for (int k = 1; k < OPT_MAX_GROUPS; ++k)
-            if (k < groups.n && i >= groups.off[k]) gi = k;
-          adamw_elem(p, m, v, i, (g[i] * inv_scale) * coef, sh_lr[gi], beta1, beta2, eps, wd, bc1, bc2_sqrt);
-        }
-        g[i] = 0.f;
-        continue;
-      }
-      int gi = 0;
-#pragma unroll
-      for (int k = 1; k < OPT_MAX_GROUPS; ++k)
-        if (k < groups.n && i >= groups.off[k]) gi = k;
-      const float lr = lr_dev[gi];
-      const float gg = g[i] * coef;
-      float pp = p[i];
-      pp *= (1.f - lr * wd);
-      const float mm = beta1 * m[i] + (1.f - beta1) * gg;
-      const float vv = beta2 * v[i] + (1.f - beta2) * gg * gg;
-      const float denom = sqrtf(vv) / bc2_sqrt + eps;
-      pp -= (lr / bc1) * (mm / denom);
-      p[i] = pp;
-      m[i] = mm;
-      v[i] = vv;
-      g[i] = 0.f;
-    }
-  }
-  if (n_entries <= 0 || skip) return;     // skip is block-uniform: p did not change, nor do the shadows
-  grid_barrier(bar, nb);
-  // ---- phase 3: one table entry per block iteration (entries have 64 ... 10240 columns: no empty work items)
-  for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb)
-    refresh_shadow_entry(p, table + static_cast<size_t>(e_i) * 8, shadow, fmt, threadIdx.x, OPT_THREADS);
-}
-
-// ------------------------------------------------------------------------------- data-parallel optimizer step
-// The gradient all-reduce FUSED into the optimizer step (train_lora_dreambooth.py:744-757,877-888:
-// DDP's bucketed all-reduce, then clip_grad_norm_ + AdamW + zero_grad): one cooperative launch per
-// rank, no NCCL call, so the whole training step is ONE CUDA graph at any world size.
+// ---- data parallel (PEERS): the gradient all-reduce FUSED into the optimizer step
+// (train_lora_dreambooth.py:744-757,877-888: DDP's bucketed all-reduce, then clip_grad_norm_ + AdamW
+// + zero_grad): one cooperative launch per rank, no NCCL call, so the whole training step is ONE
+// CUDA graph at any world size.
 //   barrier 1 (NVLink flags)  every rank's backward has finished: its flat gradient buffer is final
 //   phase 1   one-shot all-reduce by peer reads: gsum[i] = sum_r g_r[i], r = 0..world-1 in the SAME
 //             order on every rank (bitwise identical sums => replicas stay identical), 16-byte loads
@@ -822,23 +646,38 @@ __device__ __forceinline__ void dp_wait_all(const unsigned int* flags, int b, in
   if (threadIdx.x < world) wait_flag_reached(flags + b * world + threadIdx.x, epoch);
   __syncthreads();
 }
+// gsum's float4 i: the ranks' gradients summed in rank order
+__device__ __forceinline__ float4 peer_sum4(const DpPeers& peers, int world, long long i) {
+  float4 part[DP_MAX_WORLD];
+#pragma unroll
+  for (int r = 0; r < DP_MAX_WORLD; ++r)
+    if (r < world) part[r] = ld_peer16(peers.g[r] + 4 * i);
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int r = 0; r < DP_MAX_WORLD; ++r)
+    if (r < world) { a.x += part[r].x; a.y += part[r].y; a.z += part[r].z; a.w += part[r].w; }
+  return a;
+}
 
-template <bool SCALED>
+// SCALED: the lb_grad_scaler mode. PEERS: the gradient is the peer sum written to gsum, and g is
+// zeroed only after every rank has read it; otherwise the gradient is the local g, zeroed in phase 2.
+template <bool SCALED, bool PEERS>
 __global__ void __launch_bounds__(OPT_THREADS)
-optim_step_dp_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ gsum,
-                     float* __restrict__ m, float* __restrict__ v, long long n, OptGroups groups,
-                     const float* __restrict__ lr_dev, float beta1, float beta2, float eps, float wd,
-                     float max_norm, int* __restrict__ step_dev, float* __restrict__ partials,
-                     float* __restrict__ gnorm_out, const long long* __restrict__ table, int n_entries,
-                     int max_c, uint16_t* __restrict__ shadow, int fmt, unsigned int* __restrict__ bar,
-                     DpPeers peers, int world, int rank, unsigned int* __restrict__ epoch_dev,
-                     lb_grad_scaler sc) {
+optim_step_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ gsum,
+                  float* __restrict__ m, float* __restrict__ v, long long n, OptGroups groups,
+                  const float* __restrict__ lr_dev, float beta1, float beta2, float eps, float wd,
+                  float max_norm, float inv_world, int* __restrict__ step_dev, float* __restrict__ partials,
+                  float* __restrict__ gnorm_out, const long long* __restrict__ table, int n_entries,
+                  uint16_t* __restrict__ shadow, int fmt, unsigned int* __restrict__ bar, DpPeers peers,
+                  int world, int rank, unsigned int* __restrict__ epoch_dev, lb_grad_scaler sc) {
   __shared__ float sh[OPT_THREADS / 32];
   __shared__ float sh_lr[OPT_MAX_GROUPS];
   const unsigned int nb = gridDim.x;
-  const unsigned int epoch = epoch_dev[0] + 1u;          // bumped by block 0 at the very end
-  unsigned int* my_flags = peers.flags[rank];
-  const float inv_world = 1.f / static_cast<float>(world);
+  unsigned int epoch = 0u;
+  if constexpr (PEERS) {
+    epoch = epoch_dev[0] + 1u;                          // bumped by block 0 at the very end
+    inv_world = 1.f / static_cast<float>(world);        // the peer sum's average
+  }
   // scaled mode: the state every block needs, read before block 0 rewrites it (after the barrier)
   float scale = 1.f, inv_scale = 1.f;
   int t0 = 0, applied = 0;
@@ -849,43 +688,48 @@ optim_step_dp_kernel(float* __restrict__ p, float* __restrict__ g, float* __rest
     applied = sc.applied[0];
   }
   // ---- barrier 1: announce "my gradients are final" to every rank, wait for everybody's
-  if (blockIdx.x == 0 && threadIdx.x < world) {
-    __threadfence_system();
-    st_release_sys(peers.flags[threadIdx.x] + 0 * world + rank, epoch);
+  if constexpr (PEERS) {
+    if (blockIdx.x == 0 && threadIdx.x < world) {
+      __threadfence_system();
+      st_release_sys(peers.flags[threadIdx.x] + 0 * world + rank, epoch);
+    }
+    dp_wait_all(peers.flags[rank], 0, world, epoch);
   }
-  dp_wait_all(my_flags, 0, world, epoch);
-  // ---- phase 1: gsum = sum over ranks (fixed order), partial sum of squares
+  // ---- phase 1: partial sum of squares of the (unscaled) gradient; PEERS: gsum = sum over ranks
   {
     float s = 0.f;
     int bad = 0;
     const long long n4 = n >> 2;
     for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n4;
          i += static_cast<long long>(nb) * OPT_THREADS) {
-      float4 part[DP_MAX_WORLD];
-#pragma unroll
-      for (int r = 0; r < DP_MAX_WORLD; ++r)
-        if (r < world) part[r] = ld_peer16(peers.g[r] + 4 * i);
-      float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int r = 0; r < DP_MAX_WORLD; ++r)
-        if (r < world) { a.x += part[r].x; a.y += part[r].y; a.z += part[r].z; a.w += part[r].w; }
-      reinterpret_cast<float4*>(gsum)[i] = a;
-      if constexpr (SCALED) {
-        a.x *= inv_scale; a.y *= inv_scale; a.z *= inv_scale; a.w *= inv_scale;
-        bad |= !all_finite4(a);
+      float4 x;
+      if constexpr (PEERS) {
+        x = peer_sum4(peers, world, i);
+        reinterpret_cast<float4*>(gsum)[i] = x;
+      } else {
+        x = reinterpret_cast<const float4*>(g)[i];
       }
-      s += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
+      if constexpr (SCALED) {
+        x.x *= inv_scale; x.y *= inv_scale; x.z *= inv_scale; x.w *= inv_scale;
+        bad |= !all_finite4(x);
+      }
+      s += x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w;
     }
     if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
       const long long i = (n4 << 2) + threadIdx.x;
-      float a = 0.f;
-      for (int r = 0; r < world; ++r) a += *reinterpret_cast<const volatile float*>(peers.g[r] + i);
-      gsum[i] = a;
-      if constexpr (SCALED) {
-        a *= inv_scale;
-        bad |= !isfinite(a);
+      float x;
+      if constexpr (PEERS) {
+        x = 0.f;
+        for (int r = 0; r < world; ++r) x += *reinterpret_cast<const volatile float*>(peers.g[r] + i);
+        gsum[i] = x;
+      } else {
+        x = g[i];
       }
-      s += a * a;
+      if constexpr (SCALED) {
+        x *= inv_scale;
+        bad |= !isfinite(x);
+      }
+      s += x * x;
     }
     if constexpr (SCALED) bad = __syncthreads_or(bad);
     const float tot = block_sum(s, sh);
@@ -897,19 +741,19 @@ optim_step_dp_kernel(float* __restrict__ p, float* __restrict__ g, float* __rest
   }
   grid_barrier(bar, nb);
   // ---- barrier 2 (signal only): every block of this rank has finished reading the peers
-  if (blockIdx.x == 0 && threadIdx.x < world) {
-    __threadfence_system();
-    st_release_sys(peers.flags[threadIdx.x] + 1 * world + rank, epoch);
+  if constexpr (PEERS) {
+    if (blockIdx.x == 0 && threadIdx.x < world) {
+      __threadfence_system();
+      st_release_sys(peers.flags[threadIdx.x] + 1 * world + rank, epoch);
+    }
   }
-  // ---- phase 2: clip + AdamW from gsum (scaled mode: skipped on every rank alike, gsum is the same
-  // bits everywhere)
+  // ---- phase 2: clip + AdamW (scaled mode: skipped by every block alike; PEERS: by every rank
+  // alike, gsum is the same bits everywhere)
   int skip = 0;
   {
-    if constexpr (SCALED) {
-      skip = scaler_found_inf(partials, nb);
-      scaler_group_lrs(sc, groups, lr_dev, applied, sh_lr);
-      scaler_commit(sc, skip, scale, t0, applied, step_dev);
-    }
+    if constexpr (SCALED) skip = scaler_found_inf(partials, nb);
+    stage_group_lrs<SCALED>(sc, groups, lr_dev, applied, sh_lr);
+    if constexpr (SCALED) scaler_commit(sc, skip, scale, t0, applied, step_dev);
     float s = 0.f;
     for (unsigned int i = threadIdx.x; i < nb; i += OPT_THREADS) s += __ldcg(partials + i);
     const float sq = block_sum(s, sh);
@@ -922,39 +766,34 @@ optim_step_dp_kernel(float* __restrict__ p, float* __restrict__ g, float* __rest
     else t = __ldcg(step_dev);
     const float bc1 = static_cast<float>(1.0 - pow(static_cast<double>(beta1), static_cast<double>(t)));
     const float bc2_sqrt = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(beta2), static_cast<double>(t))));
-    for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n && !skip;
+    for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n;
          i += static_cast<long long>(nb) * OPT_THREADS) {
-      int gi = 0;
+      if (!skip) {
+        int gi = 0;
 #pragma unroll
-      for (int k = 1; k < OPT_MAX_GROUPS; ++k)
-        if (k < groups.n && i >= groups.off[k]) gi = k;
-      if constexpr (SCALED) {
-        adamw_elem(p, m, v, i, (__ldcg(gsum + i) * inv_scale) * coef, sh_lr[gi], beta1, beta2, eps, wd, bc1,
-                   bc2_sqrt);
-        continue;
+        for (int k = 1; k < OPT_MAX_GROUPS; ++k)
+          if (k < groups.n && i >= groups.off[k]) gi = k;
+        float gg;
+        if constexpr (PEERS) gg = __ldcg(gsum + i);
+        else gg = g[i];
+        if constexpr (SCALED) gg *= inv_scale;
+        adamw_elem(p, m, v, i, gg * coef, sh_lr[gi], beta1, beta2, eps, wd, bc1, bc2_sqrt);
       }
-      const float lr = lr_dev[gi];
-      const float gg = __ldcg(gsum + i) * coef;
-      float pp = p[i];
-      pp *= (1.f - lr * wd);
-      const float mm = beta1 * m[i] + (1.f - beta1) * gg;
-      const float vv = beta2 * v[i] + (1.f - beta2) * gg * gg;
-      const float denom = sqrtf(vv) / bc2_sqrt + eps;
-      pp -= (lr / bc1) * (mm / denom);
-      p[i] = pp;
-      m[i] = mm;
-      v[i] = vv;
+      if constexpr (!PEERS) g[i] = 0.f;
     }
   }
-  // ---- peers are done with this rank's gradients: zero them for the next backward pass
-  dp_wait_all(my_flags, 1, world, epoch);
-  for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n;
-       i += static_cast<long long>(nb) * OPT_THREADS)
-    g[i] = 0.f;
-  grid_barrier(bar, nb);
-  if (blockIdx.x == 0 && threadIdx.x == 0) epoch_dev[0] = epoch;
-  if (skip) return;                       // block-uniform: p did not change, nor do the shadows
-  // ---- phase 3: operand shadows, one table entry per block iteration
+  if constexpr (PEERS) {
+    // ---- peers are done with this rank's gradients: zero them for the next backward pass
+    dp_wait_all(peers.flags[rank], 1, world, epoch);
+    for (long long i = blockIdx.x * static_cast<long long>(OPT_THREADS) + threadIdx.x; i < n;
+         i += static_cast<long long>(nb) * OPT_THREADS)
+      g[i] = 0.f;
+    grid_barrier(bar, nb);              // also the barrier between phases 2 and 3
+    if (blockIdx.x == 0 && threadIdx.x == 0) epoch_dev[0] = epoch;
+  }
+  if (n_entries <= 0 || skip) return;   // skip is block-uniform: p did not change, nor do the shadows
+  if constexpr (!PEERS) grid_barrier(bar, nb);
+  // ---- phase 3: one table entry per block iteration (entries have 64 ... 10240 columns: no empty work items)
   for (int e_i = blockIdx.x; e_i < n_entries; e_i += nb)
     refresh_shadow_entry(p, table + static_cast<size_t>(e_i) * 8, shadow, fmt, threadIdx.x, OPT_THREADS);
 }
@@ -1028,7 +867,7 @@ int launch_t_from16(const void* gY, int fmt, const void* down, int C, int M, int
 // =============================================================================== C ABI
 using namespace lb;
 
-extern "C" int lb_abi_version(void) { return 6; }
+extern "C" int lb_abi_version(void) { return 7; }
 
 static int wgrad_run(WgArgs& a, int in_dtype, void* stream) {
   if (a.M <= 0 || a.n_pr < 1 || a.n_pr > WG_MAXP) return LB_ERR_SHAPE;
@@ -1378,30 +1217,6 @@ extern "C" int lb_cast_conv_weight(const void* src, int src_dtype, void* dst16, 
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
-extern "C" int lb_adamw_clip_step(float* p, float* g, float* m, float* v, long long n,
-                                  const long long* group_off, int n_groups, const float* lr_dev,
-                                  float beta1, float beta2, float eps, float weight_decay,
-                                  float max_norm, float inv_world, int* step_dev, float* partials,
-                                  float* gnorm_out, void* stream) {
-  if (n <= 0 || n_groups < 1 || n_groups > OPT_MAX_GROUPS) return LB_ERR_SHAPE;
-  if (reinterpret_cast<uintptr_t>(g) & 15) return LB_ERR_ALIGN;
-  OptGroups groups;
-  groups.n = n_groups;
-  for (int i = 0; i <= n_groups; ++i) groups.off[i] = group_off[i];
-  for (int i = n_groups + 1; i <= OPT_MAX_GROUPS; ++i) groups.off[i] = n;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  long long want = (n / 4 + OPT_THREADS - 1) / OPT_THREADS;
-  int nblk = static_cast<int>(want < 1 ? 1 : (want > OPT_MAX_PARTIALS ? OPT_MAX_PARTIALS : want));
-  sqnorm_partial_kernel<<<nblk, OPT_THREADS, 0, st>>>(g, n, partials, step_dev);
-  long long want2 = (n + OPT_THREADS - 1) / OPT_THREADS;
-  const int cap2 = 8 * (sm_count() > 0 ? sm_count() : 132);
-  int nblk2 = static_cast<int>(want2 > cap2 ? cap2 : want2);
-  adamw_update_kernel<<<nblk2, OPT_THREADS, 0, st>>>(p, g, m, v, n, groups, lr_dev, beta1, beta2,
-                                                     eps, weight_decay, max_norm, inv_world,
-                                                     step_dev, partials, nblk, gnorm_out);
-  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
-}
-
 // lb_grad_scaler checks (host, before any CUDA call); the ranges torch.amp.GradScaler asserts
 static bool scaler_args_ok(const lb_grad_scaler& sc, int n_groups) {
   if (sc.scale == nullptr || sc.growth_tracker == nullptr || sc.found_inf == nullptr || sc.applied == nullptr)
@@ -1416,28 +1231,45 @@ static bool scaler_args_ok(const lb_grad_scaler& sc, int n_groups) {
   return true;
 }
 
-extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
-                                   const long long* group_off, int n_groups, const float* lr_dev,
-                                   float beta1, float beta2, float eps, float weight_decay,
-                                   float max_norm, float inv_world, int* step_dev, float* partials,
-                                   float* gnorm_out, const long long* table, int n_entries, int max_C,
-                                   void* shadow16, int shadow_dtype, unsigned int* barrier2,
-                                   const lb_grad_scaler* scaler, void* stream) {
+// lb_optim_step_fused (peered = false: gsum, the peer arrays and epoch_dev are unused) and
+// lb_optim_step_dp (peered = true: inv_world is unused, the kernel forms 1 / world): the argument
+// checks, the group table, the grid size and the cooperative launch.
+static int optim_step_launch(bool peered, float* p, float* g, float* gsum, float* m, float* v, long long n,
+                             const long long* group_off, int n_groups, const float* lr_dev, float beta1,
+                             float beta2, float eps, float weight_decay, float max_norm, float inv_world,
+                             int* step_dev, float* partials, float* gnorm_out, const long long* table,
+                             int n_entries, int max_C, void* shadow16, int shadow_dtype, unsigned int* barrier2,
+                             const void* const* peer_g, void* const* peer_flags, int world, int rank,
+                             unsigned int* epoch_dev, const lb_grad_scaler* scaler, void* stream) {
   if (n <= 0 || n_groups < 1 || n_groups > OPT_MAX_GROUPS) return LB_ERR_SHAPE;
-  if (reinterpret_cast<uintptr_t>(g) & 15) return LB_ERR_ALIGN;
+  if (scaler != nullptr && !scaler_args_ok(*scaler, n_groups)) return LB_ERR_SHAPE;
+  if (peered) {
+    if (world < 1 || world > DP_MAX_WORLD || rank < 0 || rank >= world) return LB_ERR_SHAPE;
+    if (peer_g == nullptr || peer_flags == nullptr || gsum == nullptr || epoch_dev == nullptr) return LB_ERR_SHAPE;
+  }
+  if ((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(gsum)) & 15) return LB_ERR_ALIGN;
   if (n_entries > 0 && (table == nullptr || shadow16 == nullptr || max_C <= 0)) return LB_ERR_SHAPE;
   if (n_entries > 0 && shadow_dtype != LB_BF16 && shadow_dtype != LB_F16) return LB_ERR_DTYPE;
   if (barrier2 == nullptr || partials == nullptr) return LB_ERR_SHAPE;
-  if (scaler != nullptr && !scaler_args_ok(*scaler, n_groups)) return LB_ERR_SHAPE;
   OptGroups groups;
   groups.n = n_groups;
   for (int i = 0; i <= n_groups; ++i) groups.off[i] = group_off[i];
   for (int i = n_groups + 1; i <= OPT_MAX_GROUPS; ++i) groups.off[i] = n;
+  DpPeers peers = {};
+  for (int r = 0; peered && r < world; ++r) {
+    if (peer_g[r] == nullptr || peer_flags[r] == nullptr || (reinterpret_cast<uintptr_t>(peer_g[r]) & 15))
+      return LB_ERR_ALIGN;
+    peers.g[r] = reinterpret_cast<const float*>(peer_g[r]);
+    peers.flags[r] = reinterpret_cast<unsigned int*>(peer_flags[r]);
+  }
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) != cudaSuccess ||
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
     return LB_ERR_CUDA;
-  long long want = (n + OPT_THREADS - 1) / OPT_THREADS;
+  // one block per 256 elements, or per 256 float4 peer loads: the block count fixes the summation order
+  // of the norm (and so its bits), so each launch keeps its own rule
+  const long long work = peered ? n / 4 : n;
+  long long want = (work + OPT_THREADS - 1) / OPT_THREADS;
   int nblk = static_cast<int>(want < 1 ? 1 : (want > sms ? sms : want));
   const int max_blocks = scaler ? OPT_MAX_PARTIALS / 2 : OPT_MAX_PARTIALS;   // scaled: nb partials + nb flags
   if (nblk > max_blocks) nblk = max_blocks;
@@ -1454,11 +1286,24 @@ extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long 
   const int fmt = shadow_dtype == LB_BF16;
   uint16_t* sh = reinterpret_cast<uint16_t*>(shadow16);
   const lb_grad_scaler sc = scaler ? *scaler : lb_grad_scaler{};
-  cudaError_t e = cudaLaunchKernelEx(&cfg, scaler ? optim_step_fused_kernel<true> : optim_step_fused_kernel<false>,
-                                     p, g, m, v, n, groups, lr_dev, beta1, beta2, eps, weight_decay, max_norm,
-                                     inv_world, step_dev, partials, gnorm_out, table, n_entries, max_C, sh, fmt,
-                                     barrier2, sc);
+  auto kernel = peered ? (scaler ? optim_step_kernel<true, true> : optim_step_kernel<false, true>)
+                       : (scaler ? optim_step_kernel<true, false> : optim_step_kernel<false, false>);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, p, g, gsum, m, v, n, groups, lr_dev, beta1, beta2, eps,
+                                     weight_decay, max_norm, inv_world, step_dev, partials, gnorm_out, table,
+                                     n_entries, sh, fmt, barrier2, peers, world, rank, epoch_dev, sc);
   return e == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_optim_step_fused(float* p, float* g, float* m, float* v, long long n,
+                                   const long long* group_off, int n_groups, const float* lr_dev,
+                                   float beta1, float beta2, float eps, float weight_decay,
+                                   float max_norm, float inv_world, int* step_dev, float* partials,
+                                   float* gnorm_out, const long long* table, int n_entries, int max_C,
+                                   void* shadow16, int shadow_dtype, unsigned int* barrier2,
+                                   const lb_grad_scaler* scaler, void* stream) {
+  return optim_step_launch(false, p, g, nullptr, m, v, n, group_off, n_groups, lr_dev, beta1, beta2, eps,
+                           weight_decay, max_norm, inv_world, step_dev, partials, gnorm_out, table, n_entries,
+                           max_C, shadow16, shadow_dtype, barrier2, nullptr, nullptr, 1, 0, nullptr, scaler, stream);
 }
 
 // ------------------------------------------------------------------------------- CUDA IPC helpers
@@ -1513,49 +1358,8 @@ extern "C" int lb_optim_step_dp(float* p, float* g, float* gsum, float* m, float
                                 unsigned int* barrier2, const void* const* peer_g,
                                 void* const* peer_flags, int world, int rank, unsigned int* epoch_dev,
                                 const lb_grad_scaler* scaler, void* stream) {
-  if (n <= 0 || n_groups < 1 || n_groups > OPT_MAX_GROUPS) return LB_ERR_SHAPE;
-  if (scaler != nullptr && !scaler_args_ok(*scaler, n_groups)) return LB_ERR_SHAPE;
-  if (world < 1 || world > DP_MAX_WORLD || rank < 0 || rank >= world) return LB_ERR_SHAPE;
-  if (peer_g == nullptr || peer_flags == nullptr || gsum == nullptr || epoch_dev == nullptr) return LB_ERR_SHAPE;
-  if ((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(gsum)) & 15) return LB_ERR_ALIGN;
-  if (n_entries > 0 && (table == nullptr || shadow16 == nullptr || max_C <= 0)) return LB_ERR_SHAPE;
-  if (n_entries > 0 && shadow_dtype != LB_BF16 && shadow_dtype != LB_F16) return LB_ERR_DTYPE;
-  if (barrier2 == nullptr || partials == nullptr) return LB_ERR_SHAPE;
-  OptGroups groups;
-  groups.n = n_groups;
-  for (int i = 0; i <= n_groups; ++i) groups.off[i] = group_off[i];
-  for (int i = n_groups + 1; i <= OPT_MAX_GROUPS; ++i) groups.off[i] = n;
-  DpPeers peers = {};
-  for (int r = 0; r < world; ++r) {
-    if (peer_g[r] == nullptr || peer_flags[r] == nullptr || (reinterpret_cast<uintptr_t>(peer_g[r]) & 15))
-      return LB_ERR_ALIGN;
-    peers.g[r] = reinterpret_cast<const float*>(peer_g[r]);
-    peers.flags[r] = reinterpret_cast<unsigned int*>(peer_flags[r]);
-  }
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess ||
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-    return LB_ERR_CUDA;
-  long long want = (n / 4 + OPT_THREADS - 1) / OPT_THREADS;
-  int nblk = static_cast<int>(want < 1 ? 1 : (want > sms ? sms : want));
-  const int max_blocks = scaler ? OPT_MAX_PARTIALS / 2 : OPT_MAX_PARTIALS;   // scaled: nb partials + nb flags
-  if (nblk > max_blocks) nblk = max_blocks;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(nblk);
-  cfg.blockDim = dim3(OPT_THREADS);
-  cfg.dynamicSmemBytes = 0;
-  cfg.stream = reinterpret_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  const int fmt = shadow_dtype == LB_BF16;
-  uint16_t* sh = reinterpret_cast<uint16_t*>(shadow16);
-  const lb_grad_scaler sc = scaler ? *scaler : lb_grad_scaler{};
-  cudaError_t e = cudaLaunchKernelEx(&cfg, scaler ? optim_step_dp_kernel<true> : optim_step_dp_kernel<false>,
-                                     p, g, gsum, m, v, n, groups, lr_dev, beta1, beta2, eps, weight_decay, max_norm,
-                                     step_dev, partials, gnorm_out, table, n_entries, max_C, sh, fmt, barrier2, peers,
-                                     world, rank, epoch_dev, sc);
-  return e == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+  return optim_step_launch(true, p, g, gsum, m, v, n, group_off, n_groups, lr_dev, beta1, beta2, eps,
+                           weight_decay, max_norm, 0.f, step_dev, partials, gnorm_out, table, n_entries,
+                           max_C, shadow16, shadow_dtype, barrier2, peer_g, peer_flags, world, rank, epoch_dev,
+                           scaler, stream);
 }

@@ -6,9 +6,10 @@ Restates (diffusers / accelerate are not installed, so the scripts themselves ca
       add_noise, text encoder, UNet, MSE, backward, clip_grad_norm_(1.0), AdamW, zero_grad)
   lora_diffusion/cli_lora_pti.py:260-370, 585-617     -- PTI LoRA-tuning phase (same step with
       t_mutliplier and mean([1,2,3]).mean() reduction)
-Differences by design: LoRA factors/grads/moments live in a LoraArena, the
-DDP all-reduce + clip + AdamW + zero_grad are one NCCL call and two kernels, and steady-state
-steps are CUDA-graph replays (no Python, no launch gaps, no host sync).
+Differences by design: LoRA factors/grads/moments live in a LoraArena, clip + AdamW + zero_grad
+are one cooperative launch that also takes in the DDP all-reduce (peer reads over NVLink; one
+NCCL call before it without peer access), and steady-state steps are CUDA-graph replays (no
+Python, no launch gaps, no host sync).
 """
 from dataclasses import dataclass
 from typing import Optional

@@ -26,7 +26,7 @@ def test_build_and_load():
 def test_every_declared_symbol_is_exported():
     from lora_b200 import _C
     names = _declared()
-    assert "lb_lora_linear_fwd" in names and "lb_adamw_clip_step" in names and len(names) >= 13
+    assert "lb_lora_linear_fwd" in names and "lb_optim_step_fused" in names and len(names) >= 13
     lib = ctypes.CDLL(_C.LIB_PATH)
     for n in names:
         assert hasattr(lib, n), f"{n} declared in include/lora_b200.h but not exported"

@@ -3,7 +3,9 @@
   * the scaled optimizer launch (lb_optim_step_fused, lb_optim_step_dp at world 1) against
     GradScaler("cuda") + clip_grad_norm_ + AdamW + LambdaLR, over clean, inf, NaN and growth steps;
     with no scaler, both launches bit-identical to the release before loss scaling
-    (tests/golden/optim_null_scaler.pt, recorded by scripts/make_golden_optim.py);
+    (tests/golden/optim_null_scaler.pt); with a scaler, and unscaled at world_size 2, bit-identical
+    to the release before the two launches shared one kernel (tests/golden/optim_paths.pt; both
+    recorded by scripts/make_golden_optim.py);
   * the loss epilogue's grad_scale;
   * whole fp16 steps (tiny SD1.5 models) and the train_lora_w_ti.py embedding step against the oracle
     (oracle/amp_ref.py), eager and graph-replayed, with skipped steps, growth and a warm-up schedule;
@@ -156,17 +158,74 @@ def test_scaled_fused_launch_matches_torch_grad_scaler_and_dp_at_world_one():
     assert float((sa - sb).abs().max()) <= 2.0 ** -7 * float(sb.abs().max())
 
 
-def test_split_optimizer_refuses_loss_scaling():
-    from lora_b200._C import LoraB200Error
+# the loss scale before each of the eight scaled steps of optim_paths.pt: growth after two clean
+# steps, backoff on INJECT's inf (step 2) and NaN (step 4)
+PATHS_SCALES = [2.0 ** e for e in (14, 14, 15, 14, 14, 13, 13, 14)]
+OPTIM_PATHS = ("fused_scaled", "dp_scaled", "fused_world2")
+
+
+def optim_paths_inputs(arena, gen):
+    """Host inputs of tests/golden/optim_paths.pt: the arena's start point, eight loss-scaled
+    gradients (3.0 * randn on odd steps, clipped; INJECT's inf and NaN in element 7 of the second
+    factor) and three unscaled ones for the world_size=2 run (the second one clipped)."""
+    bad = arena.entries[1][3] + 7
+    scaled = []
+    for k, s in enumerate(PATHS_SCALES):
+        g = torch.randn(arena.n, generator=gen) * (3.0 if k % 2 else 0.01) * s
+        if k in INJECT:
+            g[bad] = INJECT[k]
+        scaled.append(g)
+    return {"p0": arena.p.cpu().clone(), "scaled": scaled,
+            "unscaled": [torch.randn(arena.n, generator=gen) * s for s in (0.01, 2.0, 0.01)]}
+
+
+def optim_paths_run(run, inputs):
+    """One run of optim_paths.pt: the scaled launch of lb_optim_step_fused or lb_optim_step_dp (world 1)
+    with a linear warm-up schedule, or the unscaled lb_optim_step_fused at world_size 2 (inv_world
+    0.5, the NCCL data-parallel path). Per step the norm and the device state, then the final arena.
+    Uses only the arena API both releases share, so the same function recorded the golden."""
+    from lora_b200.arena import LrSchedule
     arena = _two_group_arena()
-    arena.enable_loss_scaling()
-    arena.fused_step = False
-    with pytest.raises(LoraB200Error):
-        arena.step()
-    arena2 = _two_group_arena()
-    arena2.fused_step = False
-    with pytest.raises(LoraB200Error):
-        arena2.enable_loss_scaling()
+    if run == "dp_scaled":
+        _as_world_one_dp(arena)
+    scaled = run != "fused_world2"
+    state = {"gnorm": lambda: arena.gnorm, "step": lambda: arena.step_dev}
+    if scaled:
+        arena.enable_loss_scaling(init_scale=2.0 ** 14, growth_interval=2)
+        state.update(loss_scale=lambda: arena.loss_scale, growth_tracker=lambda: arena._growth_tracker,
+                     found_inf=lambda: arena._found_inf, applied=lambda: arena.applied_steps)
+    arena.p.copy_(inputs["p0"].to(DEV))
+    arena.refresh_shadows()
+    trace = {k: [] for k in state}
+    for k, g in enumerate(inputs["scaled" if scaled else "unscaled"]):
+        arena.g.copy_(g.to(DEV))
+        if scaled:
+            assert float(arena.loss_scale) == PATHS_SCALES[k], (run, k)
+            arena.step(0.9, 0.999, 1e-8, 1e-2, 1.0, world_size=1, schedule=LrSchedule("linear", 2, 10, (0, 1)))
+        else:
+            arena.step(0.9, 0.999, 1e-8, 1e-2, 1.0, world_size=2)
+        for name, get in state.items():
+            trace[name].append(get().clone())
+    torch.cuda.synchronize()
+    out = {name: torch.cat(ts).cpu() for name, ts in trace.items()}
+    out.update(p=arena.p.cpu(), m=arena.m.cpu(), v=arena.v.cpu(), shadow=arena.shadow.cpu())
+    return out
+
+
+def _bits(t):
+    return t.view({4: torch.int32, 2: torch.int16}[t.element_size()]) if t.is_floating_point() else t
+
+
+def test_optimizer_paths_are_bit_identical_to_the_previous_release():
+    """Both launches with loss scaling (skips, growth, the device schedule) and the unscaled launch at
+    inv_world 0.5 keep the bits of the release before they shared one kernel. Bit patterns, not
+    torch.equal: a skipped step's norm is NaN."""
+    d = torch.load(os.path.join(GOLD, "optim_paths.pt"))
+    for run in OPTIM_PATHS:
+        got = optim_paths_run(run, d["inputs"])
+        assert got.keys() == d[run].keys(), run
+        for k, want in d[run].items():
+            assert torch.equal(_bits(got[k]), _bits(want)), (run, k)
 
 
 def test_scaler_state_dict_round_trips_grad_scaler_format():

@@ -110,8 +110,9 @@ def test_cpu_tensor_raises():
 
 
 def test_arena_clip_adamw_matches_torch_and_oracle():
-    """lb_adamw_clip_step vs torch.optim.AdamW + clip_grad_norm_ (what the reference calls) and
-    vs the float64 oracle, 4 steps, two param groups, with and without the clip being active.
+    """The optimizer launch (lb_optim_step_fused) vs torch.optim.AdamW + clip_grad_norm_ (what the
+    reference calls) and vs the float64 oracle, 4 steps, two param groups, with and without the clip
+    being active.
     Tolerance 2e-6 relative on the parameters (fp32 op-order differences only)."""
     import lora_b200 as L
     from lora_b200.arena import LoraArena

@@ -1,6 +1,7 @@
 """The step's prologue / loss-epilogue kernels (csrc/step_glue.cu) against the plain torch
 formulation the reference uses (scheduler.add_noise, cat, F.mse_loss: cli_lora_pti.py:295-370,
-train_lora_dreambooth.py:822-875), and the one-launch optimizer step against the three-launch one."""
+train_lora_dreambooth.py:822-875), and the one-launch optimizer step against the float64 oracle and
+lb_refresh_shadows."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -67,10 +68,10 @@ def test_masked_mse_and_its_gradient(fmt, dtype, variant):
 
 
 def _optimizer_run(sites_spec, mode):
-    """Three optimizer steps of a LoraArena over the same seeded gradients (the second one large
-    enough to clip). sites_spec: [("linear" | "conv", r)]; mode: "fused" (lb_optim_step_fused),
-    "split" (lb_adamw_clip_step + lb_refresh_shadows) or "dp" (lb_optim_step_dp at world = 1, with the
-    arena's own gradient buffer and a zeroed flag array as the only peer)."""
+    """Three optimizer steps of a LoraArena over seeded gradients (the second one large enough to
+    clip). sites_spec: [("linear" | "conv", r)]; mode: "fused" (lb_optim_step_fused) or "dp"
+    (lb_optim_step_dp at world = 1, with the arena's own gradient buffer and a zeroed flag array as
+    the only peer). Returns the arena, its start point and the three gradients."""
     import ctypes
     import torch.nn as nn
     import lora_b200 as L
@@ -82,19 +83,24 @@ def _optimizer_run(sites_spec, mode):
     for s in sites:
         s.lora_up.weight.data.normal_(0, 0.1)
     arena = LoraArena([(sites, 1e-3)])
-    arena.fused_step = mode != "split"
     if mode == "dp":
         arena._dp_flags = torch.zeros(2, device=DEV, dtype=torch.int32)
         arena._dp_epoch = torch.zeros(1, device=DEV, dtype=torch.int32)
         arena.gsum = torch.zeros_like(arena.g)
         one = ctypes.c_void_p * 1
         arena._dp = (one(arena.g.data_ptr()), one(arena._dp_flags.data_ptr()), 1, 0)
+    p0, grads = arena.p.clone(), []
     g = torch.Generator(device=DEV).manual_seed(5)
     for step in range(3):
-        arena.g.copy_(torch.randn(arena.n, device=DEV, generator=g) * (2.0 if step == 1 else 0.01))
+        grads.append(torch.randn(arena.n, device=DEV, generator=g) * (2.0 if step == 1 else 0.01))
+        arena.g.copy_(grads[-1])
         arena.step(0.9, 0.999, 1e-8, 1e-2, 1.0, world_size=1)
     torch.cuda.synchronize()
     assert float(arena.g.abs().max()) == 0.0 and int(arena.step_dev) == 3
+    return arena, p0, grads
+
+
+def _final_state(arena):
     return arena.p.clone(), arena.m.clone(), arena.v.clone(), arena.shadow.clone(), float(arena.gnorm)
 
 
@@ -109,13 +115,36 @@ def _assert_same_step(got, want):
     assert abs(got[4] - want[4]) <= 1e-6 * abs(want[4])
 
 
-def test_one_launch_optimizer_equals_three_launches():
-    """lb_optim_step_fused (cooperative: norm, grid barrier, AdamW + zero_grad, grid barrier, shadows)
-    against lb_adamw_clip_step (2 kernels) + lb_refresh_shadows: the same parameters, moments and shadows,
-    with 16-row shadow slots only and with 32-row ones (r = 32 linear and conv sites)."""
-    for spec in ([("linear", 4)] * 5 + [("conv", 8)],
-                 [("linear", 4)] * 4 + [("linear", 32), ("conv", 32)]):
-        _assert_same_step(_optimizer_run(spec, "fused"), _optimizer_run(spec, "split"))
+def test_one_launch_optimizer_matches_oracle_and_shadow_refresh():
+    """lb_optim_step_fused / lb_optim_step_dp at world 1 (cooperative: norm, grid barrier, AdamW +
+    zero_grad, grid barrier, shadows), with 16-row shadow slots only and with 32-row ones (r = 32
+    linear and conv sites): the shadows are bit for bit a fresh lb_refresh_shadows of the final
+    parameters, and p, m, v and the norm follow the float64 clip + AdamW of oracle.lora_ops (run
+    with the fp32-rounded hyper-parameters the launch receives)."""
+    from lora_b200 import _C
+    from lora_b200._C import check, dtype_code, ptr, stream_ptr
+    from oracle import lora_ops as O
+
+    def f32(x):
+        return float(torch.tensor(x, dtype=torch.float32))
+
+    specs = ([("linear", 4)] * 5 + [("conv", 8)], [("linear", 4)] * 4 + [("linear", 32), ("conv", 32)])
+    for mode, spec in ((mode, spec) for mode in ("fused", "dp") for spec in specs):
+        arena, p0, grads = _optimizer_run(spec, mode)
+        fresh = torch.zeros_like(arena.shadow)
+        check(_C.lib.lb_refresh_shadows(ptr(arena.p), ptr(arena.table), arena.table.shape[0], arena.table_max_c,
+                                        ptr(fresh), dtype_code(arena.compute_dtype), stream_ptr()),
+              "lb_refresh_shadows")
+        torch.cuda.synchronize()
+        assert torch.equal(arena.shadow.view(torch.int16), fresh.view(torch.int16)), (mode, spec)
+        p, m, v = [p0], [torch.zeros_like(p0)], [torch.zeros_like(p0)]
+        for step, g in enumerate(grads, 1):
+            p, m, v, total = O.clip_adamw_step(p, [g], m, v, step, [f32(1e-3)], beta1=f32(0.9), beta2=f32(0.999),
+                                               eps=f32(1e-8), weight_decay=f32(1e-2), max_norm=1.0)
+        for name, got, want in (("p", arena.p, p[0]), ("m", arena.m, m[0]), ("v", arena.v, v[0])):
+            err = float((got.double().cpu() - want).norm() / want.norm())
+            assert err < 2e-6, (mode, spec, name, err)
+        assert abs(float(arena.gnorm) - total) <= 1e-5 * total, (mode, spec)
 
 
 def test_data_parallel_optimizer_at_world_one_equals_one_launch():
@@ -123,4 +152,4 @@ def test_data_parallel_optimizer_at_world_one_equals_one_launch():
     lb_optim_step_fused on an identical arena with an r = 4 and an r = 32 site: the same parameters,
     moments and shadows."""
     spec = [("linear", 4), ("conv", 32)]
-    _assert_same_step(_optimizer_run(spec, "dp"), _optimizer_run(spec, "fused"))
+    _assert_same_step(_final_state(_optimizer_run(spec, "dp")[0]), _final_state(_optimizer_run(spec, "fused")[0]))

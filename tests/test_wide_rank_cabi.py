@@ -66,7 +66,7 @@ def test_r_pad_argument_of_every_entry_point_validates_without_gpu(L):
     # a pad of 16 keeps the rank limit of 16
     assert L.lb_cast_rows_pad(p, 1, 1, p, 17, 16, 64, 0, None) == -2
     assert L.lb_lora_wgrad(p, p, None, 1.0, p, 1, 1, 8, 64, 17, 16, 0, None) == -2
-    assert L.lb_abi_version() == 6
+    assert L.lb_abi_version() == 7
 
 
 def test_rank_pad():
