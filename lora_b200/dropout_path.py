@@ -17,6 +17,8 @@ The keep-mask is a hash of (per-call device seed, element index; csrc/dropmask.c
 parity with the reference under dropout is distributional (keep probability, 1/(1-p) scaling,
 forward/backward mask consistency; tests/test_dropout_gpu.py), not bitwise.
 """
+from collections import deque
+
 import torch
 
 from . import ops
@@ -28,28 +30,54 @@ class _SeedPool:
     """One device-side draw of mask seeds per training step instead of one tiny RNG launch per
     dropout site (224 sites in the extended SD1.5 set): the step engine calls `begin_step`, every
     dropout forward takes the next int64 slot (a 1-element view: the kernels read the seed through
-    a device pointer, so a captured graph re-reads freshly drawn values on every replay)."""
+    a device pointer, so a captured graph re-reads freshly drawn values on every replay).
+
+    Gradient checkpointing runs a site's forward a second time inside the backward pass. That
+    recompute must draw the keep-mask its first forward drew -- the rest of the network consumed
+    that output -- so every forward records the slot it took (`taken`, per site, in call order) and
+    a forward that runs inside the backward pass takes the site's oldest recorded slot instead of a
+    new one. This holds whoever called torch.utils.checkpoint (the host UNet, transformers' CLIP, a
+    caller's own model). Without a step engine the seeds come from torch's CUDA generator, whose
+    state torch.utils.checkpoint restores before a recompute (preserve_rng_state, its default)."""
     pool = None
     used = 0
+    taken = {}        # id(site module) -> deque of the slots its forwards took this step
 
 
 def begin_step(device, n_slots: int = 1024):
     """Draw this step's mask seeds (graph-capturable: torch's CUDA generator, new values per replay)."""
     _SeedPool.pool = torch.randint(0, 2 ** 62, (n_slots,), device=device, dtype=torch.int64)
     _SeedPool.used = 0
+    _SeedPool.taken = {}
 
 
 def end_step():
     _SeedPool.pool = None
     _SeedPool.used = 0
+    _SeedPool.taken = {}
 
 
-def _fresh_seed(device) -> torch.Tensor:
+def _in_backward() -> bool:
+    """True while the autograd engine runs a backward pass on this thread: a forward called now is a
+    gradient-checkpointing recompute."""
+    return torch._C._current_graph_task_id() != -1
+
+
+def _fresh_seed(mod, device) -> torch.Tensor:
     pool = _SeedPool.pool
-    if pool is not None and pool.device == device and _SeedPool.used < pool.numel():
-        i = _SeedPool.used
-        _SeedPool.used = i + 1
-        return pool[i:i + 1]
+    if pool is not None and pool.device == device:
+        recompute = _in_backward()
+        if recompute:
+            slots = _SeedPool.taken.get(id(mod))
+            if slots:
+                i = slots.popleft()
+                return pool[i:i + 1]
+        if _SeedPool.used < pool.numel():
+            i = _SeedPool.used
+            _SeedPool.used = i + 1
+            if not recompute:
+                _SeedPool.taken.setdefault(id(mod), deque()).append(i)
+            return pool[i:i + 1]
     # no step engine around this call: drawn on the device from torch's CUDA generator
     return torch.randint(0, 2 ** 62, (1,), device=device, dtype=torch.int64)
 
@@ -73,7 +101,7 @@ class _LoraLinearDropoutFn(torch.autograd.Function):
         B32 = _fp32_master(B)
         diag = mod._selector_diag()
         scale, p = float(mod.scale), float(mod.dropout.p)
-        seed = _fresh_seed(x.device)
+        seed = _fresh_seed(mod, x.device)
         y, T = ops.fused_linear(x2d, w16, b32, down16, B32, r, 1, diag, scale, r, odt, True,
                                 drop_p=p, seed=seed)
         ctx.mod, ctx.cdt, ctx.scale, ctx.p, ctx.diag = mod, cdt, scale, p, diag
@@ -142,7 +170,7 @@ class _LoraConv2dDropoutFn(torch.autograd.Function):
         B32 = _fp32_master(B)
         diag = mod._selector_diag()
         scale, p = float(mod.scale), float(mod.dropout.p)
-        seed = _fresh_seed(x.device)
+        seed = _fresh_seed(mod, x.device)
         cout = conv.out_channels
         y, T = ops.fused_conv2d(x16, w_f, b32, down16, B32, 0, r, 1, 0, diag, scale, r, cout, kh, kw,
                                 ph, pw, False, odt, True, drop_p=p, seed=seed)

@@ -206,13 +206,21 @@ def forward_maybe_grouped(site, x):
     ent = st.cache.pop(id(site), None)
     if ent is not None and ent[0] == k and ent[3] == _site_sig(site):
         return ent[2]
+    # a forward inside the backward pass is a gradient-checkpointing recompute: it must launch exactly
+    # what the pass it recomputes launched (torch.utils.checkpoint matches the saved tensors one by
+    # one), so it never learns, finalizes or relearns families -- it only reuses what is learned
+    recompute = torch._C._current_graph_task_id() != -1
     if not st.learned:
+        if recompute:
+            return None
         if any(s is site for s, _ in st.trace):
             st.finalize()               # the same site again: the previous pass is complete
         else:
             st.trace.append((site, k))
             return None
     if id(site) not in st.groups:       # a site this parent has never seen (re-patched model): relearn
+        if recompute:
+            return None
         st.__init__()
         st.trace.append((site, k))
         return None

@@ -30,6 +30,7 @@ from typing import Optional, Tuple, Union
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.utils.checkpoint import checkpoint
 
 
 @dataclass
@@ -192,6 +193,22 @@ class ResnetBlock2D(nn.Module):
         return x + h
 
 
+def _capturing() -> bool:
+    return torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing()
+
+
+def _run(block: nn.Module, layer: nn.Module, *args):
+    """diffusers' gradient checkpointing of one ResnetBlock2D / Transformer2DModel call: in training
+    mode with checkpointing on, the layer's activations are dropped after the forward and recomputed
+    in backward (non-reentrant, so frozen inputs still give every LoRA factor its gradient). torch's
+    generator state cannot be read or set while a CUDA graph is captured; nothing in this model draws
+    from it then (its own dropouts are p = 0, LoRA dropout seeds come from the step's seed pool), so a
+    capture skips stashing it."""
+    if block.gradient_checkpointing and block.training:
+        return checkpoint(layer, *args, use_reentrant=False, preserve_rng_state=not _capturing())
+    return layer(*args)
+
+
 class Downsample2D(nn.Module):
     def __init__(self, channels: int):
         super().__init__()
@@ -222,13 +239,14 @@ class DownBlock(nn.Module):
             [ResnetBlock2D(cin if i == 0 else cout, cout, temb, groups) for i in range(layers)])
         self.downsamplers = nn.ModuleList([Downsample2D(cout)]) if add_down else None
         self.has_attn = has_attn
+        self.gradient_checkpointing = False
 
     def forward(self, x, temb, context):
         outs = []
         for i, res in enumerate(self.resnets):
-            x = res(x, temb)
+            x = _run(self, res, x, temb)
             if self.has_attn:
-                x = self.attentions[i](x, context)
+                x = _run(self, self.attentions[i], x, context)
             outs.append(x)
         if self.downsamplers is not None:
             x = self.downsamplers[0](x)
@@ -252,13 +270,14 @@ class UpBlock(nn.Module):
         self.resnets = nn.ModuleList(resnets)
         self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_up else None
         self.has_attn = has_attn
+        self.gradient_checkpointing = False
 
     def forward(self, x, skips, temb, context):
         for i, res in enumerate(self.resnets):
             x = torch.cat([x, skips.pop()], dim=1)
-            x = res(x, temb)
+            x = _run(self, res, x, temb)
             if self.has_attn:
-                x = self.attentions[i](x, context)
+                x = _run(self, self.attentions[i], x, context)
         if self.upsamplers is not None:
             x = self.upsamplers[0](x)
         return x
@@ -271,11 +290,12 @@ class MidBlock(nn.Module):
         super().__init__()
         self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, ctx_dim, groups, linear)])
         self.resnets = nn.ModuleList([ResnetBlock2D(ch, ch, temb, groups) for _ in range(2)])
+        self.gradient_checkpointing = False
 
     def forward(self, x, temb, context):
-        x = self.resnets[0](x, temb)
-        x = self.attentions[0](x, context)
-        return self.resnets[1](x, temb)
+        x = _run(self, self.resnets[0], x, temb)
+        x = _run(self, self.attentions[0], x, context)
+        return _run(self, self.resnets[1], x, temb)
 
 
 class TimestepEmbedding(nn.Module):
@@ -342,6 +362,26 @@ class UNet2DConditionModel(nn.Module):
         self.mid_block = MidBlock(ch[-1], temb, heads[-1], cfg.cross_attention_dim, g, linear=lin)
         self.conv_norm_out = nn.GroupNorm(g, ch[0], eps=1e-5)
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
+
+    # diffusers' gradient-checkpointing API: every ResnetBlock2D and Transformer2DModel of the down,
+    # mid and up blocks runs under torch.utils.checkpoint in training mode; conv_in, the time
+    # embedding, the samplers and conv_out are never checkpointed
+    _supports_gradient_checkpointing = True
+
+    def _set_gradient_checkpointing(self, value: bool):
+        for m in self.modules():
+            if hasattr(m, "gradient_checkpointing"):
+                m.gradient_checkpointing = value
+
+    def enable_gradient_checkpointing(self):
+        self._set_gradient_checkpointing(True)
+
+    def disable_gradient_checkpointing(self):
+        self._set_gradient_checkpointing(False)
+
+    @property
+    def is_gradient_checkpointing(self) -> bool:
+        return any(getattr(m, "gradient_checkpointing", False) for m in self.modules())
 
     @property
     def device(self):

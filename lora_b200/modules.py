@@ -315,6 +315,7 @@ class LoraInjectedLinear(nn.Module):
         return torch.diagonal(w.reshape(self.r, self.r)).to(torch.float32).contiguous()
 
     def forward(self, input):
+        ops.wgrad_segment_boundary()
         if self.r > ops.MAX_RANK:   # joined LoRAs above rank 64 (lora_manager.py:13-71): rank chunks of 64
             from .rank_chunks import lora_linear_chunked
             return lora_linear_chunked(self, input)
@@ -380,6 +381,7 @@ class LoraInjectedConv2d(nn.Module):
         return torch.diagonal(w.reshape(self.r, self.r)).to(torch.float32).contiguous()
 
     def forward(self, input):
+        ops.wgrad_segment_boundary()
         from .conv_path import lora_conv2d
         return lora_conv2d(self, input)
 

@@ -32,7 +32,8 @@ def _count(n: int = 1):
 # Deferred factor gradients: dA / dB feed only the optimizer, so (when they accumulate straight into
 # an arena) a step engine can QUEUE every linear-site reduction of the backward pass and run them
 # all in ceil(n/24) launches at its end (lb_lora_wgrad_batch) instead of one small launch per site.
-# The queue keeps the operand tensors alive until the flush.
+# The queue keeps the operand tensors alive until the flush; under gradient checkpointing it is also
+# flushed when the next segment's recompute starts (wgrad_segment_boundary).
 import ctypes as _ct
 
 
@@ -75,17 +76,35 @@ def _wgrad_enqueue(S, V, out, out_js, out_cs, M, C, r, scale, diag, drop_p=0.0, 
     _WG_QUEUE.setdefault(S.dtype, []).append((item, (S, V, out, diag, seed)))
 
 
+def _wgrad_launch_all(q) -> int:
+    n_launch = 0
+    for dtype, items in q.items():
+        if items:
+            n_launch += _wgrad_launch(dtype, items)
+    return n_launch
+
+
 def wgrad_flush():
     """Run every queued reduction (lb_lora_wgrad_batch) and leave deferral mode."""
     global _WG_QUEUE
     q, _WG_QUEUE = _WG_QUEUE, None
     if not q:
         return 0
-    n_launch = 0
-    for dtype, items in q.items():
-        if items:
-            n_launch += _wgrad_launch(dtype, items)
-    return n_launch
+    return _wgrad_launch_all(q)
+
+
+def wgrad_segment_boundary() -> int:
+    """Called by every LoRA site's forward. A forward that runs inside the backward pass is a
+    gradient-checkpointing recompute, so the backward of the segment checkpointed before it (later
+    in the forward order) has finished: run what the queue holds now and keep deferring. The queue
+    then never keeps one segment's recomputed activations alive while the next one is recomputed;
+    the step takes about one batched launch per checkpointed segment with LoRA sites instead of
+    ceil(n/24). Without checkpointing no site forward runs during backward and nothing changes."""
+    global _WG_QUEUE
+    if not _WG_QUEUE or torch._C._current_graph_task_id() == -1:
+        return 0
+    q, _WG_QUEUE = _WG_QUEUE, {}
+    return _wgrad_launch_all(q)
 
 
 def _req_cuda(*ts):

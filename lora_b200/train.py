@@ -99,6 +99,22 @@ class StepConfig:
     growth_factor: float = 2.0
     backoff_factor: float = 0.5
     growth_interval: int = 2000
+    # `--gradient_checkpointing` (train_lora_dreambooth.py:627-630): unet.enable_gradient_checkpointing(),
+    # and text_encoder.gradient_checkpointing_enable() when the text encoder runs with gradients. Every
+    # ResnetBlock2D / Transformer2DModel / CLIP encoder layer drops its activations after the forward
+    # and runs again in backward: less activation memory for one more forward. Gradients equal the
+    # un-checkpointed ones (non-reentrant checkpointing; dropout masks survive the recompute).
+    gradient_checkpointing: bool = False
+
+
+def _enable_gradient_checkpointing(unet: nn.Module, text_encoder: nn.Module, text_grad: bool):
+    """train_lora_dreambooth.py:627-630. The step draws nothing from torch's generator inside a
+    checkpointed segment (LoRA dropout seeds come from dropout_path's pool), and the generator state
+    cannot be read while a CUDA graph is captured: CLIP's layers skip stashing it."""
+    unet.enable_gradient_checkpointing()
+    if text_grad:
+        text_encoder.gradient_checkpointing_enable(
+            gradient_checkpointing_kwargs={"use_reentrant": False, "preserve_rng_state": False})
 
 
 PREDICTION_TYPES = ("epsilon", "v_prediction")
@@ -203,6 +219,8 @@ class LoraTrainStep:
                 self.arena._dp = None
         self.unet.train()
         self.text_encoder.train()
+        if cfg.gradient_checkpointing:
+            _enable_gradient_checkpointing(unet, text_encoder, cfg.train_text_encoder or self._text_encoder_grad)
 
     # ------------------------------------------------------------------ the step body
     def _fwd_bwd(self):
@@ -516,6 +534,8 @@ class TextualInversionStep(LoraTrainStep):
                         self._frozen.append(prm)
         self.unet.eval()               # cli_lora_pti.py:411-412
         self.text_encoder.train()
+        if cfg.gradient_checkpointing:  # the UNet runs in eval mode here: only the text encoder recomputes
+            _enable_gradient_checkpointing(unet, text_encoder, cfg.train_text_encoder)
 
     def prepare(self):
         return None                    # eager loop (phase 1 is not the timed path)
