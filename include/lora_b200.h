@@ -498,6 +498,38 @@ int lb_step_prologue_v(const float* latents, const float* noise, const long long
                        const float* inpaint_mask, const float* masked_latents, void* out, int out_dtype,
                        float* velocity, int B, int C, int H, int W, void* stream);
 
+/* Image ingest, one launch (torchvision ToTensor + Normalize([0.5], [0.5]) of the reference's datasets,
+ * dataset.py:108-116): pixels_u8 = 1: pixels uint8 [B,H,W,3] (HWC, as decoded), each value evaluated
+ * op by op as x / 255.f, (x - 0.5f) / 0.5f (no contraction: bit-equal to torchvision); pixels_u8 = 0:
+ * pixels fp32 [B,3,H,W], already normalised (a cast). out [B,3,H,W] of out_dtype, NCHW or
+ * (channels_last = 1) NHWC. mask [B,1,H,W] fp32 (mask_u8 = 0) or uint8 (1), and masked_out (same
+ * layout as out), both or neither: masked_out = image * (mask < 0.5), the product in fp32. */
+int lb_pixels_ingest(const void* pixels, int pixels_u8, const void* mask, int mask_u8, void* out,
+                     void* masked_out, int out_dtype, int channels_last, int B, int H, int W, void* stream);
+
+/* lb_step_prologue / lb_step_prologue_v with the VAE posterior sample in front, one launch
+ * (train_lora_dreambooth.py:818-821, cli_lora_pti.py:273-290). moments: diffusers'
+ * DiagonalGaussianDistribution.parameters [B,2C,H,W] of moments_dtype (mean = channels < C, logvar
+ * the rest), element (b, c, pixel) at b*stride_b + c*stride_c + pixel*stride_p (NCHW or channels_last).
+ * posterior_noise [B,C,H,W] NCHW of moments_dtype or LB_F32 (other dtypes: LB_ERR_DTYPE).
+ *   latents = (mean + exp(0.5 * clamp(logvar, -30, 20)) * posterior_noise) * scaling
+ * with the clamp, product by 0.5 and exp rounded to moments_dtype and the rest to the promoted dtype
+ * (fp32 when posterior_noise is fp32), as torch evaluates it; written to `latents` (fp32 NCHW) and
+ * then noised exactly as lb_step_prologue does (velocity NULL) or lb_step_prologue_v (velocity fp32
+ * NCHW). Inpainting: mask [B,1,8H,8W] fp32 (mask_u8 = 0) or uint8 (1) at image resolution, with
+ * masked_moments (same strides as moments), masked_posterior_noise, masked_latents and inpaint_mask
+ * [B,1,H,W] fp32 outputs: inpaint_mask = mask[b, 0, 8h, 8w] (F.interpolate(scale_factor=1/8),
+ * nearest), masked_latents the posterior sample of masked_moments; out is the 9-channel concat.
+ * NULL mask: no inpainting (the masked_* arguments are ignored). */
+int lb_step_prologue_posterior(const void* moments, int moments_dtype, long long stride_b, long long stride_c,
+                               long long stride_p, const void* posterior_noise, int posterior_noise_dtype,
+                               float scaling, float* latents, const void* masked_moments,
+                               const void* masked_posterior_noise, const void* mask, int mask_u8,
+                               float* masked_latents, float* inpaint_mask, const float* noise,
+                               const long long* timesteps, const float* sqrt_acp,
+                               const float* sqrt_one_minus_acp, int n_timesteps, void* out, int out_dtype,
+                               float* velocity, int B, int C, int H, int W, void* stream);
+
 /* Loss epilogue, one launch (cli_lora_pti.py:340-370, train_lora_dreambooth.py:855-875):
  *   loss = sum_b weights[b] * mean_{c,h,w} (mask[b,h,w] * (pred - target))^2      (weights NULL: 1/B)
  *   grad = d loss / d pred = 2 weights[b] mask^2 (pred - target) / (C H W)        (pred's dtype/layout)

@@ -1,14 +1,19 @@
 // The two ends of a training step, either side of the UNet call:
+//   lb_pixels_ingest      uint8 HWC images -> ToTensor + Normalize([0.5], [0.5]) -> the VAE's dtype and
+//                         layout (+ the inpainting masked image), dataset.py:108-116, 240-252
 //   lb_step_prologue      scheduler.add_noise + cast + NCHW -> NHWC (+ the inpainting concat)
 //                         cli_lora_pti.py:295-313, train_lora_dreambooth.py:822-840
 //   lb_step_prologue_v    the same, plus the v-prediction target scheduler.get_velocity
 //                         cli_lora_pti.py:333-338, train_lora_dreambooth.py:846-853
+//   lb_step_prologue_posterior  the same with the VAE posterior sample in front:
+//                         latent_dist.sample() * 0.18215 (+ the latent-grid inpainting mask),
+//                         train_lora_dreambooth.py:818-821, cli_lora_pti.py:273-290
 //   lb_masked_mse_fwd_bwd the (mask-weighted) MSE of cli_lora_pti.py:340-370 /
 //                         train_lora_dreambooth.py:855-875 and its gradient w.r.t. the prediction,
 //                         in one pass (the loss is a scalar: its backward is known in the forward),
 //                         optionally times the fp16 loss scale (GradScaler.scale(loss).backward())
-// Both are HBM-bound over a few hundred KB: what they buy is launch count (about ten small torch
-// kernels per step and their intermediates), not bandwidth.
+// All are HBM-bound over a few hundred KB (a few MB of pixels): what they buy is launch count (about
+// ten small torch kernels per step and their intermediates), not bandwidth.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -28,6 +33,26 @@ __device__ __forceinline__ void st_any(void* p, long long i, int dt, float x) {
   else if (dt == LB_BF16) reinterpret_cast<__nv_bfloat16*>(p)[i] = __float2bfloat16_rn(x);
   else reinterpret_cast<__half*>(p)[i] = __float2half_rn(x);
 }
+// x rounded to dt and widened back: torch's result of one bf16 / fp16 op evaluated in fp32
+__device__ __forceinline__ float round_to(int dt, float x) {
+  if (dt == LB_BF16) return __bfloat162float(__float2bfloat16_rn(x));
+  if (dt == LB_F16) return __half2float(__float2half_rn(x));
+  return x;
+}
+
+// two rounded products and one rounded sum (difference), as torch evaluates add_noise and
+// get_velocity (no FMA contraction): both equal torch's result bit for bit
+__device__ __forceinline__ void noise_one(void* out, long long o, int out_dt, float* velocity, long long src,
+                                          float a, float s, float x, float e) {
+  st_any(out, o, out_dt, __fadd_rn(__fmul_rn(a, x), __fmul_rn(s, e)));
+  if (velocity) velocity[src] = __fsub_rn(__fmul_rn(a, e), __fmul_rn(s, x));   // consecutive px: coalesced
+}
+
+__device__ __forceinline__ float clamp_timestep_coef(const long long* t, const float* tab, int b, int T) {
+  long long tt = t[b];
+  tt = tt < 0 ? 0 : (tt >= T ? T - 1 : tt);
+  return tab[tt];
+}
 
 // out[b, p, c] (NHWC, C_out = C or C + 1 + C) = sqrt_acp[t_b] * x0[b, c, p] + sqrt_1m[t_b] * eps[b, c, p]
 // for c < C; channel C = inpaint mask[b, p]; channels C+1.. = masked-image latents[b, c', p].
@@ -40,23 +65,111 @@ prologue_kernel(const float* __restrict__ x0, const float* __restrict__ eps, con
   const long long i = blockIdx.x * 256ll + threadIdx.x;
   if (i >= static_cast<long long>(B) * P) return;
   const int b = static_cast<int>(i / P), px = static_cast<int>(i % P);
-  long long tt = t[b];
-  tt = tt < 0 ? 0 : (tt >= T ? T - 1 : tt);
-  const float a = sqrt_acp[tt], s = sqrt_1m[tt];
+  const float a = clamp_timestep_coef(t, sqrt_acp, b, T), s = clamp_timestep_coef(t, sqrt_1m, b, T);
   const int c_out = inp_mask ? 2 * C + 1 : C;
   const long long obase = i * c_out;
   for (int c = 0; c < C; ++c) {
     const long long src = (static_cast<long long>(b) * C + c) * P + px;
-    const float x = x0[src], e = eps[src];
-    // two rounded products and one rounded sum (difference), as torch evaluates add_noise and
-    // get_velocity (no FMA contraction): both equal torch's result bit for bit
-    st_any(out, obase + c, out_dt, __fadd_rn(__fmul_rn(a, x), __fmul_rn(s, e)));
-    if (velocity) velocity[src] = __fsub_rn(__fmul_rn(a, e), __fmul_rn(s, x));   // consecutive px: coalesced
+    noise_one(out, obase + c, out_dt, velocity, src, a, s, x0[src], eps[src]);
   }
   if (inp_mask) {
     st_any(out, obase + C, out_dt, inp_mask[static_cast<long long>(b) * P + px]);
     for (int c = 0; c < C; ++c)
       st_any(out, obase + C + 1 + c, out_dt, masked_lat[(static_cast<long long>(b) * C + c) * P + px]);
+  }
+}
+
+// One pixel of torchvision's ToTensor + Normalize([0.5], [0.5]) on a uint8 value, op by op as the
+// data loader evaluates it on the CPU: x.float() / 255, then (x - 0.5) / 0.5, each rounded once.
+__device__ __forceinline__ float normalise_u8(unsigned char v) {
+  return __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(v), 255.f), 0.5f), 0.5f);
+}
+
+// out (VAE input, [B, 3, H, W] NCHW or channels_last, out_dt) <- pixels: uint8 [B, H, W, 3] (normalised
+// here) or fp32 [B, 3, H, W] (already normalised: a cast). With mask [B, 1, H, W] (fp32 or uint8):
+// masked = image * (mask < 0.5), the product in fp32, then the same cast (dataset.py:115).
+__global__ void __launch_bounds__(256)
+pixels_ingest_kernel(const void* __restrict__ pixels, int pixels_u8, const void* __restrict__ mask, int mask_u8,
+                     void* __restrict__ out, void* __restrict__ masked, int out_dt, int channels_last, int B,
+                     long long P) {
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= B * P) return;
+  const long long b = i / P, p = i % P;
+  float keep = 0.f;
+  if (mask) {
+    const float m = mask_u8 ? static_cast<float>(reinterpret_cast<const unsigned char*>(mask)[i])
+                            : reinterpret_cast<const float*>(mask)[i];
+    keep = m < 0.5f ? 1.f : 0.f;          // NaN < 0.5 is false, as in torch
+  }
+  for (int c = 0; c < 3; ++c) {
+    const long long nchw = (b * 3 + c) * P + p;
+    const float x = pixels_u8 ? normalise_u8(reinterpret_cast<const unsigned char*>(pixels)[i * 3 + c])
+                              : reinterpret_cast<const float*>(pixels)[nchw];
+    const long long o = channels_last ? i * 3 + c : nchw;
+    st_any(out, o, out_dt, x);
+    if (mask) st_any(masked, o, out_dt, __fmul_rn(x, keep));   // x * 0 keeps the sign of x, as torch does
+  }
+}
+
+// diffusers' DiagonalGaussianDistribution(moments).sample() * scaling, each op rounded as torch rounds
+// it: logvar.clamp(-30, 20) -> std = exp(0.5 * logvar) in the moments' dtype md; std * eps and
+// mean + that in the promoted dtype td (md when eps has md, else fp32); then * scaling in td.
+__device__ __forceinline__ float posterior_sample(const void* mom, int md, long long i_mean, long long i_logvar,
+                                                  const void* post_eps, int ed, long long i_eps, int td,
+                                                  float scaling) {
+  const float mean = ld_any(mom, i_mean, md);
+  float lv = ld_any(mom, i_logvar, md);
+  lv = lv < -30.f ? -30.f : (lv > 20.f ? 20.f : lv);     // torch.clamp: NaN stays NaN
+  const float sd = round_to(md, expf(round_to(md, __fmul_rn(0.5f, lv))));
+  const float x = round_to(td, __fadd_rn(mean, round_to(td, __fmul_rn(sd, ld_any(post_eps, i_eps, ed)))));
+  return round_to(td, __fmul_rn(x, scaling));
+}
+
+// prologue_kernel's output from VAE moments instead of latents: latents[b, c, p] = the posterior sample
+// (moments element (b, c, p) at b*sb + c*sc + p*sp, logvar C channels further; post_eps fp32 NCHW or
+// the moments' dtype), written out in fp32 and noised as prologue_kernel does. Inpainting (mask != NULL):
+// the latent-grid mask is mask[b, 0, 8h, 8w] of the image-resolution mask (F.interpolate(scale_factor=
+// 1/8), nearest), the masked-image latents the posterior sample of the masked moments; both are written
+// out (fp32 NCHW) and into the concat.
+__global__ void __launch_bounds__(256)
+prologue_posterior_kernel(const void* __restrict__ mom, int md, long long sb, long long sc, long long sp,
+                          const void* __restrict__ post_eps, int ed, float scaling, float* __restrict__ lat_out,
+                          const void* __restrict__ mmom, const void* __restrict__ mpost_eps,
+                          const void* __restrict__ mask, int mask_u8, float* __restrict__ mlat_out,
+                          float* __restrict__ mask_out, const float* __restrict__ eps,
+                          const long long* __restrict__ t, const float* __restrict__ sqrt_acp,
+                          const float* __restrict__ sqrt_1m, void* __restrict__ out, int out_dt,
+                          float* __restrict__ velocity, int B, int C, int H, int W, int T) {
+  const int P = H * W;
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= static_cast<long long>(B) * P) return;
+  const int b = static_cast<int>(i / P), px = static_cast<int>(i % P);
+  const float a = clamp_timestep_coef(t, sqrt_acp, b, T), s = clamp_timestep_coef(t, sqrt_1m, b, T);
+  const int td = ed == md ? md : LB_F32;
+  const int c_out = mask ? 2 * C + 1 : C;
+  const long long obase = i * c_out;
+  const long long mbase = b * sb + px * sp;
+  for (int c = 0; c < C; ++c) {
+    const long long src = (static_cast<long long>(b) * C + c) * P + px;
+    const long long mi = mbase + c * sc;
+    const float x = posterior_sample(mom, md, mi, mi + C * sc, post_eps, ed, src, td, scaling);
+    lat_out[src] = x;
+    noise_one(out, obase + c, out_dt, velocity, src, a, s, x, eps[src]);
+  }
+  if (mask) {
+    const int h = px / W, w = px % W;
+    const long long mpix = (static_cast<long long>(b) * 8 * H + 8 * h) * (8ll * W) + 8 * w;
+    const float m = mask_u8 ? static_cast<float>(reinterpret_cast<const unsigned char*>(mask)[mpix])
+                            : reinterpret_cast<const float*>(mask)[mpix];
+    mask_out[static_cast<long long>(b) * P + px] = m;
+    st_any(out, obase + C, out_dt, m);
+    for (int c = 0; c < C; ++c) {
+      const long long src = (static_cast<long long>(b) * C + c) * P + px;
+      const long long mi = mbase + c * sc;
+      const float x = posterior_sample(mmom, md, mi, mi + C * sc, mpost_eps, ed, src, td, scaling);
+      mlat_out[src] = x;
+      st_any(out, obase + C + 1 + c, out_dt, x);
+    }
   }
 }
 
@@ -145,6 +258,45 @@ extern "C" int lb_step_prologue_v(const float* latents, const float* noise, cons
   if (velocity == nullptr) return LB_ERR_SHAPE;
   return launch_prologue(latents, noise, timesteps, sqrt_acp, sqrt_one_minus_acp, n_timesteps, inpaint_mask,
                          masked_latents, out, out_dtype, velocity, B, C, H, W, stream);
+}
+
+static bool float_dtype(int dt) { return dt == LB_BF16 || dt == LB_F16 || dt == LB_F32; }
+
+extern "C" int lb_pixels_ingest(const void* pixels, int pixels_u8, const void* mask, int mask_u8, void* out,
+                                void* masked_out, int out_dtype, int channels_last, int B, int H, int W,
+                                void* stream) {
+  if (B <= 0 || H <= 0 || W <= 0 || pixels == nullptr || out == nullptr) return LB_ERR_SHAPE;
+  if (!float_dtype(out_dtype)) return LB_ERR_DTYPE;
+  if ((mask == nullptr) != (masked_out == nullptr)) return LB_ERR_SHAPE;
+  const long long P = static_cast<long long>(H) * W, n = B * P;
+  pixels_ingest_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      pixels, pixels_u8 != 0, mask, mask_u8 != 0, out, masked_out, out_dtype, channels_last != 0, B, P);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_step_prologue_posterior(const void* moments, int moments_dtype, long long stride_b,
+                                          long long stride_c, long long stride_p, const void* posterior_noise,
+                                          int posterior_noise_dtype, float scaling, float* latents,
+                                          const void* masked_moments, const void* masked_posterior_noise,
+                                          const void* mask, int mask_u8, float* masked_latents,
+                                          float* inpaint_mask, const float* noise, const long long* timesteps,
+                                          const float* sqrt_acp, const float* sqrt_one_minus_acp,
+                                          int n_timesteps, void* out, int out_dtype, float* velocity, int B,
+                                          int C, int H, int W, void* stream) {
+  if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || n_timesteps <= 0) return LB_ERR_SHAPE;
+  if (!float_dtype(moments_dtype) || !float_dtype(out_dtype)) return LB_ERR_DTYPE;
+  if (posterior_noise_dtype != moments_dtype && posterior_noise_dtype != LB_F32) return LB_ERR_DTYPE;
+  if (moments == nullptr || posterior_noise == nullptr || latents == nullptr) return LB_ERR_SHAPE;
+  const bool inp = mask != nullptr;
+  if (inp && (masked_moments == nullptr || masked_posterior_noise == nullptr || masked_latents == nullptr ||
+              inpaint_mask == nullptr))
+    return LB_ERR_SHAPE;
+  const long long n = static_cast<long long>(B) * H * W;
+  prologue_posterior_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      moments, moments_dtype, stride_b, stride_c, stride_p, posterior_noise, posterior_noise_dtype, scaling,
+      latents, masked_moments, masked_posterior_noise, mask, mask_u8 != 0, masked_latents, inpaint_mask, noise,
+      timesteps, sqrt_acp, sqrt_one_minus_acp, out, out_dtype, velocity, B, C, H, W, n_timesteps);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
 extern "C" int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long stride_b, long long stride_c,

@@ -1,8 +1,13 @@
 """The two ends of a training step as single kernels (csrc/step_glue.cu):
 
+  pixels_ingest     uint8 HWC images -> ToTensor + Normalize([0.5], [0.5]) -> the VAE's dtype,
+                    channels_last (+ the inpainting masked image)   dataset.py:108-116
   step_prologue     scheduler.add_noise + cast to the model dtype + NCHW -> channels_last
                     (+ the 9-channel inpainting concat)   cli_lora_pti.py:295-313
                     (+ the v-prediction target scheduler.get_velocity, cli_lora_pti.py:333-338)
+  step_prologue_posterior  the same with the VAE posterior sample in front
+                    (latent_dist.sample() * 0.18215, train_lora_dreambooth.py:818-821,
+                    cli_lora_pti.py:273-290)
   fused_masked_mse  (mask-weighted) MSE and its gradient w.r.t. the prediction in one pass
                     cli_lora_pti.py:340-370, train_lora_dreambooth.py:855-875
 
@@ -41,6 +46,119 @@ def step_prologue(latents: torch.Tensor, noise: torch.Tensor, timesteps: torch.T
         check(_C.lib.lb_step_prologue_v(*args, ptr(v), B, C, H, W, stream_ptr()), "lb_step_prologue_v")
     else:
         check(_C.lib.lb_step_prologue(*args, B, C, H, W, stream_ptr()), "lb_step_prologue")
+    ops._count()
+    return (out, v) if velocity else out
+
+
+def _mask_arg(mask: Optional[torch.Tensor], shape):
+    """(tensor, is_uint8) of a [B, 1, H, W] mask for the glue kernels: fp32 or uint8, contiguous."""
+    if mask is None:
+        return None, 0
+    if tuple(mask.shape) != tuple(shape):
+        raise _C.LoraB200Error(f"mask of shape {tuple(mask.shape)}, expected {tuple(shape)}")
+    if mask.dtype == torch.uint8:
+        return mask.contiguous(), 1
+    return mask.float().contiguous(), 0
+
+
+def pixels_ingest(pixels: torch.Tensor, out_dtype: torch.dtype, mask: Optional[torch.Tensor] = None,
+                  channels_last: bool = True):
+    """The VAE input from a batch of images, one launch: `(x, masked)`, [B, 3, H, W] tensors of
+    `out_dtype` (channels_last or contiguous NCHW); masked is None without a mask.
+
+    pixels: uint8 [B, H, W, 3] (decoded images, HWC) -> torchvision's ToTensor + Normalize([0.5], [0.5]),
+    bit for bit; or fp32 [B, 3, H, W] already normalised (a cast). mask: fp32 or uint8 [B, 1, H, W]:
+    masked = image * (mask < 0.5), the inpainting dataset's masked image (dataset.py:115)."""
+    if not pixels.is_cuda:
+        raise _C.LoraB200Error("pixels_ingest needs CUDA tensors (no CPU path)")
+    if pixels.dtype == torch.uint8:
+        if pixels.dim() != 4 or pixels.shape[3] != 3:
+            raise _C.LoraB200Error(f"uint8 pixels must be [B, H, W, 3], got {tuple(pixels.shape)}")
+        B, H, W, _ = pixels.shape
+    elif pixels.dtype == torch.float32:
+        if pixels.dim() != 4 or pixels.shape[1] != 3:
+            raise _C.LoraB200Error(f"float32 pixels must be [B, 3, H, W], got {tuple(pixels.shape)}")
+        B, _, H, W = pixels.shape
+    else:
+        raise _C.LoraB200Error(f"pixels must be uint8 or float32, got {pixels.dtype}")
+    px = pixels.contiguous()
+    m, m_u8 = _mask_arg(mask, (B, 1, H, W))
+    fmt = torch.channels_last if channels_last else torch.contiguous_format
+    x = torch.empty((B, 3, H, W), device=pixels.device, dtype=out_dtype, memory_format=fmt)
+    xm = None if m is None else torch.empty_like(x)
+    check(_C.lib.lb_pixels_ingest(ptr(px), int(px.dtype == torch.uint8), ptr(m), m_u8, ptr(x), ptr(xm),
+                                  dtype_code(out_dtype), int(channels_last), B, H, W, stream_ptr()),
+          "lb_pixels_ingest")
+    ops._count()
+    return x, xm
+
+
+def _moments_strides(moments: torch.Tensor):
+    sb, sc, sh, sw = moments.stride()
+    if sh != moments.shape[3] * sw:
+        moments = moments.contiguous()
+        sb, sc, sh, sw = moments.stride()
+    return moments, (sb, sc, sw)
+
+
+def step_prologue_posterior(moments: torch.Tensor, posterior_noise: torch.Tensor, noise: torch.Tensor,
+                            timesteps: torch.Tensor, noiser, out_dtype: torch.dtype, latents: torch.Tensor,
+                            scaling: float = 0.18215, masked_moments: Optional[torch.Tensor] = None,
+                            masked_posterior_noise: Optional[torch.Tensor] = None,
+                            mask: Optional[torch.Tensor] = None, masked_latents: Optional[torch.Tensor] = None,
+                            inpaint_mask: Optional[torch.Tensor] = None, velocity: bool = False):
+    """step_prologue with the VAE posterior sample in front, one launch.
+
+    moments: `vae.encode(x).latent_dist.parameters` [B, 2C, h, w] (mean ; logvar) in the VAE's dtype;
+    posterior_noise: [B, C, h, w] standard normal in that dtype or fp32. The latents
+    `DiagonalGaussianDistribution(moments).sample() * scaling` (each op rounded as torch rounds it) are
+    written to `latents` (fp32 [B, C, h, w], contiguous) and noised as step_prologue noises latents.
+    Inpainting: mask [B, 1, 8h, 8w] (image resolution, fp32 or uint8), masked_moments and
+    masked_posterior_noise give the masked-image latents; `masked_latents` ([B, C, h, w]) and
+    `inpaint_mask` ([B, 1, h, w], the mask at (8i, 8j): F.interpolate(scale_factor=1/8)) are fp32
+    outputs, and the UNet input is the 9-channel concat. Returns what step_prologue returns."""
+    if not moments.is_cuda:
+        raise _C.LoraB200Error("step_prologue_posterior needs CUDA tensors (no CPU path)")
+    B, C2, H, W = moments.shape
+    C = C2 // 2
+    shape = (B, C, H, W)
+    if C2 != 2 * C or tuple(posterior_noise.shape) != shape or tuple(latents.shape) != shape:
+        raise _C.LoraB200Error(f"moments {tuple(moments.shape)}, posterior noise {tuple(posterior_noise.shape)}, "
+                               f"latents {tuple(latents.shape)}: need [B, 2C, h, w] and two [B, C, h, w]")
+    if latents.dtype != torch.float32 or not latents.is_contiguous():
+        raise _C.LoraB200Error("latents must be a contiguous float32 tensor")
+    mom, (sb, sc, sp) = _moments_strides(moments)
+    pe = posterior_noise.contiguous()
+    eps = noise.float().contiguous()
+    t = timesteps.to(torch.int64).contiguous()
+    m, m_u8 = _mask_arg(mask, (B, 1, 8 * H, 8 * W))
+    mm = mpe = None
+    if m is not None:
+        if masked_moments is None or masked_posterior_noise is None or masked_latents is None or inpaint_mask is None:
+            raise _C.LoraB200Error("inpainting needs masked_moments, masked_posterior_noise, masked_latents and "
+                                   "inpaint_mask with the mask")
+        if tuple(masked_moments.shape) != tuple(moments.shape) or masked_moments.dtype != moments.dtype:
+            raise _C.LoraB200Error("masked_moments must have the shape and dtype of moments")
+        if (tuple(masked_posterior_noise.shape) != shape or masked_posterior_noise.dtype != posterior_noise.dtype
+                or tuple(masked_latents.shape) != shape or tuple(inpaint_mask.shape) != (B, 1, H, W)):
+            raise _C.LoraB200Error("masked posterior noise / masked_latents [B, C, h, w], inpaint_mask [B, 1, h, w]")
+        for o in (masked_latents, inpaint_mask):
+            if o.dtype != torch.float32 or not o.is_contiguous():
+                raise _C.LoraB200Error("masked_latents and inpaint_mask must be contiguous float32 tensors")
+        mm = masked_moments
+        if mm.stride() != mom.stride():          # one stride set serves both (two outputs of one VAE agree)
+            mom, mm = mom.contiguous(), mm.contiguous()
+            sb, sc, _, sp = mom.stride()
+        mpe = masked_posterior_noise.contiguous()
+    c_out = C if m is None else 2 * C + 1
+    out = torch.empty((B, c_out, H, W), device=moments.device, dtype=out_dtype, memory_format=torch.channels_last)
+    v = torch.empty(shape, device=moments.device, dtype=torch.float32) if velocity else None
+    check(_C.lib.lb_step_prologue_posterior(
+        ptr(mom), dtype_code(mom.dtype), sb, sc, sp, ptr(pe), dtype_code(pe.dtype), float(scaling), ptr(latents),
+        ptr(mm), ptr(mpe), ptr(m), m_u8, ptr(masked_latents if m is not None else None),
+        ptr(inpaint_mask if m is not None else None), ptr(eps), ptr(t), ptr(noiser.sqrt_acp),
+        ptr(noiser.sqrt_one_minus_acp), int(noiser.num_train_timesteps), ptr(out), dtype_code(out_dtype), ptr(v),
+        B, C, H, W, stream_ptr()), "lb_step_prologue_posterior")
     ops._count()
     return (out, v) if velocity else out
 

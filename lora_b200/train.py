@@ -105,6 +105,30 @@ class StepConfig:
     # and runs again in backward: less activation memory for one more forward. Gradients equal the
     # un-checkpointed ones (non-reentrant checkpointing; dropout masks survive the recompute).
     gradient_checkpointing: bool = False
+    # train from images (train_lora_dreambooth.py:818-821; cli_lora_pti.py:273-290 with cached_latents=False):
+    # the step's input is a batch of images (`self.pixels`, uint8 [B, 8h, 8w, 3] by default) that the frozen
+    # VAE (LoraTrainStep's `vae=`) encodes inside the step, in its own dtype, and a NEW posterior sample
+    # `latent_dist.sample() * vae_scaling` is drawn every step -- the trainers' behaviour, unlike
+    # step_ops.LatentCache, which freezes one sample per image. With train_inpainting the masked image is
+    # encoded too and the image-resolution mask (`self.pixel_mask`) is resized to the latent grid.
+    encode_images: bool = False
+    vae_scaling: float = 0.18215
+    # the posterior noise's dtype: False draws it in the VAE's dtype (current diffusers' randn_tensor),
+    # True in fp32 (diffusers releases of the reference's era; std * eps then promotes to fp32)
+    posterior_noise_fp32: bool = False
+    # the image buffer's dtype: torch.uint8 (decoded images, [B, H, W, 3]) or torch.float32 (images already
+    # normalised to [-1, 1] by a float loader, [B, 3, H, W])
+    pixel_dtype: torch.dtype = torch.uint8
+
+
+def _check_encode_images(cfg: StepConfig, vae):
+    """StepConfig.encode_images needs a VAE; refused before any CUDA call."""
+    if not cfg.encode_images:
+        return
+    if vae is None:
+        raise ValueError("StepConfig.encode_images needs the frozen VAE: pass vae= (an AutoencoderKL)")
+    if cfg.pixel_dtype not in (torch.uint8, torch.float32):
+        raise ValueError(f"StepConfig.pixel_dtype must be torch.uint8 or torch.float32, got {cfg.pixel_dtype}")
 
 
 def _enable_gradient_checkpointing(unet: nn.Module, text_encoder: nn.Module, text_grad: bool):
@@ -164,9 +188,10 @@ class LoraTrainStep:
     _arena_rows = None
 
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, cfg: StepConfig,
-                 latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
+                 latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None, vae: Optional[nn.Module] = None):
         _check_prediction_type(cfg)
         _check_grad_scaler(cfg)
+        _check_encode_images(cfg, vae)
         self.cfg = cfg
         self.unet, self.text_encoder = unet, text_encoder
         self.device = torch.device(device or "cuda")
@@ -192,6 +217,7 @@ class LoraTrainStep:
         if cfg.train_inpainting:
             self.inpaint_mask = torch.zeros((latent_shape[0], 1, latent_shape[2], latent_shape[3]), device=self.device)
             self.masked_latents = torch.zeros(latent_shape, device=self.device, dtype=torch.float32)
+        self._init_image_inputs(vae, latent_shape)
         self.global_step = 0
         # pinned host mirrors for the end-to-end path
         self.h_latents = torch.zeros(latent_shape, dtype=torch.float32).pin_memory()
@@ -222,6 +248,71 @@ class LoraTrainStep:
         if cfg.gradient_checkpointing:
             _enable_gradient_checkpointing(unet, text_encoder, cfg.train_text_encoder or self._text_encoder_grad)
 
+    def _init_image_inputs(self, vae, latent_shape):
+        """Static inputs of a StepConfig.encode_images step (graph-stable addresses): the images at 8x the
+        latent grid (+ the image-resolution inpainting mask) with pinned host mirrors, and with
+        external_noise the posterior noise beside `self.noise`. The latents buffers then hold what the
+        step samples: `self.latents` (and `self.masked_latents` / `self.inpaint_mask`) are outputs."""
+        self.vae = vae
+        cfg = self.cfg
+        if not cfg.encode_images:
+            return
+        B, _, h, w = latent_shape
+        self.vae_dtype = next(vae.parameters()).dtype
+        self.posterior_noise_dtype = torch.float32 if cfg.posterior_noise_fp32 else self.vae_dtype
+        shape = (B, 8 * h, 8 * w, 3) if cfg.pixel_dtype == torch.uint8 else (B, 3, 8 * h, 8 * w)
+        self.pixels = torch.zeros(shape, device=self.device, dtype=cfg.pixel_dtype)
+        self.h_pixels = torch.zeros(shape, dtype=cfg.pixel_dtype).pin_memory()
+        if cfg.train_inpainting:
+            self.pixel_mask = torch.zeros((B, 1, 8 * h, 8 * w), device=self.device, dtype=torch.float32)
+            self.h_pixel_mask = torch.zeros((B, 1, 8 * h, 8 * w), dtype=torch.float32).pin_memory()
+        if cfg.external_noise:
+            self.posterior_noise = torch.zeros(latent_shape, device=self.device, dtype=self.posterior_noise_dtype)
+            if cfg.train_inpainting:
+                self.masked_posterior_noise = torch.zeros_like(self.posterior_noise)
+
+    def _encode_images(self, fused: bool):
+        """train_lora_dreambooth.py:818-821 / cli_lora_pti.py:273-290: images -> VAE input -> the frozen
+        VAE (no_grad, its own dtype) -> posterior moments, then the posterior noise (image first, then
+        the masked image: the reference's draw order, before the step's noise and timesteps).
+        Returns (moments, posterior noise, masked moments, masked posterior noise) for the fused
+        prologue; the unfused path samples here, into self.latents (+ masked_latents, inpaint_mask)."""
+        cfg = self.cfg
+        inpaint = cfg.train_inpainting
+        with torch.no_grad():
+            if fused:
+                from .step_ops import pixels_ingest
+                x, xm = pixels_ingest(self.pixels, self.vae_dtype, self.pixel_mask if inpaint else None)
+            else:
+                x = self.pixels
+                if x.dtype == torch.uint8:           # torchvision's ToTensor + Normalize([0.5], [0.5])
+                    x = x.permute(0, 3, 1, 2).float().div(255).sub(0.5).div(0.5)
+                xm = x * (self.pixel_mask < 0.5) if inpaint else None        # dataset.py:115
+                x = x.to(self.vae_dtype).contiguous(memory_format=torch.channels_last)
+                if inpaint:
+                    xm = xm.to(self.vae_dtype).contiguous(memory_format=torch.channels_last)
+            moments = self.vae.encode(x).latent_dist.parameters
+            masked_moments = self.vae.encode(xm).latent_dist.parameters if inpaint else None
+        if cfg.external_noise:
+            pe = self.posterior_noise
+            mpe = self.masked_posterior_noise if inpaint else None
+        else:
+            pe = torch.randn(self.latents.shape, device=self.latents.device, dtype=self.posterior_noise_dtype)
+            mpe = torch.randn_like(pe) if inpaint else None
+        if not fused:
+            from .host.vae import DiagonalGaussianDistribution
+
+            def sample(m, e):                        # latent_dist.sample() * 0.18215
+                post = DiagonalGaussianDistribution(m)
+                return (post.mean + post.std * e) * cfg.vae_scaling
+
+            with torch.no_grad():
+                self.latents.copy_(sample(moments, pe))
+                if inpaint:
+                    self.masked_latents.copy_(sample(masked_moments, mpe))
+                    self.inpaint_mask.copy_(F.interpolate(self.pixel_mask, scale_factor=1 / 8))
+        return moments, pe, masked_moments, mpe
+
     # ------------------------------------------------------------------ the step body
     def _fwd_bwd(self):
         """noise -> text encoder -> UNet -> MSE -> backward; dA/dB land in the arena's g buffer."""
@@ -235,16 +326,27 @@ class LoraTrainStep:
                 for mod in (self.unet, self.text_encoder) for m in mod.modules())
         if lat.is_cuda and self._has_dropout:
             dropout_path.begin_step(lat.device)      # one RNG launch for all dropout sites of the step
+        fused = cfg.fused_glue and lat.is_cuda
+        if cfg.encode_images:
+            moments, post_eps, masked_moments, masked_post_eps = self._encode_images(fused)
         if cfg.external_noise:
             noise, timesteps = self.noise, self.timesteps
         else:
             noise = torch.randn_like(lat)
             t_max = int(self.noiser.num_train_timesteps * cfg.t_multiplier)
             timesteps = torch.randint(0, t_max, (bsz,), device=lat.device).long()
-        fused = cfg.fused_glue and lat.is_cuda
         v_pred = cfg.prediction_type == "v_prediction"
         target = noise
-        if fused:
+        if fused and cfg.encode_images:
+            from .step_ops import step_prologue_posterior
+            inp = cfg.train_inpainting
+            noisy = step_prologue_posterior(moments, post_eps, noise, timesteps, self.noiser, self.model_dtype, lat,
+                                            cfg.vae_scaling, masked_moments, masked_post_eps,
+                                            self.pixel_mask if inp else None, self.masked_latents if inp else None,
+                                            self.inpaint_mask if inp else None, velocity=v_pred)
+            if v_pred:
+                noisy, target = noisy
+        elif fused:
             from .step_ops import step_prologue
             noisy = step_prologue(lat, noise, timesteps, self.noiser, self.model_dtype,
                                   self.inpaint_mask if cfg.train_inpainting else None,
@@ -459,18 +561,53 @@ class LoraTrainStep:
             self._body()
         return self.loss
 
-    def step_host(self, latents_cpu: torch.Tensor, input_ids_cpu: torch.Tensor) -> torch.Tensor:
+    def step_host(self, latents_cpu: torch.Tensor, input_ids_cpu: torch.Tensor,
+                  mask: Optional[torch.Tensor] = None) -> torch.Tensor:
         """End-to-end step from pinned host memory: H2D inputs, step, D2H loss (async, returns the
-        pinned loss buffer; synchronise the stream before reading it)."""
-        self.h_latents.copy_(latents_cpu)
-        self.h_input_ids.copy_(input_ids_cpu)
-        self.latents.copy_(self.h_latents, non_blocking=True)
+        pinned loss buffer; synchronise the stream before reading it).
+        With StepConfig.encode_images the first argument is the batch of images instead, shaped and
+        typed like `self.pixels` (uint8 [B, 8h, 8w, 3], or fp32 [B, 3, 8h, 8w] with pixel_dtype
+        float32), and `mask` the image-resolution inpainting mask [B, 1, 8h, 8w] (train_inpainting)."""
+        if self.cfg.encode_images:
+            self._check_pixels(latents_cpu, mask)
+            self.h_pixels.copy_(latents_cpu)
+            self.pixels.copy_(self.h_pixels, non_blocking=True)
+            if mask is not None:
+                self.h_pixel_mask.copy_(mask.reshape(self.h_pixel_mask.shape))
+                self.pixel_mask.copy_(self.h_pixel_mask, non_blocking=True)
+            self.h_input_ids.copy_(input_ids_cpu)
+        else:
+            self.h_latents.copy_(latents_cpu)
+            self.h_input_ids.copy_(input_ids_cpu)
+            self.latents.copy_(self.h_latents, non_blocking=True)
         self.input_ids.copy_(self.h_input_ids, non_blocking=True)
         self.step_device()
         self.h_loss.copy_(self.loss, non_blocking=True)
         return self.h_loss
 
+    def _check_pixels(self, pixels: torch.Tensor, mask: Optional[torch.Tensor]):
+        """Refuse, before any copy, images the encode_images step cannot take."""
+        cfg = self.cfg
+        if pixels.dtype not in (torch.uint8, torch.float32):
+            raise ValueError(f"pixels must be uint8 or float32, got {pixels.dtype}")
+        if pixels.dtype != self.pixels.dtype:
+            raise ValueError(f"pixels are {pixels.dtype} but the step was built for StepConfig.pixel_dtype="
+                             f"{self.pixels.dtype}")
+        if tuple(pixels.shape) != tuple(self.pixels.shape):
+            raise ValueError(f"pixels of shape {tuple(pixels.shape)}: the step takes {tuple(self.pixels.shape)}, "
+                             f"8x the latent grid {tuple(self.latents.shape[2:])}")
+        if cfg.train_inpainting:
+            if mask is None:
+                raise ValueError("train_inpainting from images needs the image-resolution mask: step_host(..., mask=)")
+            if mask.numel() != self.pixel_mask.numel():
+                raise ValueError(f"mask of shape {tuple(mask.shape)}: the step takes {tuple(self.pixel_mask.shape)}")
+        elif mask is not None:
+            raise ValueError("a mask is the inpainting input: StepConfig.train_inpainting is off")
+
     def h2d_bytes(self) -> int:
+        if self.cfg.encode_images:
+            n = self.h_pixels.numel() * self.h_pixels.element_size() + self.h_input_ids.numel() * 8
+            return n + (self.h_pixel_mask.numel() * 4 if self.cfg.train_inpainting else 0)
         return self.h_latents.numel() * 4 + self.h_input_ids.numel() * 8
 
     def d2h_bytes(self) -> int:
@@ -492,10 +629,11 @@ class TextualInversionStep(LoraTrainStep):
 
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, placeholder_token_ids, cfg: StepConfig,
                  lr: float = 5e-4, weight_decay: float = 0.0, clip_ti_decay: bool = True,
-                 latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
+                 latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None, vae: Optional[nn.Module] = None):
         from .ti import TextualInversionRows
         _check_prediction_type(cfg)
         _check_grad_scaler(cfg, refuse="TextualInversionStep")
+        _check_encode_images(cfg, vae)
         self.cfg = cfg
         self.unet, self.text_encoder = unet, text_encoder
         self.device = torch.device(device or "cuda")
@@ -511,6 +649,7 @@ class TextualInversionStep(LoraTrainStep):
         if cfg.train_inpainting:
             self.inpaint_mask = torch.zeros((latent_shape[0], 1, latent_shape[2], latent_shape[3]), device=self.device)
             self.masked_latents = torch.zeros(latent_shape, device=self.device, dtype=torch.float32)
+        self._init_image_inputs(vae, latent_shape)
         from .dist import world_info
         _, self._world = world_info()
         if self._world > 1:
@@ -611,7 +750,8 @@ class LoraEmbeddingStep(LoraTrainStep):
 
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, placeholder_token_ids, cfg: StepConfig,
                  lr_embedding: float, mode: str = "table", unfreeze_lora_step: Optional[int] = None,
-                 row_capacity: int = 1024, latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
+                 row_capacity: int = 1024, latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None,
+                 vae: Optional[nn.Module] = None):
         from ._C import LoraB200Error
         from .embed_rows import MAX_SCATTER_TOKENS, MODES, EmbeddingRows
         from .dist import world_info
@@ -641,7 +781,7 @@ class LoraEmbeddingStep(LoraTrainStep):
                                row_capacity=int(row_capacity), D=int(D), vocab=int(table.shape[0]), mode=mode,
                                latent_shape=tuple(int(s) for s in latent_shape), seq_len=int(seq_len))
         self._arena_rows = (int(row_capacity), int(D), float(lr_embedding))
-        super().__init__(unet, text_encoder, cfg, latent_shape=latent_shape, seq_len=seq_len, device=device)
+        super().__init__(unet, text_encoder, cfg, latent_shape=latent_shape, seq_len=seq_len, device=device, vae=vae)
         self.rows = EmbeddingRows(text_encoder, self.arena, placeholder_token_ids, mode=mode,
                                   weight_decay=cfg.adam_weight_decay)
         if self._world > 1:
@@ -704,10 +844,11 @@ class LoraEmbeddingStep(LoraTrainStep):
         self.rows.restore(snap["rows"])
         super()._restore(snap)
 
-    def step_host(self, latents_cpu: torch.Tensor, input_ids_cpu: torch.Tensor) -> torch.Tensor:
+    def step_host(self, latents_cpu: torch.Tensor, input_ids_cpu: torch.Tensor,
+                  mask: Optional[torch.Tensor] = None) -> torch.Tensor:
         """LoraTrainStep.step_host; an overflow of the row slots in this step raises no later than the
         next call (the flag is copied to pinned memory behind the step and read one call later)."""
-        out = super().step_host(latents_cpu, input_ids_cpu)
+        out = super().step_host(latents_cpu, input_ids_cpu, mask)
         i = self._host_calls % 2
         self._h_flags[i].copy_(self.rows.state[3:4], non_blocking=True)
         ev = torch.cuda.Event()
