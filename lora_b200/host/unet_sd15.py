@@ -22,6 +22,22 @@ cross-attention dim 1024 (OpenCLIP-H text encoder, host/clip.py) and `nn.Linear`
 the SD2 UNet has the same 144 default sites. diffusers' `upcast_attention` (softmax in fp32 for the
 768-v model) is not restated: F.scaled_dot_product_attention already keeps its softmax in fp32 under
 bf16 / fp16, and attention scores are not a LoRA site.
+
+SDXL (`UNetConfig.sdxl()`, stable-diffusion-xl-base-1.0's UNet) takes the same line further:
+  * three blocks (320, 640, 1280), no attention in the first down block (nor the last up block), heads
+    (5, 10, 20) -- head dim 64 --, cross-attention dim 2048 (the two text encoders' states concatenated,
+    host/clip.py:build_sdxl_text_encoders) and linear proj_in / proj_out;
+  * `transformer_layers_per_block` (1, 2, 10): BasicTransformerBlocks stacked in each Transformer2DModel
+    (up blocks take the values reversed, the mid block the last one): 70 blocks, 630 default LoRA sites;
+  * the "text_time" additional embedding: time_ids [B, 6] -> add_time_proj (sinusoidal, 256 per id)
+    -> [B, 1536], concatenated after the pooled text embedding `text_embeds` [B, 1280] -> add_embedding
+    (a TimestepEmbedding 2816 -> 1280) -> added to the timestep embedding;
+  * BasicTransformerBlock registers attn1 -> attn2 -> ff (norm1, attn1, norm2, attn2, norm3, ff), the
+    registration order of diffusers >= 0.19, the first release with SDXL. It fixes the `unet:{i}` indices of
+    saved files. No SDXL LoRA file of the reference exists to check it against: this is an assumption about
+    the diffusers release an SDXL user runs, not a fixture-pinned fact as the SD order is.
+The SDXL VAE has the architecture of host/vae.py; only the latent scaling differs (0.13025, set through
+StepConfig.vae_scaling).
 """
 import math
 from dataclasses import dataclass, field
@@ -49,6 +65,17 @@ class UNetConfig:
     down_has_attn: Tuple[bool, ...] = (True, True, True, False)
     # Transformer2DModel proj_in / proj_out as nn.Linear on NHWC tokens (SD2.x) instead of 1x1 convs
     use_linear_projection: bool = False
+    # BasicTransformerBlocks per Transformer2DModel: one int, or one per down block (SDXL: (1, 2, 10)) --
+    # up blocks take the tuple reversed, the mid block its last entry
+    transformer_layers_per_block: Union[int, Tuple[int, ...]] = 1
+    # None, or "text_time" (SDXL): an add_embedding of [text_embeds, sinusoidal(time_ids)] added to the
+    # timestep embedding; forward() then needs added_cond_kwargs={"text_embeds", "time_ids"}
+    addition_embed_type: Optional[str] = None
+    addition_time_embed_dim: int = 256
+    projection_class_embeddings_input_dim: int = 2816
+    # registration order inside BasicTransformerBlock, which fixes the LoRA site order: "attn1_ff_attn2"
+    # (diffusers 0.11, the reference's fixture files) or "attn1_attn2_ff" (diffusers >= 0.19, SDXL)
+    transformer_block_order: str = "attn1_ff_attn2"
 
     @staticmethod
     def sd15() -> "UNetConfig":
@@ -68,6 +95,29 @@ class UNetConfig:
                           cross_attention_dim=64, norm_num_groups=8,
                           down_has_attn=(True, True, False), layers_per_block=1,
                           use_linear_projection=True)
+
+    @staticmethod
+    def sdxl() -> "UNetConfig":
+        """stable-diffusion-xl-base-1.0 (1024 px, 128x128 latents)."""
+        return UNetConfig(block_out_channels=(320, 640, 1280), attention_head_dim=(5, 10, 20),
+                          cross_attention_dim=2048, down_has_attn=(False, True, True),
+                          use_linear_projection=True, transformer_layers_per_block=(1, 2, 10),
+                          addition_embed_type="text_time", addition_time_embed_dim=256,
+                          projection_class_embeddings_input_dim=2816,
+                          transformer_block_order="attn1_attn2_ff")
+
+    @staticmethod
+    def sdxl_tiny() -> "UNetConfig":
+        """SDXL features at toy widths (CPU tests): stacked transformer blocks, the text_time embedding
+        (pooled width 40 + 6 x 8), the SDXL block order, and a cross-attention width of 88 -- host/clip.py's
+        tiny encoders (48 + 40 wide) concatenated -- unlike the UNet's and either encoder's."""
+        return UNetConfig(block_out_channels=(32, 64, 64), attention_head_dim=(2, 4, 4),
+                          cross_attention_dim=88, norm_num_groups=8,
+                          down_has_attn=(False, True, True), layers_per_block=1,
+                          use_linear_projection=True, transformer_layers_per_block=(1, 2, 3),
+                          addition_embed_type="text_time", addition_time_embed_dim=8,
+                          projection_class_embeddings_input_dim=40 + 6 * 8,
+                          transformer_block_order="attn1_attn2_ff")
 
     @staticmethod
     def tiny() -> "UNetConfig":
@@ -125,15 +175,29 @@ class FeedForward(nn.Module):
         return x
 
 
+BLOCK_ORDERS = ("attn1_ff_attn2", "attn1_attn2_ff")
+
+
 class BasicTransformerBlock(nn.Module):
-    def __init__(self, dim: int, heads: int, dim_head: int, cross_attention_dim: int):
+    def __init__(self, dim: int, heads: int, dim_head: int, cross_attention_dim: int,
+                 order: str = "attn1_ff_attn2"):
         super().__init__()
-        self.attn1 = CrossAttention(dim, None, heads, dim_head)
-        self.ff = FeedForward(dim)
-        self.attn2 = CrossAttention(dim, cross_attention_dim, heads, dim_head)
-        self.norm1 = nn.LayerNorm(dim)
-        self.norm2 = nn.LayerNorm(dim)
-        self.norm3 = nn.LayerNorm(dim)
+        if order == "attn1_ff_attn2":        # diffusers 0.11
+            self.attn1 = CrossAttention(dim, None, heads, dim_head)
+            self.ff = FeedForward(dim)
+            self.attn2 = CrossAttention(dim, cross_attention_dim, heads, dim_head)
+            self.norm1 = nn.LayerNorm(dim)
+            self.norm2 = nn.LayerNorm(dim)
+            self.norm3 = nn.LayerNorm(dim)
+        elif order == "attn1_attn2_ff":      # diffusers >= 0.19
+            self.norm1 = nn.LayerNorm(dim)
+            self.attn1 = CrossAttention(dim, None, heads, dim_head)
+            self.norm2 = nn.LayerNorm(dim)
+            self.attn2 = CrossAttention(dim, cross_attention_dim, heads, dim_head)
+            self.norm3 = nn.LayerNorm(dim)
+            self.ff = FeedForward(dim)
+        else:
+            raise ValueError(f"transformer_block_order {order!r}: one of {BLOCK_ORDERS}")
 
     def forward(self, x, context):
         x = self.attn1(self.norm1(x)) + x
@@ -143,14 +207,16 @@ class BasicTransformerBlock(nn.Module):
 
 
 class Transformer2DModel(nn.Module):
-    def __init__(self, channels: int, heads: int, cross_attention_dim: int, groups: int, linear: bool = False):
+    def __init__(self, channels: int, heads: int, cross_attention_dim: int, groups: int, linear: bool = False,
+                 depth: int = 1, order: str = "attn1_ff_attn2"):
         super().__init__()
         self.linear = linear
         proj = (lambda: nn.Linear(channels, channels)) if linear else (lambda: nn.Conv2d(channels, channels, 1))
         self.norm = nn.GroupNorm(groups, channels, eps=1e-6)
         self.proj_in = proj()
         self.transformer_blocks = nn.ModuleList(
-            [BasicTransformerBlock(channels, heads, channels // heads, cross_attention_dim)])
+            [BasicTransformerBlock(channels, heads, channels // heads, cross_attention_dim, order)
+             for _ in range(depth)])
         self.proj_out = proj()
 
     def forward(self, x, context):
@@ -230,11 +296,12 @@ class Upsample2D(nn.Module):
 class DownBlock(nn.Module):
     """CrossAttnDownBlock2D / DownBlock2D."""
 
-    def __init__(self, cin, cout, temb, layers, has_attn, heads, ctx_dim, groups, add_down, linear=False):
+    def __init__(self, cin, cout, temb, layers, has_attn, heads, ctx_dim, groups, add_down, linear=False,
+                 depth=1, order="attn1_ff_attn2"):
         super().__init__()
         if has_attn:
             self.attentions = nn.ModuleList(
-                [Transformer2DModel(cout, heads, ctx_dim, groups, linear) for _ in range(layers)])
+                [Transformer2DModel(cout, heads, ctx_dim, groups, linear, depth, order) for _ in range(layers)])
         self.resnets = nn.ModuleList(
             [ResnetBlock2D(cin if i == 0 else cout, cout, temb, groups) for i in range(layers)])
         self.downsamplers = nn.ModuleList([Downsample2D(cout)]) if add_down else None
@@ -257,11 +324,12 @@ class DownBlock(nn.Module):
 class UpBlock(nn.Module):
     """CrossAttnUpBlock2D / UpBlock2D."""
 
-    def __init__(self, cin, cout, cprev, temb, layers, has_attn, heads, ctx_dim, groups, add_up, linear=False):
+    def __init__(self, cin, cout, cprev, temb, layers, has_attn, heads, ctx_dim, groups, add_up, linear=False,
+                 depth=1, order="attn1_ff_attn2"):
         super().__init__()
         if has_attn:
             self.attentions = nn.ModuleList(
-                [Transformer2DModel(cout, heads, ctx_dim, groups, linear) for _ in range(layers)])
+                [Transformer2DModel(cout, heads, ctx_dim, groups, linear, depth, order) for _ in range(layers)])
         resnets = []
         for i in range(layers):
             skip = cin if i == layers - 1 else cout
@@ -286,9 +354,9 @@ class UpBlock(nn.Module):
 class MidBlock(nn.Module):
     """UNetMidBlock2DCrossAttn: resnet, attention, resnet."""
 
-    def __init__(self, ch, temb, heads, ctx_dim, groups, linear=False):
+    def __init__(self, ch, temb, heads, ctx_dim, groups, linear=False, depth=1, order="attn1_ff_attn2"):
         super().__init__()
-        self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, ctx_dim, groups, linear)])
+        self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, ctx_dim, groups, linear, depth, order)])
         self.resnets = nn.ModuleList([ResnetBlock2D(ch, ch, temb, groups) for _ in range(2)])
         self.gradient_checkpointing = False
 
@@ -309,7 +377,7 @@ class TimestepEmbedding(nn.Module):
 
 
 def sinusoidal_embedding(timesteps: torch.Tensor, dim: int) -> torch.Tensor:
-    """flip_sin_to_cos = True, freq_shift = 0 (SD1.5)."""
+    """flip_sin_to_cos = True, freq_shift = 0 (SD1.5's time_proj and SDXL's add_time_proj)."""
     half = dim // 2
     freqs = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32, device=timesteps.device) / half)
     args = timesteps.float()[:, None] * freqs[None, :]
@@ -335,9 +403,20 @@ class UNet2DConditionModel(nn.Module):
             heads = (heads,) * len(ch)
         if len(heads) != len(ch):
             raise ValueError(f"attention_head_dim {heads}: one head count per block {ch}")
+        depth = cfg.transformer_layers_per_block
+        if isinstance(depth, int):
+            depth = (depth,) * len(ch)
+        if len(depth) != len(ch):
+            raise ValueError(f"transformer_layers_per_block {depth}: one value per block {ch}")
+        if cfg.addition_embed_type not in (None, "text_time"):
+            raise ValueError(f"addition_embed_type {cfg.addition_embed_type!r}: None or 'text_time'")
+        order = cfg.transformer_block_order
         lin = cfg.use_linear_projection
         self.conv_in = nn.Conv2d(cfg.in_channels, ch[0], 3, padding=1)
         self.time_embedding = TimestepEmbedding(ch[0], temb)
+        if cfg.addition_embed_type == "text_time":
+            # add_time_proj (sinusoidal, no parameters) is a function call in forward()
+            self.add_embedding = TimestepEmbedding(cfg.projection_class_embeddings_input_dim, temb)
         self.down_blocks = nn.ModuleList()
         self.mid_block = None            # plain attribute for now; registered after up_blocks
         self.up_blocks = nn.ModuleList()
@@ -347,10 +426,11 @@ class UNet2DConditionModel(nn.Module):
             last = i == len(ch) - 1
             self.down_blocks.append(DownBlock(cin, cout, temb, cfg.layers_per_block,
                                               cfg.down_has_attn[i], heads[i], cfg.cross_attention_dim,
-                                              g, add_down=not last, linear=lin))
+                                              g, add_down=not last, linear=lin, depth=depth[i], order=order))
         rev = list(reversed(ch))
         rev_attn = list(reversed(cfg.down_has_attn))
         rev_heads = list(reversed(heads))
+        rev_depth = list(reversed(depth))
         cout = rev[0]
         for i, c in enumerate(rev):
             cprev, cout = cout, c
@@ -358,8 +438,9 @@ class UNet2DConditionModel(nn.Module):
             last = i == len(ch) - 1
             self.up_blocks.append(UpBlock(cin, cout, cprev, temb, cfg.layers_per_block + 1,
                                           rev_attn[i], rev_heads[i], cfg.cross_attention_dim, g,
-                                          add_up=not last, linear=lin))
-        self.mid_block = MidBlock(ch[-1], temb, heads[-1], cfg.cross_attention_dim, g, linear=lin)
+                                          add_up=not last, linear=lin, depth=rev_depth[i], order=order))
+        self.mid_block = MidBlock(ch[-1], temb, heads[-1], cfg.cross_attention_dim, g, linear=lin,
+                                  depth=depth[-1], order=order)
         self.conv_norm_out = nn.GroupNorm(g, ch[0], eps=1e-5)
         self.conv_out = nn.Conv2d(ch[0], cfg.out_channels, 3, padding=1)
 
@@ -391,7 +472,7 @@ class UNet2DConditionModel(nn.Module):
     def dtype(self):
         return self.conv_in.weight.dtype
 
-    def forward(self, sample, timesteps, encoder_hidden_states):
+    def forward(self, sample, timesteps, encoder_hidden_states, added_cond_kwargs=None):
         if not torch.is_tensor(timesteps):
             timesteps = torch.tensor([timesteps], device=sample.device)
         if timesteps.dim() == 0:
@@ -399,6 +480,8 @@ class UNet2DConditionModel(nn.Module):
         timesteps = timesteps.expand(sample.shape[0])
         t_emb = sinusoidal_embedding(timesteps, self.cfg.block_out_channels[0]).to(sample.dtype)
         temb = self.time_embedding(t_emb)
+        if self.cfg.addition_embed_type == "text_time":
+            temb = temb + self.text_time_embedding(added_cond_kwargs, temb.dtype)
         ctx = encoder_hidden_states
         x = self.conv_in(sample)
         skips = [x]
@@ -410,3 +493,15 @@ class UNet2DConditionModel(nn.Module):
             x = blk(x, skips, temb, ctx)
         x = self.conv_out(F.silu(self.conv_norm_out(x)))
         return UNetOutput(x)
+
+    def text_time_embedding(self, added_cond_kwargs, dtype: torch.dtype) -> torch.Tensor:
+        """diffusers' "text_time" branch: add_embedding(cat([text_embeds, add_time_proj(time_ids)], -1)), the
+        concatenation cast to the timestep embedding's dtype first."""
+        if not added_cond_kwargs or "text_embeds" not in added_cond_kwargs or "time_ids" not in added_cond_kwargs:
+            raise ValueError("addition_embed_type 'text_time' needs added_cond_kwargs with 'text_embeds' and "
+                             "'time_ids'")
+        text_embeds, time_ids = added_cond_kwargs["text_embeds"], added_cond_kwargs["time_ids"]
+        time_embeds = sinusoidal_embedding(time_ids.flatten(), self.cfg.addition_time_embed_dim)
+        time_embeds = time_embeds.reshape((text_embeds.shape[0], -1))
+        add_embeds = torch.cat([text_embeds, time_embeds], dim=-1)
+        return self.add_embedding(add_embeds.to(dtype))

@@ -11,6 +11,7 @@ are one cooperative launch that also takes in the DDP all-reduce (peer reads ove
 NCCL call before it without peer access), and steady-state steps are CUDA-graph replays (no
 Python, no launch gaps, no host sync).
 """
+import contextlib
 from dataclasses import dataclass
 from typing import Optional
 
@@ -112,6 +113,7 @@ class StepConfig:
     # step_ops.LatentCache, which freezes one sample per image. With train_inpainting the masked image is
     # encoded too and the image-resolution mask (`self.pixel_mask`) is resized to the latent grid.
     encode_images: bool = False
+    # the VAE's latent scaling: 0.18215 for SD 1.x / 2.x, 0.13025 for SDXL (same VAE architecture)
     vae_scaling: float = 0.18215
     # the posterior noise's dtype: False draws it in the VAE's dtype (current diffusers' randn_tensor),
     # True in fp32 (diffusers releases of the reference's era; std * eps then promotes to fp32)
@@ -131,14 +133,16 @@ def _check_encode_images(cfg: StepConfig, vae):
         raise ValueError(f"StepConfig.pixel_dtype must be torch.uint8 or torch.float32, got {cfg.pixel_dtype}")
 
 
-def _enable_gradient_checkpointing(unet: nn.Module, text_encoder: nn.Module, text_grad: bool):
+def _enable_gradient_checkpointing(unet: nn.Module, text_encoder: nn.Module, text_grad: bool, *more_encoders):
     """train_lora_dreambooth.py:627-630. The step draws nothing from torch's generator inside a
     checkpointed segment (LoRA dropout seeds come from dropout_path's pool), and the generator state
-    cannot be read while a CUDA graph is captured: CLIP's layers skip stashing it."""
+    cannot be read while a CUDA graph is captured: CLIP's layers skip stashing it. SDXL's second text
+    encoder comes in `more_encoders` and is checkpointed like the first."""
     unet.enable_gradient_checkpointing()
     if text_grad:
-        text_encoder.gradient_checkpointing_enable(
-            gradient_checkpointing_kwargs={"use_reentrant": False, "preserve_rng_state": False})
+        for te in (text_encoder,) + more_encoders:
+            te.gradient_checkpointing_enable(
+                gradient_checkpointing_kwargs={"use_reentrant": False, "preserve_rng_state": False})
 
 
 PREDICTION_TYPES = ("epsilon", "v_prediction")
@@ -196,11 +200,9 @@ class LoraTrainStep:
         self.unet, self.text_encoder = unet, text_encoder
         self.device = torch.device(device or "cuda")
         from .grouping import link_sites
-        link_sites(unet, text_encoder)       # a copied / unpickled model has lost its back-references
-        groups = [(unet, cfg.learning_rate)]
-        if cfg.train_text_encoder:
-            groups.append((text_encoder, cfg.learning_rate_text))
-        self.arena = LoraArena(groups, compute_dtype=cfg.compute_dtype, device=self.device,
+        encoders = self._text_encoders()
+        link_sites(unet, *encoders)          # a copied / unpickled model has lost its back-references
+        self.arena = LoraArena(self._arena_groups(), compute_dtype=cfg.compute_dtype, device=self.device,
                                rows=self._arena_rows)
         if cfg.grad_scaler:
             self.arena.enable_loss_scaling(cfg.init_scale, cfg.growth_factor, cfg.backoff_factor, cfg.growth_interval)
@@ -244,9 +246,23 @@ class LoraTrainStep:
                 self.peer_allreduce = False
                 self.arena._dp = None
         self.unet.train()
-        self.text_encoder.train()
+        for te in encoders:
+            te.train()
         if cfg.gradient_checkpointing:
-            _enable_gradient_checkpointing(unet, text_encoder, cfg.train_text_encoder or self._text_encoder_grad)
+            _enable_gradient_checkpointing(unet, text_encoder, cfg.train_text_encoder or self._text_encoder_grad,
+                                           *encoders[1:])
+
+    def _text_encoders(self):
+        """The step's text encoders, in arena-group order."""
+        return (self.text_encoder,)
+
+    def _arena_groups(self):
+        """(model or site list, lr) per optimizer param-group: the UNet, then each text encoder when trained."""
+        cfg = self.cfg
+        groups = [(self.unet, cfg.learning_rate)]
+        if cfg.train_text_encoder:
+            groups += [(te, cfg.learning_rate_text) for te in self._text_encoders()]
+        return groups
 
     def _init_image_inputs(self, vae, latent_shape):
         """Static inputs of a StepConfig.encode_images step (graph-stable addresses): the images at 8x the
@@ -323,7 +339,7 @@ class LoraTrainStep:
         if lat.is_cuda and getattr(self, "_has_dropout", None) is None:
             self._has_dropout = any(
                 type(m).__name__ in ("LoraInjectedLinear", "LoraInjectedConv2d") and m.dropout.p > 0.0
-                for mod in (self.unet, self.text_encoder) for m in mod.modules())
+                for mod in (self.unet,) + self._text_encoders() for m in mod.modules())
         if lat.is_cuda and self._has_dropout:
             dropout_path.begin_step(lat.device)      # one RNG launch for all dropout sites of the step
         fused = cfg.fused_glue and lat.is_cuda
@@ -362,14 +378,7 @@ class LoraTrainStep:
         ac = (torch.autocast("cuda", dtype=cfg.autocast_dtype) if cfg.autocast_dtype is not None
               else torch.autocast("cuda", enabled=False))
         with ac:
-            if cfg.train_text_encoder or self._text_encoder_grad:
-                ehs = self.text_encoder(self.input_ids)[0]
-            else:
-                with torch.no_grad():
-                    ehs = self.text_encoder(self.input_ids)[0]
-            if not fused:
-                noisy = noisy.to(self.model_dtype).contiguous(memory_format=torch.channels_last)
-            pred = self.unet(noisy, timesteps, ehs.to(self.model_dtype)).sample
+            pred = self._predict(noisy, timesteps)
         m = None
         if cfg.use_mask:
             m = (self.mask.float() + 0.01).pow(cfg.mask_temperature)
@@ -409,6 +418,24 @@ class LoraTrainStep:
             ops.wgrad_defer_cancel()
         dropout_path.end_step()
         self.loss.copy_(loss.detach())
+
+    def _text_grad(self):
+        """The text encoders run with gradients, or under no_grad when nothing of theirs is trained."""
+        if self.cfg.train_text_encoder or self._text_encoder_grad:
+            return contextlib.nullcontext()
+        return torch.no_grad()
+
+    def _unet_input(self, noisy):
+        """The fused prologue already wrote the model's dtype in channels_last; the torch path casts here."""
+        if self.cfg.fused_glue and noisy.is_cuda:
+            return noisy
+        return noisy.to(self.model_dtype).contiguous(memory_format=torch.channels_last)
+
+    def _predict(self, noisy, timesteps):
+        """Conditioning and the UNet, under the step's autocast: text encoder -> UNet -> prediction."""
+        with self._text_grad():
+            ehs = self.text_encoder(self.input_ids)[0]
+        return self.unet(self._unet_input(noisy), timesteps, ehs.to(self.model_dtype)).sample
 
     def set_loss_mask(self, mask_image_res: torch.Tensor):
         """`batch["mask"]` of the PTI dataset (image resolution, [B,1,8h,8w] or anything that
@@ -612,6 +639,113 @@ class LoraTrainStep:
 
     def d2h_bytes(self) -> int:
         return 4
+
+
+def _check_xl_models(unet: nn.Module, text_encoder: nn.Module, text_encoder_2: nn.Module):
+    """The SDXL pair of encoders must fit the UNet: refused before any CUDA call."""
+    ucfg = getattr(unet, "cfg", None) or getattr(unet, "config", None)
+    if getattr(ucfg, "addition_embed_type", None) != "text_time":
+        raise ValueError("LoraXLTrainStep needs an SDXL UNet (addition_embed_type='text_time')")
+    c1, c2 = text_encoder.config, text_encoder_2.config
+    if not hasattr(text_encoder_2, "text_projection"):
+        raise ValueError("text_encoder_2 must be a CLIPTextModelWithProjection: its text_embeds are the pooled "
+                         "conditioning")
+    ctx = c1.hidden_size + c2.hidden_size
+    if ctx != ucfg.cross_attention_dim:
+        raise ValueError(f"the text encoders' widths {c1.hidden_size} + {c2.hidden_size} = {ctx} do not match the "
+                         f"UNet's cross_attention_dim {ucfg.cross_attention_dim}")
+    add_in = c2.projection_dim + 6 * ucfg.addition_time_embed_dim
+    if add_in != ucfg.projection_class_embeddings_input_dim:
+        raise ValueError(f"text_encoder_2's projection_dim {c2.projection_dim} + 6 x {ucfg.addition_time_embed_dim} "
+                         f"= {add_in} does not match the UNet's projection_class_embeddings_input_dim "
+                         f"{ucfg.projection_class_embeddings_input_dim}")
+
+
+class LoraXLTrainStep(LoraTrainStep):
+    """The LoRA step on SDXL: two text encoders and the "text_time" conditioning, the conditioning of
+    diffusers' train_dreambooth_lora_sdxl.py (`encode_prompt`, `compute_time_ids`, the UNet call with
+    added_cond_kwargs). Per step:
+
+        h1 = text_encoder(input_ids, output_hidden_states=True).hidden_states[-2]
+        out2 = text_encoder_2(input_ids_2, output_hidden_states=True)
+        encoder_hidden_states = cat([h1, out2.hidden_states[-2]], -1)      # [B, 77, 768 + 1280]
+        unet(noisy, t, encoder_hidden_states,
+             added_cond_kwargs={"text_embeds": out2.text_embeds, "time_ids": time_ids})
+
+    Everything else -- noise, timesteps, the latents or the image encode (StepConfig.vae_scaling = 0.13025
+    for the SDXL VAE), the loss and its options, clip + AdamW -- is LoraTrainStep's. The arena has up to
+    three groups: (unet, learning_rate), then (text_encoder, learning_rate_text) and (text_encoder_2,
+    learning_rate_text) with train_text_encoder; one global clip and one optimizer launch cover all three.
+    The sites of the first encoder's last layer are not trained (see _arena_groups).
+
+    Static inputs besides LoraTrainStep's: `input_ids_2` [B, seq_len] (the second tokenizer's ids) and
+    `time_ids` [B, 6] fp32 (original size, crop top-left, target size), which starts at (8h, 8w, 0, 0, 8h,
+    8w) for every sample -- the Dreambooth script's default -- and keeps what is written into it."""
+
+    def __init__(self, unet: nn.Module, text_encoder: nn.Module, text_encoder_2: nn.Module, cfg: StepConfig,
+                 latent_shape=(1, 4, 128, 128), seq_len: int = 77, device=None, vae: Optional[nn.Module] = None):
+        _check_xl_models(unet, text_encoder, text_encoder_2)
+        self.text_encoder_2 = text_encoder_2
+        super().__init__(unet, text_encoder, cfg, latent_shape=latent_shape, seq_len=seq_len, device=device,
+                         vae=vae)
+        B, _, h, w = latent_shape
+        self.input_ids_2 = torch.zeros((B, seq_len), device=self.device, dtype=torch.long)
+        size = [8.0 * h, 8.0 * w, 0.0, 0.0, 8.0 * h, 8.0 * w]
+        self.time_ids = torch.tensor([size] * B, device=self.device, dtype=torch.float32)
+        self.h_input_ids_2 = torch.zeros((B, seq_len), dtype=torch.long).pin_memory()
+        self.h_time_ids = self.time_ids.cpu().pin_memory()
+
+    def _text_encoders(self):
+        return (self.text_encoder, self.text_encoder_2)
+
+    def _arena_groups(self):
+        """The first encoder's last layer only feeds hidden_states[-1], which the conditioning never reads:
+        its LoRA factors get no gradient, and torch's AdamW leaves a parameter without a gradient as it is
+        (no weight decay either). They stay out of the arena, so they are never updated either."""
+        groups = super()._arena_groups()
+        if self.cfg.train_text_encoder:
+            from .arena import lora_sites
+            dead = {id(m) for m in lora_sites(self.text_encoder.text_model.encoder.layers[-1])}
+            groups[1] = ([m for m in lora_sites(self.text_encoder) if id(m) not in dead], groups[1][1])
+        return groups
+
+    def _predict(self, noisy, timesteps):
+        """diffusers' SDXL encode_prompt: both encoders' penultimate hidden states, concatenated; encoder 2's
+        projected pooled output and the time ids as the UNet's added conditioning."""
+        with self._text_grad():
+            out1 = self.text_encoder(self.input_ids, output_hidden_states=True)
+            out2 = self.text_encoder_2(self.input_ids_2, output_hidden_states=True)
+            ehs = torch.cat([out1.hidden_states[-2], out2.hidden_states[-2]], dim=-1)
+            added = {"text_embeds": out2.text_embeds, "time_ids": self.time_ids}
+        return self.unet(self._unet_input(noisy), timesteps, ehs.to(self.model_dtype), added_cond_kwargs=added).sample
+
+    def _check_xl_inputs(self, input_ids_2: torch.Tensor, time_ids: Optional[torch.Tensor]):
+        if tuple(input_ids_2.shape) != tuple(self.input_ids_2.shape):
+            raise ValueError(f"input_ids_2 of shape {tuple(input_ids_2.shape)}: the step takes "
+                             f"{tuple(self.input_ids_2.shape)}")
+        if input_ids_2.dtype.is_floating_point or input_ids_2.dtype.is_complex:
+            raise ValueError(f"input_ids_2 must be integer token ids, got {input_ids_2.dtype}")
+        if time_ids is not None and tuple(time_ids.shape) != tuple(self.time_ids.shape):
+            raise ValueError(f"time_ids of shape {tuple(time_ids.shape)}: the step takes {tuple(self.time_ids.shape)} "
+                             "(original size, crop top-left, target size per sample)")
+
+    def step_host(self, latents_cpu: torch.Tensor, input_ids_cpu: torch.Tensor, input_ids_2_cpu: torch.Tensor,
+                  time_ids: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """LoraTrainStep.step_host with the second encoder's ids and, optionally, new time ids [B, 6]
+        (None keeps the buffer's current contents)."""
+        self._check_xl_inputs(input_ids_2_cpu, time_ids)
+        if self.cfg.encode_images:
+            self._check_pixels(latents_cpu, mask)
+        self.h_input_ids_2.copy_(input_ids_2_cpu)
+        self.input_ids_2.copy_(self.h_input_ids_2, non_blocking=True)
+        if time_ids is not None:
+            self.h_time_ids.copy_(time_ids)
+            self.time_ids.copy_(self.h_time_ids, non_blocking=True)
+        return super().step_host(latents_cpu, input_ids_cpu, mask)
+
+    def h2d_bytes(self) -> int:
+        """Per step_host call, with new time ids."""
+        return super().h2d_bytes() + self.h_input_ids_2.numel() * 8 + self.h_time_ids.numel() * 4
 
 
 class TextualInversionStep(LoraTrainStep):
