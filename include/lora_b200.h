@@ -544,6 +544,34 @@ int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long stride_b, 
                           unsigned int* counter, int B, int C, int H, int W, const float* grad_scale,
                           void* stream);
 
+/* One step of the sampling loop around one UNet call (diffusers' StableDiffusionPipeline denoising loop
+ * with the scheduler's step folded into coefficients, lora_b200/host/schedulers.py), one launch.
+ * table: fp32 [table_rows, 8] on the device; row 0 = (init_noise_sigma, s_0, t_0, ...), row 1 + i =
+ * (alpha, beta, gamma, s_next, t_next, last, ...) of step i. step_index: a device int32 [1] naming the
+ * step; counter: one zero-initialised uint32 (self-resetting). model_out [G*B, C, H, W] of model_dtype,
+ * element (n, c, pixel) at n*stride_b + c*stride_c + pixel*stride_p; G = 2: rows [0, B) unconditional,
+ * [B, 2B) conditional; guidance: device fp32 [1]. x: fp32 NCHW latents [B, C, H, W], updated in place.
+ * noise: fp32 [table_rows, B, C, H, W]; slice 1 + i is step i's z (not read when gamma = 0).
+ *   m = m_u + g (m_c - m_u)  (G = 1: m = model_out);  x = alpha x + beta m + gamma z
+ *   unet_in [G*B, C, H, W] NHWC of unet_dtype: every half = s_next * x;  *timestep = t_next (fp32)
+ *   last: vae_in [B, C, H, W] (NCHW, or NHWC with vae_channels_last) of vae_dtype = vae_inv_scaling * x
+ *   (vae_inv_scaling = fp32(1 / scaling): the pipeline's `1 / scaling * latents`; it must be > 0)
+ * Every block reads *step_index; the last block to finish advances it, so one captured launch replays
+ * as each step in turn. init != 0: x = noise[0] * init_noise_sigma, unet_in = s_0 * x, *timestep = t_0,
+ * *step_index = 0 (model_out, guidance and vae_in are not read). Allocates nothing; capturable. */
+int lb_sample_step(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                   long long stride_p, int G, float* x, const float* noise, const float* table, int table_rows,
+                   const float* guidance, int* step_index, unsigned int* counter, void* unet_in, int unet_dtype,
+                   float* timestep, void* vae_in, int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B,
+                   int C, int H, int W, int init, void* stream);
+
+/* Image emit, one launch, the mirror of lb_pixels_ingest: image [B,3,H,W] of image_dtype, NCHW or
+ * (channels_last = 1) NHWC -> out uint8 [B,H,W,3] = round_half_even(float((image / 2 + 0.5).clamp(0, 1))
+ * * 255), the division, sum and clamp each rounded to image_dtype: diffusers' post-processing and
+ * numpy_to_pil, bit for bit (NaN -> 0). */
+int lb_pixels_emit(const void* image, int image_dtype, int channels_last, unsigned char* out, int B, int H, int W,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,6 +12,11 @@
 //                         train_lora_dreambooth.py:855-875 and its gradient w.r.t. the prediction,
 //                         in one pass (the loss is a scalar: its backward is known in the forward),
 //                         optionally times the fp16 loss scale (GradScaler.scale(loss).backward())
+// and the two ends of a sampling step (the denoising loop of diffusers' StableDiffusionPipeline):
+//   lb_sample_step        the guidance sum, the scheduler's update as folded coefficients, the next UNet
+//                         input and timestep (+ the decoder input on the last step); or, with init, the
+//                         first UNet input from the initial noise
+//   lb_pixels_emit        the decoded image -> (x / 2 + 0.5).clamp(0, 1) -> uint8 HWC (numpy_to_pil)
 // All are HBM-bound over a few hundred KB (a few MB of pixels): what they buy is launch count (about
 // ten small torch kernels per step and their intermediates), not bandwidth.
 #include <cuda_bf16.h>
@@ -225,6 +230,104 @@ masked_mse_kernel(const void* __restrict__ pred, int pred_dt, long long sb, long
   }
 }
 
+// One sampling step, element (b, c, p) of the latents [B, C, P] (fp32 NCHW), step row k = 1 + *step_index
+// of the [rows, 8] table: (alpha, beta, gamma, s_next, t_next, last, -, -):
+//   m_hat = m_u + g (m_c - m_u)      (G = 2: m_u row b, m_c row B + b of the UNet output; G = 1: m_hat = m)
+//   x'    = alpha x + beta m_hat + gamma z      (z: noise slice k of [rows, B, C, P]; unread when gamma = 0)
+//   unet_in[g B + b, c, p] = (s_next x') in the UNet's dtype, NHWC, for each of the G halves
+//   last row: vae_in[b, c, p] = (1 / scaling) x' in the VAE's dtype (NCHW or NHWC), the pipeline's
+//   `1 / scaling * latents` with the reciprocal rounded to fp32 as torch rounds a scalar factor
+// init: x = z_0 * init_noise_sigma (row 0: (sigma, s_0, t_0)), the first UNet input and timestep, and the
+// step index and arrival counter reset. Every block reads *step_index; the last block to arrive
+// advances it, so one captured launch replays as every step in turn.
+__global__ void __launch_bounds__(256)
+sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long sc, long long sp, int G,
+                   float* __restrict__ x, const float* __restrict__ noise, const float* __restrict__ table,
+                   int rows, const float* __restrict__ guidance, int* __restrict__ step_index,
+                   unsigned int* __restrict__ counter, void* __restrict__ unet_in, int udt,
+                   float* __restrict__ timestep, void* __restrict__ vae_in, int vdt, int vae_cl, float vae_inv_scaling,
+                   int B, int C, int P, int init) {
+  __shared__ int s_row;
+  __shared__ bool last_block;
+  if (threadIdx.x == 0) {
+    int k = init ? 0 : 1 + *step_index;
+    s_row = k < 0 ? 0 : (k >= rows ? rows - 1 : k);
+  }
+  __syncthreads();
+  const float* row = table + 8ll * s_row;
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  const long long slice = static_cast<long long>(B) * C * P;
+  if (i < static_cast<long long>(B) * P) {
+    const int b = static_cast<int>(i / P), px = static_cast<int>(i % P);
+    float s_next, alpha = 0.f, beta = 0.f, gamma = 0.f, g = 0.f;
+    bool last = false;
+    if (init) {
+      s_next = row[1];
+    } else {
+      alpha = row[0]; beta = row[1]; gamma = row[2]; s_next = row[3]; last = row[5] != 0.f;
+      g = *guidance;
+    }
+    const float* z = noise + (init ? 0ll : s_row * slice);
+    for (int c = 0; c < C; ++c) {
+      const long long xi = (static_cast<long long>(b) * C + c) * P + px;
+      float xn;
+      if (init) {
+        xn = __fmul_rn(z[xi], row[0]);
+      } else {
+        float m = ld_any(mo, b * sb + c * sc + px * sp, mdt);
+        if (G == 2) {
+          const float mc = ld_any(mo, (B + b) * sb + c * sc + px * sp, mdt);
+          m = fmaf(g, mc - m, m);
+        }
+        xn = fmaf(alpha, x[xi], beta * m);
+        if (gamma != 0.f) xn = fmaf(gamma, z[xi], xn);
+      }
+      x[xi] = xn;
+      const float u = __fmul_rn(s_next, xn);
+      for (int h = 0; h < G; ++h) st_any(unet_in, (static_cast<long long>(h * B + b) * P + px) * C + c, udt, u);
+      if (last) st_any(vae_in, vae_cl ? i * C + c : xi, vdt, __fmul_rn(vae_inv_scaling, xn));
+    }
+  }
+  if (init) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+      *timestep = row[2];
+      *step_index = 0;
+      *counter = 0u;
+    }
+    return;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) *timestep = row[4];
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last_block = atomicAdd(counter, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (last_block && threadIdx.x == 0) {
+    *step_index += 1;
+    *counter = 0u;
+    __threadfence();
+  }
+}
+
+// diffusers' image post-processing, op by op: (image / 2 + 0.5).clamp(0, 1), each op rounded in the
+// image's dtype; then .float() * 255, round half to even, cast to uint8 (numpy_to_pil). in: [B, 3, P]
+// NCHW or NHWC; out: uint8 [B, P, 3].
+__global__ void __launch_bounds__(256)
+pixels_emit_kernel(const void* __restrict__ img, int dt, int channels_last, unsigned char* __restrict__ out, int B,
+                   long long P) {
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (i >= B * P) return;
+  const long long b = i / P, p = i % P;
+  for (int c = 0; c < 3; ++c) {
+    const float v = ld_any(img, channels_last ? i * 3 + c : (b * 3 + c) * P + p, dt);
+    float y = round_to(dt, __fadd_rn(round_to(dt, __fdiv_rn(v, 2.f)), 0.5f));
+    y = y < 0.f ? 0.f : (y > 1.f ? 1.f : y);       // NaN stays NaN
+    const float q = rintf(__fmul_rn(y, 255.f));
+    out[i * 3 + c] = q == q ? static_cast<unsigned char>(q) : 0;
+  }
+}
+
 }  // namespace lbglue
 
 using namespace lbglue;
@@ -314,5 +417,37 @@ extern "C" int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long
   masked_mse_kernel<<<static_cast<int>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       pred, pred_dtype, stride_b, stride_c, stride_p, target, mask, weights, grad, loss, partials64, counter, B, C,
       H * W, grad_scale);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_sample_step(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                              long long stride_p, int G, float* x, const float* noise, const float* table,
+                              int table_rows, const float* guidance, int* step_index, unsigned int* counter,
+                              void* unet_in, int unet_dtype, float* timestep, void* vae_in, int vae_dtype,
+                              int vae_channels_last, float vae_inv_scaling, int B, int C, int H, int W, int init,
+                              void* stream) {
+  if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || (G != 1 && G != 2) || table_rows < 2) return LB_ERR_SHAPE;
+  if (!float_dtype(unet_dtype) || !float_dtype(vae_dtype) || (!init && !float_dtype(model_dtype)))
+    return LB_ERR_DTYPE;
+  if (x == nullptr || noise == nullptr || table == nullptr || step_index == nullptr || counter == nullptr ||
+      unet_in == nullptr || timestep == nullptr)
+    return LB_ERR_SHAPE;
+  if (!init && (model_out == nullptr || guidance == nullptr || vae_in == nullptr || !(vae_inv_scaling > 0.f)))
+    return LB_ERR_SHAPE;
+  const long long n = static_cast<long long>(B) * H * W;
+  sample_step_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows, guidance, step_index,
+      counter, unet_in, unet_dtype, timestep, vae_in, vae_dtype, vae_channels_last != 0, vae_inv_scaling, B, C, H * W,
+      init != 0);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_pixels_emit(const void* image, int image_dtype, int channels_last, unsigned char* out, int B,
+                              int H, int W, void* stream) {
+  if (B <= 0 || H <= 0 || W <= 0 || image == nullptr || out == nullptr) return LB_ERR_SHAPE;
+  if (!float_dtype(image_dtype)) return LB_ERR_DTYPE;
+  const long long P = static_cast<long long>(H) * W, n = B * P;
+  pixels_emit_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      image, image_dtype, channels_last != 0, out, B, P);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }

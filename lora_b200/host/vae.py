@@ -1,5 +1,5 @@
-"""SD 1.x / 2.x VAE encoder *host model* (plain PyTorch; stands in for the encoder half of diffusers'
-AutoencoderKL).
+"""SD 1.x / 2.x VAE *host model* (plain PyTorch; stands in for diffusers' AutoencoderKL): the encoder
+half always, the decoder half on request.
 
 diffusers is not installed here, so the frozen encoder the reference's trainers call every step
 (`vae.encode(pixel_values).latent_dist.sample()`, train_lora_dreambooth.py:818-821,
@@ -18,6 +18,13 @@ checkpoint; state dicts with the later names (`to_q`, `to_k`, `to_v`, `to_out.0`
 `encode(x).latent_dist` is a DiagonalGaussianDistribution with diffusers' attributes, so a diffusers
 AutoencoderKL and this encoder fill the same slot of the step engine (which reads only
 `.latent_dist.parameters`).
+
+`AutoencoderKL(cfg, with_decoder=True)` adds diffusers' `post_quant_conv` (1x1) and `Decoder`: conv_in
+from the latents to the widest channel count, the mid block, four UpDecoderBlock2D (the encoder's
+widths reversed, three ResnetBlock2D each, nearest x2 upsampling + 3x3 conv after all but the last),
+GroupNorm + SiLU + conv_out to 3 channels. `decode(z).sample` is the image in [-1, 1] (before
+clamping). The decoder is built after the encoder and quant_conv, so those draw the same random
+numbers, and have the same keys, with or without it.
 """
 from dataclasses import dataclass
 from typing import Optional, Tuple
@@ -193,17 +200,74 @@ class Encoder(nn.Module):
         return self.conv_out(F.silu(self.conv_norm_out(x)))
 
 
-class AutoencoderKL(nn.Module):
-    """The encoder half of diffusers' AutoencoderKL: `encode(x)` of [B, 3, H, W] images in [-1, 1]
-    gives the posterior over [B, 4, H/8, W/8] latents. Runs in whatever dtype / memory format the
-    module is given (the step engine uses the VAE's dtype and channels_last); no host sync and no
-    data-dependent allocation, so it runs inside a captured CUDA graph."""
+class Upsample2D(nn.Module):
+    def __init__(self, channels: int):
+        super().__init__()
+        self.conv = nn.Conv2d(channels, channels, 3, padding=1)
 
-    def __init__(self, cfg: VAEConfig = VAEConfig()):
+    def forward(self, x):
+        return self.conv(F.interpolate(x, scale_factor=2.0, mode="nearest"))
+
+
+class UpDecoderBlock2D(nn.Module):
+    def __init__(self, cin: int, cout: int, layers: int, groups: int, add_up: bool):
+        super().__init__()
+        self.resnets = nn.ModuleList([ResnetBlock2D(cin if i == 0 else cout, cout, groups) for i in range(layers)])
+        self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_up else None
+
+    def forward(self, x):
+        for res in self.resnets:
+            x = res(x)
+        if self.upsamplers is not None:
+            x = self.upsamplers[0](x)
+        return x
+
+
+class Decoder(nn.Module):
+    def __init__(self, cfg: VAEConfig):
+        super().__init__()
+        ch, g = tuple(reversed(cfg.block_out_channels)), cfg.norm_num_groups
+        self.conv_in = nn.Conv2d(cfg.latent_channels, ch[0], 3, padding=1)
+        self.mid_block = UNetMidBlock2D(ch[0], g)
+        self.up_blocks = nn.ModuleList()
+        cout = ch[0]
+        for i, c in enumerate(ch):
+            cin, cout = cout, c
+            self.up_blocks.append(UpDecoderBlock2D(cin, cout, cfg.layers_per_block + 1, g,
+                                                   add_up=i < len(ch) - 1))
+        self.conv_norm_out = nn.GroupNorm(g, ch[-1], eps=1e-6)
+        self.conv_out = nn.Conv2d(ch[-1], cfg.in_channels, 3, padding=1)
+
+    def forward(self, z):
+        x = self.mid_block(self.conv_in(z))
+        for blk in self.up_blocks:
+            x = blk(x)
+        return self.conv_out(F.silu(self.conv_norm_out(x)))
+
+
+class DecoderOutput:
+    __slots__ = ("sample",)
+
+    def __init__(self, sample):
+        self.sample = sample
+
+
+class AutoencoderKL(nn.Module):
+    """diffusers' AutoencoderKL: `encode(x)` of [B, 3, H, W] images in [-1, 1] gives the posterior over
+    [B, 4, H/8, W/8] latents; with `with_decoder=True`, `decode(z).sample` maps latents back to images.
+    Runs in whatever dtype / memory format the module is given (the step engine uses the VAE's dtype
+    and channels_last); no host sync and no data-dependent allocation, so it runs inside a captured
+    CUDA graph."""
+
+    def __init__(self, cfg: VAEConfig = VAEConfig(), with_decoder: bool = False):
         super().__init__()
         self.cfg = cfg
         self.encoder = Encoder(cfg)
         self.quant_conv = nn.Conv2d(2 * cfg.latent_channels, 2 * cfg.latent_channels, 1)
+        self.has_decoder = with_decoder
+        if with_decoder:
+            self.decoder = Decoder(cfg)
+            self.post_quant_conv = nn.Conv2d(cfg.latent_channels, cfg.latent_channels, 1)
 
     @property
     def dtype(self):
@@ -215,3 +279,8 @@ class AutoencoderKL(nn.Module):
 
     def encode(self, x: torch.Tensor) -> AutoencoderKLOutput:
         return AutoencoderKLOutput(DiagonalGaussianDistribution(self.quant_conv(self.encoder(x))))
+
+    def decode(self, z: torch.Tensor) -> DecoderOutput:
+        if not self.has_decoder:
+            raise ValueError("this AutoencoderKL was built without its decoder: AutoencoderKL(cfg, with_decoder=True)")
+        return DecoderOutput(self.decoder(self.post_quant_conv(z)))

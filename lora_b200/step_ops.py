@@ -11,6 +11,12 @@
   fused_masked_mse  (mask-weighted) MSE and its gradient w.r.t. the prediction in one pass
                     cli_lora_pti.py:340-370, train_lora_dreambooth.py:855-875
 
+and the two ends of a sampling step (lora_b200/sample.py):
+
+  sample_step       guidance sum + the scheduler's update (folded coefficients) + the next UNet input
+                    and timestep (+ the decoder input on the last step); init=True: the first input
+  pixels_emit       decoded image -> (x / 2 + 0.5).clamp(0, 1) -> uint8 HWC, diffusers' post-processing
+
 and the latent cache of cli_lora_pti.py:141-151 (`cached_latents=True`): the VAE runs once per
 image, training steps start from stored latents.
 """
@@ -161,6 +167,88 @@ def step_prologue_posterior(moments: torch.Tensor, posterior_noise: torch.Tensor
         B, C, H, W, stream_ptr()), "lb_step_prologue_posterior")
     ops._count()
     return (out, v) if velocity else out
+
+
+def _dense_hw_strides(t: torch.Tensor, what: str):
+    """(stride_b, stride_c, stride_p) of a [N, C, H, W] tensor dense in (H, W) (NCHW or channels_last)."""
+    sb, sc, sh, sw = t.stride()
+    if sh != t.shape[3] * sw:
+        raise _C.LoraB200Error(f"{what} must be dense in (H, W) (contiguous or channels_last), strides {t.stride()}")
+    return sb, sc, sw
+
+
+def sample_step(model_out: Optional[torch.Tensor], x: torch.Tensor, noise: torch.Tensor, table: torch.Tensor,
+                guidance: Optional[torch.Tensor], step_index: torch.Tensor, counter: torch.Tensor,
+                unet_in: torch.Tensor, timestep: torch.Tensor, vae_in: Optional[torch.Tensor],
+                vae_scaling: float, init: bool = False):
+    """One launch of lb_sample_step, in place on preallocated buffers (nothing is allocated: capturable).
+
+    model_out: the UNet output [G*B, C, H, W] (G = 2: [uncond ; cond]) in any float dtype, dense in (H, W);
+    x: fp32 contiguous latents [B, C, H, W]; noise: fp32 [rows, B, C, H, W] (slice 0 is z_0); table: fp32
+    [rows, 8] (host/schedulers.pack_table); guidance: fp32 [1]; step_index: int32 [1]; counter: int32 [1]
+    zero-initialised; unet_in: [G*B, C, H, W] channels_last in the UNet's dtype; timestep: fp32 [1];
+    vae_in: [B, C, H, W] in the VAE's dtype, contiguous or channels_last, written on the last step as
+    `1 / vae_scaling * x` (the pipeline's expression, the reciprocal rounded to fp32).
+    init=True: x = z_0 * init_noise_sigma and the first UNet input and timestep; the index is reset."""
+    if not x.is_cuda:
+        raise _C.LoraB200Error("sample_step needs CUDA tensors (no CPU path)")
+    if not vae_scaling > 0.0:
+        raise _C.LoraB200Error(f"sample_step: vae_scaling must be positive, got {vae_scaling}")
+    B, C, H, W = x.shape
+    G = unet_in.shape[0] // B
+    if x.dtype != torch.float32 or not x.is_contiguous():
+        raise _C.LoraB200Error("sample_step: x must be a contiguous float32 tensor")
+    if (tuple(unet_in.shape) != (G * B, C, H, W) or unet_in.shape[0] % B
+            or not unet_in.is_contiguous(memory_format=torch.channels_last)):
+        raise _C.LoraB200Error(f"sample_step: unet_in must be a channels_last [G*B, {C}, {H}, {W}] tensor, "
+                               f"got {tuple(unet_in.shape)}")
+    if (table.dtype != torch.float32 or table.dim() != 2 or table.shape[1] != 8 or not table.is_contiguous()
+            or noise.dtype != torch.float32 or tuple(noise.shape) != (table.shape[0], B, C, H, W)
+            or not noise.is_contiguous()):
+        raise _C.LoraB200Error("sample_step: table must be fp32 [rows, 8] and noise fp32 [rows, B, C, H, W]")
+    if step_index.dtype != torch.int32 or counter.dtype != torch.int32 or timestep.dtype != torch.float32:
+        raise _C.LoraB200Error("sample_step: step_index / counter int32 [1], timestep fp32 [1]")
+    sb = sc = sp = 0
+    mdt = vdt = _C.LB_F32
+    vcl = 0
+    if not init:
+        if model_out is None or tuple(model_out.shape) != (G * B, C, H, W):
+            raise _C.LoraB200Error(f"sample_step: model_out must be [{G * B}, {C}, {H}, {W}]")
+        sb, sc, sp = _dense_hw_strides(model_out, "model_out")
+        mdt = dtype_code(model_out.dtype)
+        if vae_in is None or tuple(vae_in.shape) != (B, C, H, W):
+            raise _C.LoraB200Error(f"sample_step: vae_in must be [{B}, {C}, {H}, {W}]")
+        vcl = int(not vae_in.is_contiguous())
+        if vcl and not vae_in.is_contiguous(memory_format=torch.channels_last):
+            raise _C.LoraB200Error("sample_step: vae_in must be contiguous or channels_last")
+        vdt = dtype_code(vae_in.dtype)
+        if guidance is None or guidance.dtype != torch.float32:
+            raise _C.LoraB200Error("sample_step: guidance must be a float32 [1] tensor")
+    check(_C.lib.lb_sample_step(ptr(model_out), mdt, sb, sc, sp, G, ptr(x), ptr(noise), ptr(table), table.shape[0],
+                                ptr(guidance), ptr(step_index), ptr(counter), ptr(unet_in),
+                                dtype_code(unet_in.dtype), ptr(timestep), ptr(vae_in), vdt, vcl, 1.0 / float(vae_scaling),
+                                B, C, H, W, int(init), stream_ptr()), "lb_sample_step")
+    ops._count()
+
+
+def pixels_emit(image: torch.Tensor, out: torch.Tensor):
+    """uint8 [B, H, W, 3] images from the decoder's [B, 3, H, W] output (fp32 / bf16 / fp16, contiguous or
+    channels_last), into `out`: diffusers' `(image / 2 + 0.5).clamp(0, 1)` and numpy_to_pil's
+    `(x.float() * 255).round().astype(uint8)`, bit for bit, one launch."""
+    if not image.is_cuda:
+        raise _C.LoraB200Error("pixels_emit needs CUDA tensors (no CPU path)")
+    if image.dim() != 4 or image.shape[1] != 3:
+        raise _C.LoraB200Error(f"pixels_emit: image must be [B, 3, H, W], got {tuple(image.shape)}")
+    B, _, H, W = image.shape
+    if out.dtype != torch.uint8 or tuple(out.shape) != (B, H, W, 3) or not out.is_contiguous():
+        raise _C.LoraB200Error(f"pixels_emit: out must be a contiguous uint8 [{B}, {H}, {W}, 3] tensor")
+    cl = not image.is_contiguous()
+    if cl and not image.is_contiguous(memory_format=torch.channels_last):
+        raise _C.LoraB200Error("pixels_emit: image must be contiguous or channels_last")
+    check(_C.lib.lb_pixels_emit(ptr(image), dtype_code(image.dtype), int(cl), ptr(out), B, H, W, stream_ptr()),
+          "lb_pixels_emit")
+    ops._count()
+    return out
 
 
 class _MaskedMSE(torch.autograd.Function):
