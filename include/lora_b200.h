@@ -565,6 +565,45 @@ int lb_sample_step(const void* model_out, int model_dtype, long long stride_b, l
                    float* timestep, void* vae_in, int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B,
                    int C, int H, int W, int init, void* stream);
 
+/* lb_sample_step into a UNet input of unet_channels >= C channels: unet_in [G*B, unet_channels, H, W]
+ * NHWC, of which only channels [0, C) are written (the 9-channel inpainting UNet's mask and
+ * masked-image channels, written once by lb_sample_init, are left as they are). lb_sample_step is this
+ * with unet_channels = C. unet_channels < C: LB_ERR_SHAPE. */
+int lb_sample_step_ch(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                      long long stride_p, int G, float* x, const float* noise, const float* table, int table_rows,
+                      const float* guidance, int* step_index, unsigned int* counter, void* unet_in, int unet_dtype,
+                      int unet_channels, float* timestep, void* vae_in, int vae_dtype, int vae_channels_last,
+                      float vae_inv_scaling, int B, int C, int H, int W, int init, void* stream);
+
+/* The start of an img2img or inpainting sampling loop, one launch (diffusers' StableDiffusionImg2Img-
+ * Pipeline.prepare_latents / StableDiffusionInpaintPipeline.prepare_mask_latents). Row 0 of the table is
+ * (c_noise, s_start, t_start, c_lat, ...) (host/schedulers.pack_table); noise slice 0 is z_0.
+ *   moments != NULL, mask == NULL (img2img): lat = (mean + exp(0.5 * clamp(logvar, -30, 20)) * eps) *
+ *     scaling, rounded as lb_step_prologue_posterior rounds it (moments [B,2C,H,W] of moments_dtype at
+ *     b*stride_b + c*stride_c + pixel*stride_p; posterior_noise [B,C,H,W] NCHW of moments_dtype or
+ *     LB_F32); x = fl(fl(c_lat * lat) + fl(c_noise * z_0)), the scheduler's add_noise.
+ *   moments == NULL or mask != NULL: x = z_0 * c_noise (randn * init_noise_sigma).
+ * x is written to x (fp32 NCHW [B,C,H,W]) and s_start * x to channels [0, C) of every half of unet_in
+ * [G*B, unet_channels, H, W] NHWC of unet_dtype. mask (inpainting, uint8 [B, 8H, 8W], 0..255 over 255
+ * as the pipeline reads an L-mode image; needs moments, those of the masked image, and unet_channels =
+ * 2C + 1; otherwise unet_channels = C): channel C of every half = the mask binarised at 0.5 and read at
+ * pixel (8h, 8w) (F.interpolate to the latent grid, nearest); channels C+1 .. 2C = the masked image's
+ * posterior sample. *timestep = t_start, *step_index = 0, *counter = 0. Allocates nothing; capturable. */
+int lb_sample_init(const void* moments, int moments_dtype, long long stride_b, long long stride_c,
+                   long long stride_p, const void* posterior_noise, int posterior_noise_dtype, float scaling,
+                   const unsigned char* mask, const float* noise, const float* table, int table_rows, float* x,
+                   int* step_index, unsigned int* counter, void* unet_in, int unet_dtype, int unet_channels,
+                   float* timestep, int G, int B, int C, int H, int W, void* stream);
+
+/* The inpainting pipeline's masked image, one launch (diffusers' prepare_mask_and_masked_image):
+ * pixels uint8 [B,H,W,3], mask uint8 [B,H,W] (an L-mode image, 0..255): mask = (mask / 255.f >= 0.5),
+ * masked_out [B,3,H,W] of out_dtype, NCHW or (channels_last = 1) NHWC = image * (mask < 0.5) with image
+ * = uint8 / 127.5 - 1, evaluated as lb_pixels_ingest evaluates uint8 pixels (equal bit for bit: the two
+ * normalisations differ by exact powers of two). Unlike lb_pixels_ingest's uint8 mask, the mask is not
+ * read as 0 / 1. */
+int lb_pixels_ingest_inpaint(const void* pixels, const unsigned char* mask, void* masked_out, int out_dtype,
+                             int channels_last, int B, int H, int W, void* stream);
+
 /* Image emit, one launch, the mirror of lb_pixels_ingest: image [B,3,H,W] of image_dtype, NCHW or
  * (channels_last = 1) NHWC -> out uint8 [B,H,W,3] = round_half_even(float((image / 2 + 0.5).clamp(0, 1))
  * * 255), the division, sum and clamp each rounded to image_dtype: diffusers' post-processing and

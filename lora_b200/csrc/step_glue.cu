@@ -16,6 +16,13 @@
 //   lb_sample_step        the guidance sum, the scheduler's update as folded coefficients, the next UNet
 //                         input and timestep (+ the decoder input on the last step); or, with init, the
 //                         first UNet input from the initial noise
+//   lb_sample_step_ch     the same into a UNet input of more channels than the latents (the 9-channel
+//                         inpainting UNet): only the latent channels are written
+//   lb_sample_init        the start of an img2img or inpainting loop: the posterior sample of the encoded
+//                         image, scheduler.add_noise at the first kept timestep, the first UNet input,
+//                         and for inpainting the constant mask and masked-image channels
+//   lb_pixels_ingest_inpaint  uint8 image + uint8 0..255 mask -> the inpainting pipeline's masked image
+//                         (prepare_mask_and_masked_image) in the VAE's dtype and layout
 //   lb_pixels_emit        the decoded image -> (x / 2 + 0.5).clamp(0, 1) -> uint8 HWC (numpy_to_pil)
 // All are HBM-bound over a few hundred KB (a few MB of pixels): what they buy is launch count (about
 // ten small torch kernels per step and their intermediates), not bandwidth.
@@ -90,11 +97,21 @@ __device__ __forceinline__ float normalise_u8(unsigned char v) {
   return __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(v), 255.f), 0.5f), 0.5f);
 }
 
+// diffusers' prepare_mask_and_masked_image on one uint8 L-mode mask value: v / 255 in fp32, then
+// binarised (< 0.5 -> 0, >= 0.5 -> 1). 127 -> 0, 128 -> 1.
+__device__ __forceinline__ float binarise_u8(unsigned char v) {
+  return __fdiv_rn(static_cast<float>(v), 255.f) < 0.5f ? 0.f : 1.f;
+}
+
+enum { MASK_F32 = 0, MASK_U8 = 1, MASK_U8_PIPELINE = 2 };
+
 // out (VAE input, [B, 3, H, W] NCHW or channels_last, out_dt) <- pixels: uint8 [B, H, W, 3] (normalised
-// here) or fp32 [B, 3, H, W] (already normalised: a cast). With mask [B, 1, H, W] (fp32 or uint8):
-// masked = image * (mask < 0.5), the product in fp32, then the same cast (dataset.py:115).
+// here) or fp32 [B, 3, H, W] (already normalised: a cast). With mask [B, 1, H, W]: masked = image *
+// (mask < 0.5), the product in fp32, then the same cast. mask_mode MASK_F32 / MASK_U8: the mask's value
+// as stored (the training dataset's 0 / 1 mask, dataset.py:115); MASK_U8_PIPELINE: a 0..255 mask
+// binarised first (binarise_u8). out may be NULL when only the masked image is wanted.
 __global__ void __launch_bounds__(256)
-pixels_ingest_kernel(const void* __restrict__ pixels, int pixels_u8, const void* __restrict__ mask, int mask_u8,
+pixels_ingest_kernel(const void* __restrict__ pixels, int pixels_u8, const void* __restrict__ mask, int mask_mode,
                      void* __restrict__ out, void* __restrict__ masked, int out_dt, int channels_last, int B,
                      long long P) {
   const long long i = blockIdx.x * 256ll + threadIdx.x;
@@ -102,8 +119,10 @@ pixels_ingest_kernel(const void* __restrict__ pixels, int pixels_u8, const void*
   const long long b = i / P, p = i % P;
   float keep = 0.f;
   if (mask) {
-    const float m = mask_u8 ? static_cast<float>(reinterpret_cast<const unsigned char*>(mask)[i])
-                            : reinterpret_cast<const float*>(mask)[i];
+    const unsigned char* m8 = reinterpret_cast<const unsigned char*>(mask);
+    const float m = mask_mode == MASK_U8_PIPELINE ? binarise_u8(m8[i])
+                    : mask_mode == MASK_U8        ? static_cast<float>(m8[i])
+                                                  : reinterpret_cast<const float*>(mask)[i];
     keep = m < 0.5f ? 1.f : 0.f;          // NaN < 0.5 is false, as in torch
   }
   for (int c = 0; c < 3; ++c) {
@@ -111,7 +130,7 @@ pixels_ingest_kernel(const void* __restrict__ pixels, int pixels_u8, const void*
     const float x = pixels_u8 ? normalise_u8(reinterpret_cast<const unsigned char*>(pixels)[i * 3 + c])
                               : reinterpret_cast<const float*>(pixels)[nchw];
     const long long o = channels_last ? i * 3 + c : nchw;
-    st_any(out, o, out_dt, x);
+    if (out) st_any(out, o, out_dt, x);
     if (mask) st_any(masked, o, out_dt, __fmul_rn(x, keep));   // x * 0 keeps the sign of x, as torch does
   }
 }
@@ -234,7 +253,9 @@ masked_mse_kernel(const void* __restrict__ pred, int pred_dt, long long sb, long
 // of the [rows, 8] table: (alpha, beta, gamma, s_next, t_next, last, -, -):
 //   m_hat = m_u + g (m_c - m_u)      (G = 2: m_u row b, m_c row B + b of the UNet output; G = 1: m_hat = m)
 //   x'    = alpha x + beta m_hat + gamma z      (z: noise slice k of [rows, B, C, P]; unread when gamma = 0)
-//   unet_in[g B + b, c, p] = (s_next x') in the UNet's dtype, NHWC, for each of the G halves
+//   unet_in[g B + b, c, p] = (s_next x') in the UNet's dtype, NHWC with Cu >= C channels (only channels
+//   [0, C) are written: the inpainting UNet's mask and masked-image channels stay as sample_init_kernel
+//   wrote them), for each of the G halves
 //   last row: vae_in[b, c, p] = (1 / scaling) x' in the VAE's dtype (NCHW or NHWC), the pipeline's
 //   `1 / scaling * latents` with the reciprocal rounded to fp32 as torch rounds a scalar factor
 // init: x = z_0 * init_noise_sigma (row 0: (sigma, s_0, t_0)), the first UNet input and timestep, and the
@@ -244,7 +265,7 @@ __global__ void __launch_bounds__(256)
 sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long sc, long long sp, int G,
                    float* __restrict__ x, const float* __restrict__ noise, const float* __restrict__ table,
                    int rows, const float* __restrict__ guidance, int* __restrict__ step_index,
-                   unsigned int* __restrict__ counter, void* __restrict__ unet_in, int udt,
+                   unsigned int* __restrict__ counter, void* __restrict__ unet_in, int udt, int Cu,
                    float* __restrict__ timestep, void* __restrict__ vae_in, int vdt, int vae_cl, float vae_inv_scaling,
                    int B, int C, int P, int init) {
   __shared__ int s_row;
@@ -284,7 +305,7 @@ sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long
       }
       x[xi] = xn;
       const float u = __fmul_rn(s_next, xn);
-      for (int h = 0; h < G; ++h) st_any(unet_in, (static_cast<long long>(h * B + b) * P + px) * C + c, udt, u);
+      for (int h = 0; h < G; ++h) st_any(unet_in, (static_cast<long long>(h * B + b) * P + px) * Cu + c, udt, u);
       if (last) st_any(vae_in, vae_cl ? i * C + c : xi, vdt, __fmul_rn(vae_inv_scaling, xn));
     }
   }
@@ -307,6 +328,65 @@ sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long
     *step_index += 1;
     *counter = 0u;
     __threadfence();
+  }
+}
+
+// The start of an img2img or inpainting sampling loop (StableDiffusionImg2ImgPipeline /
+// StableDiffusionInpaintPipeline), element (b, c, p) of the latents [B, C, P], from row 0 of the table:
+// (c_noise, s_start, t_start, c_lat). With moments and no mask (img2img):
+//   lat = the posterior sample of the image's moments * scaling (posterior_sample)
+//   x   = fl(fl(c_lat lat) + fl(c_noise z_0))       scheduler.add_noise(init_latents, z_0, t_start)
+// Without moments, or with the mask (inpainting): x = z_0 * c_noise (randn * init_noise_sigma).
+// unet_in[g B + b, :, p] (NHWC, Cu channels) = s_start x in channels [0, C) of each of the G halves; with
+// the mask also channel C = the binarised mask at pixel (8h, 8w) of the image-resolution uint8 mask
+// (F.interpolate to the latent grid, nearest) and channels C+1 .. 2C = the posterior sample of the
+// masked image's moments * scaling. Those channels are constant over the loop: only this launch writes
+// them. Then *timestep = t_start, and the step index and arrival counter reset as lb_sample_step's init.
+__global__ void __launch_bounds__(256)
+sample_init_kernel(const void* __restrict__ mom, int md, long long sb, long long sc, long long sp,
+                   const void* __restrict__ post_eps, int ed, float scaling,
+                   const unsigned char* __restrict__ mask, const float* __restrict__ noise,
+                   const float* __restrict__ table, float* __restrict__ x, int* __restrict__ step_index,
+                   unsigned int* __restrict__ counter, void* __restrict__ unet_in, int udt, int Cu,
+                   float* __restrict__ timestep, int G, int B, int C, int H, int W) {
+  const int P = H * W;
+  const long long i = blockIdx.x * 256ll + threadIdx.x;
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    *timestep = table[2];
+    *step_index = 0;
+    *counter = 0u;
+  }
+  if (i >= static_cast<long long>(B) * P) return;
+  const int b = static_cast<int>(i / P), px = static_cast<int>(i % P);
+  const float c_noise = table[0], s = table[1], c_lat = table[3];
+  const int td = ed == md ? md : LB_F32;
+  const bool from_image = mom != nullptr && mask == nullptr;
+  const long long mbase = b * sb + px * sp;
+  for (int c = 0; c < C; ++c) {
+    const long long xi = (static_cast<long long>(b) * C + c) * P + px;
+    float xn;
+    if (from_image) {
+      const long long mi = mbase + c * sc;
+      const float lat = posterior_sample(mom, md, mi, mi + C * sc, post_eps, ed, xi, td, scaling);
+      xn = __fadd_rn(__fmul_rn(c_lat, lat), __fmul_rn(c_noise, noise[xi]));
+    } else {
+      xn = __fmul_rn(noise[xi], c_noise);
+    }
+    x[xi] = xn;
+    const float u = __fmul_rn(s, xn);
+    for (int h = 0; h < G; ++h) st_any(unet_in, (static_cast<long long>(h * B + b) * P + px) * Cu + c, udt, u);
+  }
+  if (mask) {
+    const int h = px / W, w = px % W;
+    const float m = binarise_u8(mask[(static_cast<long long>(b) * 8 * H + 8 * h) * (8ll * W) + 8 * w]);
+    for (int g = 0; g < G; ++g) st_any(unet_in, (static_cast<long long>(g * B + b) * P + px) * Cu + C, udt, m);
+    for (int c = 0; c < C; ++c) {
+      const long long mi = mbase + c * sc;
+      const long long xi = (static_cast<long long>(b) * C + c) * P + px;
+      const float ml = posterior_sample(mom, md, mi, mi + C * sc, post_eps, ed, xi, td, scaling);
+      for (int g = 0; g < G; ++g)
+        st_any(unet_in, (static_cast<long long>(g * B + b) * P + px) * Cu + C + 1 + c, udt, ml);
+    }
   }
 }
 
@@ -420,13 +500,25 @@ extern "C" int lb_masked_mse_fwd_bwd(const void* pred, int pred_dtype, long long
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
-extern "C" int lb_sample_step(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+extern "C" int lb_pixels_ingest_inpaint(const void* pixels, const unsigned char* mask, void* masked_out,
+                                        int out_dtype, int channels_last, int B, int H, int W, void* stream) {
+  if (B <= 0 || H <= 0 || W <= 0 || pixels == nullptr || mask == nullptr || masked_out == nullptr)
+    return LB_ERR_SHAPE;
+  if (!float_dtype(out_dtype)) return LB_ERR_DTYPE;
+  const long long P = static_cast<long long>(H) * W, n = B * P;
+  pixels_ingest_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      pixels, 1, mask, MASK_U8_PIPELINE, nullptr, masked_out, out_dtype, channels_last != 0, B, P);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+static int launch_sample_step(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
                               long long stride_p, int G, float* x, const float* noise, const float* table,
                               int table_rows, const float* guidance, int* step_index, unsigned int* counter,
-                              void* unet_in, int unet_dtype, float* timestep, void* vae_in, int vae_dtype,
-                              int vae_channels_last, float vae_inv_scaling, int B, int C, int H, int W, int init,
-                              void* stream) {
+                              void* unet_in, int unet_dtype, int unet_channels, float* timestep, void* vae_in,
+                              int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B, int C, int H,
+                              int W, int init, void* stream) {
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || (G != 1 && G != 2) || table_rows < 2) return LB_ERR_SHAPE;
+  if (unet_channels < C) return LB_ERR_SHAPE;
   if (!float_dtype(unet_dtype) || !float_dtype(vae_dtype) || (!init && !float_dtype(model_dtype)))
     return LB_ERR_DTYPE;
   if (x == nullptr || noise == nullptr || table == nullptr || step_index == nullptr || counter == nullptr ||
@@ -437,8 +529,55 @@ extern "C" int lb_sample_step(const void* model_out, int model_dtype, long long 
   const long long n = static_cast<long long>(B) * H * W;
   sample_step_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows, guidance, step_index,
-      counter, unet_in, unet_dtype, timestep, vae_in, vae_dtype, vae_channels_last != 0, vae_inv_scaling, B, C, H * W,
-      init != 0);
+      counter, unet_in, unet_dtype, unet_channels, timestep, vae_in, vae_dtype, vae_channels_last != 0,
+      vae_inv_scaling, B, C, H * W, init != 0);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
+}
+
+extern "C" int lb_sample_step(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                              long long stride_p, int G, float* x, const float* noise, const float* table,
+                              int table_rows, const float* guidance, int* step_index, unsigned int* counter,
+                              void* unet_in, int unet_dtype, float* timestep, void* vae_in, int vae_dtype,
+                              int vae_channels_last, float vae_inv_scaling, int B, int C, int H, int W, int init,
+                              void* stream) {
+  return launch_sample_step(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows,
+                            guidance, step_index, counter, unet_in, unet_dtype, C, timestep, vae_in, vae_dtype,
+                            vae_channels_last, vae_inv_scaling, B, C, H, W, init, stream);
+}
+
+extern "C" int lb_sample_step_ch(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                                 long long stride_p, int G, float* x, const float* noise, const float* table,
+                                 int table_rows, const float* guidance, int* step_index, unsigned int* counter,
+                                 void* unet_in, int unet_dtype, int unet_channels, float* timestep, void* vae_in,
+                                 int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B, int C, int H,
+                                 int W, int init, void* stream) {
+  return launch_sample_step(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows,
+                            guidance, step_index, counter, unet_in, unet_dtype, unet_channels, timestep, vae_in,
+                            vae_dtype, vae_channels_last, vae_inv_scaling, B, C, H, W, init, stream);
+}
+
+extern "C" int lb_sample_init(const void* moments, int moments_dtype, long long stride_b, long long stride_c,
+                              long long stride_p, const void* posterior_noise, int posterior_noise_dtype,
+                              float scaling, const unsigned char* mask, const float* noise, const float* table,
+                              int table_rows, float* x, int* step_index, unsigned int* counter, void* unet_in,
+                              int unet_dtype, int unet_channels, float* timestep, int G, int B, int C, int H, int W,
+                              void* stream) {
+  if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || (G != 1 && G != 2) || table_rows < 2) return LB_ERR_SHAPE;
+  if (!float_dtype(unet_dtype)) return LB_ERR_DTYPE;
+  if (x == nullptr || noise == nullptr || table == nullptr || step_index == nullptr || counter == nullptr ||
+      unet_in == nullptr || timestep == nullptr)
+    return LB_ERR_SHAPE;
+  if (unet_channels != (mask ? 2 * C + 1 : C)) return LB_ERR_SHAPE;
+  if (mask && moments == nullptr) return LB_ERR_SHAPE;
+  if (moments) {
+    if (!float_dtype(moments_dtype)) return LB_ERR_DTYPE;
+    if (posterior_noise_dtype != moments_dtype && posterior_noise_dtype != LB_F32) return LB_ERR_DTYPE;
+    if (posterior_noise == nullptr) return LB_ERR_SHAPE;
+  }
+  const long long n = static_cast<long long>(B) * H * W;
+  sample_init_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      moments, moments_dtype, stride_b, stride_c, stride_p, posterior_noise, posterior_noise_dtype, scaling, mask,
+      noise, table, x, step_index, counter, unet_in, unet_dtype, unet_channels, timestep, G, B, C, H, W);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 

@@ -33,6 +33,16 @@ clip_sample=False, "leading" spacing):
                 v_prediction: x0 = a^0.5 x - (1 - a)^0.5 m,  eps = a^0.5 m + (1 - a)^0.5 x
                 x' = a_prev^0.5 x0 + (1 - a_prev)^0.5 eps            (gamma = 0, s = 1)
 
+img2img (StableDiffusionImg2ImgPipeline) starts part-way down the same schedule. get_timesteps, as in
+diffusers 0.11-0.14 (the releases without the older `steps_offset` term):
+  init_timestep = min(int(n * strength), n);  t_start = max(n - init_timestep, 0)
+  timesteps[t_start:] run, with the full schedule's per-step coefficients (the schedulers look their
+  sigma / alpha up by timestep), and the start latents are scheduler.add_noise(init_latents, z_0, t):
+  Euler-ancestral  x = init_latents + z_0 * sigma[t_start]             (init_noise_sigma is not used)
+  DDIM             x = sqrt(acp[t]) * init_latents + sqrt(1 - acp[t]) * z_0   (float32 tables)
+`int(n * strength)` truncates the float product: 50 * 0.58 = 28.999999999999996 runs 28 steps.
+txt2img and inpainting start from x = init_noise_sigma * z_0, the first UNet input s_0 * x.
+
 DDPM / PNDM sampling are not provided: DDPM's strided-variance rule changed between diffusers
 releases, and no copy of them is installed to pin it against.
 """
@@ -44,7 +54,7 @@ import torch
 SCHEDULERS = ("euler_ancestral", "ddim")
 PREDICTION_TYPES = ("epsilon", "v_prediction")
 NUM_TRAIN_TIMESTEPS = 1000
-TABLE_COLS = 8          # row 0: (init_noise_sigma, s_0, t_0, 0...); row 1 + i: (alpha, beta, gamma, s_next, t_next, last, 0, 0)
+TABLE_COLS = 8          # row 0: (c_noise, s_start, t_start, c_lat, 0...); row 1 + i: (alpha, beta, gamma, s_next, t_next, last, 0, 0)
 
 
 def check(scheduler: str, prediction_type: str):
@@ -118,13 +128,53 @@ def coefficients(scheduler: str, prediction_type: str, n: int):
     return (1.0, 1.0, ts[0]), steps
 
 
-def pack_table(scheduler: str, prediction_type: str, n: int, max_steps: int) -> torch.Tensor:
-    """The float32 [max_steps + 1, TABLE_COLS] table lb_sample_step reads (rows past n are zero)."""
-    if n > max_steps:
-        raise ValueError(f"num_inference_steps {n} exceeds max_steps {max_steps}")
+def t_start(n: int, strength: float) -> int:
+    """The index of the first timestep an img2img run of n steps at `strength` keeps (get_timesteps of
+    diffusers 0.11-0.14); n - t_start steps run. Refuses a strength that would run no step."""
+    if not 0.0 < strength <= 1.0:
+        raise ValueError(f"strength must be in (0, 1], got {strength}")
+    init_timestep = min(int(n * strength), n)
+    if init_timestep == 0:
+        raise ValueError(f"strength {strength} with {n} steps runs no denoising step (int({n} * {strength}) == 0)")
+    return max(n - init_timestep, 0)
+
+
+def add_noise_coefficients(scheduler: str, n: int, start: int):
+    """(c_lat, c_noise): the float32 scalars scheduler.add_noise(x, z, timesteps[start]) evaluates as
+    c_lat * x + c_noise * z (Euler-ancestral: 1 and sigma[start]; DDIM: sqrt(acp[t]) and sqrt(1 - acp[t]),
+    each rounded to float32 as torch computes them from the float32 alphas_cumprod)."""
+    if scheduler == "euler_ancestral":
+        return np.float32(1.0), euler_sigmas(n)[start]
+    acp = alphas_cumprod().numpy()
+    t = int(timesteps("ddim", n)[start])
+    return np.sqrt(acp[t]), np.sqrt(np.float32(1.0) - acp[t])
+
+
+def pack_table(scheduler: str, prediction_type: str, n: int, max_steps: int, t_start: int = 0,
+               from_image: bool = False) -> torch.Tensor:
+    """The float32 [max_steps + 1, TABLE_COLS] table lb_sample_step (and lb_sample_init) reads.
+
+    Rows 1..k (k = n - t_start) are coefficients()[t_start:], `last` set on row k; rows past k are zero.
+    Row 0 is (c_noise, s_start, t_start's timestep, c_lat): txt2img / inpainting (from_image=False,
+    t_start = 0) start from init_noise_sigma * z_0 (c_lat = 0); img2img (from_image=True) from
+    add_noise(init_latents, z_0, timesteps[t_start]) (add_noise_coefficients)."""
+    k = n - t_start
+    if not 0 <= t_start < n:
+        raise ValueError(f"t_start {t_start} outside [0, {n})")
+    if t_start and not from_image:
+        raise ValueError("only an img2img table (from_image=True) starts part-way down the schedule")
+    if k > max_steps:
+        raise ValueError(f"{k} denoising steps exceed max_steps {max_steps}")
     (sigma0, s0, t0), steps = coefficients(scheduler, prediction_type, n)
     tab = np.zeros((max_steps + 1, TABLE_COLS), dtype=np.float64)
-    tab[0, :3] = (sigma0, s0, t0)
-    tab[1:n + 1, :5] = steps
-    tab[n, 5] = 1.0
+    if t_start:
+        s0 = steps[t_start - 1, 3]                 # the step before's s_next / t_next: s and t at t_start
+        t0 = steps[t_start - 1, 4]
+    if from_image:
+        c_lat, c_noise = add_noise_coefficients(scheduler, n, t_start)
+        tab[0, :4] = (c_noise, s0, t0, c_lat)
+    else:
+        tab[0, :3] = (sigma0, s0, t0)
+    tab[1:k + 1, :5] = steps[t_start:]
+    tab[k, 5] = 1.0
     return torch.from_numpy(tab.astype(np.float32))

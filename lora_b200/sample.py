@@ -8,21 +8,39 @@ the same host models and fused LoRA kernels the training steps use.
     s.prepare()
     img = s.sample(input_ids, negative_input_ids, seed=0)   # uint8 [B, 8h, 8w, 3] on the device
 
+img2img (StableDiffusionImg2ImgPipeline) and inpainting (StableDiffusionInpaintPipeline on the
+9-channel UNet) run through the same three graphs, with `SamplerConfig(task="img2img" | "inpaint")`:
+
+    s = LoraSampler(unet, text_encoder, vae, SamplerConfig(task="img2img", strength=0.75), latent_shape=...)
+    img = s.sample(input_ids, negative_input_ids, seed=0, image=init_u8)             # [B, 8h, 8w, 3] uint8
+    s = LoraSampler(unet_9ch, text_encoder, vae, SamplerConfig(task="inpaint"), latent_shape=...)
+    img = s.sample(input_ids, negative_input_ids, seed=0, image=init_u8, mask_image=mask_u8)  # [B, 8h, 8w]
+
+Images and masks come at the sampler's resolution (8h x 8w; resizing is the caller's job) and are
+copied into static buffers. The mask is the pipeline's: uint8 0..255, white (>= 128) repainted.
+
 A `sample()` replays three CUDA graphs, with no host sync and no allocation between them:
   A  the sampled sites' down factors re-cast into the 16-bit operands graph B reads, the text encoder on
      [negative ; prompt] ids, and the init launch of lb_sample_step (x = z_0 * init_noise_sigma);
+     img2img / inpaint: the image ingest (lb_pixels_ingest / lb_pixels_ingest_inpaint), the VAE encoder
+     (torch, in the VAE's dtype and layout) and lb_sample_init in place of that init launch: the posterior
+     sample, add_noise at the first kept timestep (img2img), the first UNet input, and for inpainting
+     the mask and masked-image latent channels of the UNet input, which no later launch rewrites;
   B  one denoising step: the UNet at batch G*B, then lb_sample_step (guidance sum, the scheduler's update
      as folded coefficients, the next UNet input and timestep). Replayed N times: the step index lives
-     on the device and the kernel advances it;
+     on the device and the kernel advances it. img2img runs the last k = n - t_start steps of the
+     n-step schedule (host/schedulers.t_start: int(n * strength) steps), so B is replayed k times;
   C  the VAE decoder and lb_pixels_emit.
 `use_cuda_graph=False` runs the same code eagerly. The number of steps (up to `max_steps`), the
-scheduler, the guidance scale and the seed may change per call: they rewrite device tables. A guidance
+scheduler, the guidance scale, the seed, the strength, the image and the mask may change per call:
+they rewrite device tables and buffers. A guidance
 scale <= 1 runs without the unconditional half (G = 1), as the pipeline does; that is a capture of its own.
 The graphs are captured again only when something baked into a launch changes: a site's scale, a
 selector, the set of sites or their parameter storage, the grouping policy (`captures` counts them).
 
-All noise (z_0 and each step's z_i) is one draw of [N + 1, B, C, h, w] from the sampler's own
-torch.Generator seeded by `seed`; the global CUDA RNG stream is never touched, so a training step's noise
+All noise (z_0 and each step's z_i) is one draw of [k + 1, B, C, h, w] from the sampler's own
+torch.Generator seeded by `seed`, then (img2img / inpaint) the posterior noise [B, C, h, w] of the one
+encoded image, in the VAE's dtype as DiagonalGaussianDistribution.sample draws it; the global CUDA RNG stream is never touched, so a training step's noise
 is the same with or without sampling in between. The models run in eval() under no_grad and get their
 train / eval modes back afterwards.
 """
@@ -34,7 +52,7 @@ import torch.nn as nn
 
 from . import _C, ops
 from .host import schedulers
-from .step_ops import pixels_emit, sample_step
+from .step_ops import pixels_emit, pixels_ingest, pixels_ingest_inpaint, sample_init, sample_step, sample_step_ch
 
 _SITE_NAMES = ("LoraInjectedLinear", "LoraInjectedConv2d")
 
@@ -54,6 +72,13 @@ class SamplerConfig:
     # read the noise from `self.noise` ([max_steps + 1, B, C, h, w], caller-filled) instead of drawing it
     external_noise: bool = False
     graph_warmup: int = 2
+    # "txt2img" | "img2img" (StableDiffusionImg2ImgPipeline) | "inpaint" (StableDiffusionInpaintPipeline,
+    # a UNet of 2C + 1 input channels); with external_noise the caller fills `self.posterior_noise` too
+    task: str = "txt2img"
+    strength: float = 0.8                      # img2img: the part of the schedule run (the pipeline's default)
+
+
+TASKS = ("txt2img", "img2img", "inpaint")
 
 
 def _sites(*models):
@@ -69,9 +94,19 @@ class LoraSampler:
             raise ValueError("LoraSampler does not sample SDXL UNets (addition_embed_type "
                              f"{ucfg.addition_embed_type!r}): their pooled and time-id conditioning is not supported")
         B, C, h, w = latent_shape
-        if getattr(ucfg, "in_channels", C) != C:
+        if cfg.task not in TASKS:
+            raise ValueError(f"unknown task {cfg.task!r}: one of {TASKS}")
+        Cu = 2 * C + 1 if cfg.task == "inpaint" else C
+        if getattr(ucfg, "in_channels", Cu) != Cu:
+            if cfg.task == "inpaint":
+                raise ValueError(f"task 'inpaint' needs a UNet of {Cu} input channels (latents, mask, masked-image "
+                                 f"latents), this one takes {ucfg.in_channels}")
             raise ValueError(f"the UNet takes {ucfg.in_channels} input channels, the latents have {C}: inpainting "
-                             "UNets are not sampled")
+                             "UNets are sampled with SamplerConfig(task='inpaint')")
+        if cfg.task == "img2img":
+            schedulers.t_start(cfg.num_inference_steps, cfg.strength)        # refuses strengths that run no step
+        elif not 0.0 < cfg.strength <= 1.0:
+            raise ValueError(f"strength must be in (0, 1], got {cfg.strength}")
         if not getattr(vae, "has_decoder", hasattr(vae, "decoder")):
             raise ValueError("the VAE has no decoder: build it with AutoencoderKL(cfg, with_decoder=True)")
         if cfg.num_inference_steps < 1 or cfg.max_steps < cfg.num_inference_steps:
@@ -94,12 +129,18 @@ class LoraSampler:
         self.step_index = torch.zeros(1, device=dev, dtype=torch.int32)
         self._counter = torch.zeros(1, device=dev, dtype=torch.int32)
         self.timestep = torch.zeros(1, device=dev, dtype=torch.float32)
-        self.unet_in = {G: torch.zeros((G * B, C, h, w), device=dev, dtype=self.model_dtype).contiguous(
+        self.unet_in = {G: torch.zeros((G * B, Cu, h, w), device=dev, dtype=self.model_dtype).contiguous(
             memory_format=torch.channels_last) for G in (1, 2)}
         self.vae_in = torch.zeros(latent_shape, device=dev, dtype=self.vae_dtype).contiguous(
             memory_format=torch.channels_last if vae_cl else torch.contiguous_format)
         self.image = torch.zeros((B, 8 * h, 8 * w, 3), device=dev, dtype=torch.uint8)
         self.generator = torch.Generator(device=dev)
+        if cfg.task != "txt2img":
+            self.vae_enc_cl = not vae.encoder.conv_in.weight.is_contiguous()
+            self.pixels = torch.zeros((B, 8 * h, 8 * w, 3), device=dev, dtype=torch.uint8)
+            self.posterior_noise = torch.zeros(latent_shape, device=dev, dtype=next(vae.encoder.parameters()).dtype)
+        if cfg.task == "inpaint":
+            self.mask_image = torch.zeros((B, 8 * h, 8 * w), device=dev, dtype=torch.uint8)
         self._ehs = {}
         self._table_key = None
         self._graphs = {}             # G -> (A, B, C)
@@ -167,14 +208,27 @@ class LoraSampler:
         ids = self.input_ids if G == 2 else self.input_ids[B:]
         with self._autocast():
             self._ehs[G] = self.text_encoder(ids)[0].to(self.model_dtype)
-        sample_step(None, self.latents, self.noise, self.table, None, self.step_index, self._counter,
-                    self.unet_in[G], self.timestep, None, self.cfg.vae_scaling, init=True)
+        task = self.cfg.task
+        if task == "txt2img":
+            sample_step(None, self.latents, self.noise, self.table, None, self.step_index, self._counter,
+                        self.unet_in[G], self.timestep, None, self.cfg.vae_scaling, init=True)
+            return
+        enc_dtype = self.posterior_noise.dtype
+        if task == "img2img":          # preprocess: 2 * (u8 / 255) - 1, equal to the ingest bit for bit
+            x, _ = pixels_ingest(self.pixels, enc_dtype, channels_last=self.vae_enc_cl)
+        else:                          # prepare_mask_and_masked_image
+            x = pixels_ingest_inpaint(self.pixels, self.mask_image, enc_dtype, channels_last=self.vae_enc_cl)
+        moments = self.vae.encode(x).latent_dist.parameters
+        sample_init(moments, self.posterior_noise, self.latents, self.noise, self.table, self.step_index,
+                    self._counter, self.unet_in[G], self.timestep, self.cfg.vae_scaling,
+                    mask=self.mask_image if task == "inpaint" else None)
 
     def _body_b(self, G: int):
         with self._autocast():
             out = self.unet(self.unet_in[G], self.timestep, self._ehs[G]).sample
-        sample_step(out, self.latents, self.noise, self.table, self.guidance, self.step_index, self._counter,
-                    self.unet_in[G], self.timestep, self.vae_in, self.cfg.vae_scaling)
+        step = sample_step_ch if self.cfg.task == "inpaint" else sample_step
+        step(out, self.latents, self.noise, self.table, self.guidance, self.step_index, self._counter,
+             self.unet_in[G], self.timestep, self.vae_in, self.cfg.vae_scaling)
 
     def _body_c(self):
         pixels_emit(self.vae.decode(self.vae_in).sample, self.image)
@@ -231,7 +285,8 @@ class LoraSampler:
             m.training = training
 
     # ------------------------------------------------------------------ public API
-    def _options(self, num_inference_steps, scheduler, guidance_scale):
+    def _options(self, num_inference_steps, scheduler, guidance_scale, strength=None):
+        """(n, scheduler, guidance, t_start) of a call."""
         cfg = self.cfg
         n = cfg.num_inference_steps if num_inference_steps is None else int(num_inference_steps)
         sched = cfg.scheduler if scheduler is None else scheduler
@@ -239,34 +294,65 @@ class LoraSampler:
         schedulers.check(sched, cfg.prediction_type)
         if not 1 <= n <= cfg.max_steps:
             raise ValueError(f"num_inference_steps {n}: need 1 <= n <= max_steps ({cfg.max_steps})")
-        return n, sched, g
+        if strength is not None and cfg.task != "img2img":
+            raise ValueError(f"strength applies to img2img only, not to task {cfg.task!r}")
+        start = schedulers.t_start(n, cfg.strength if strength is None else float(strength)) \
+            if cfg.task == "img2img" else 0
+        return n, sched, g, start
 
-    def _set_table(self, sched: str, n: int):
-        key = (sched, n)
+    def _set_table(self, sched: str, n: int, start: int = 0):
+        key = (sched, n, start)
         if key != self._table_key:
-            self.table.copy_(schedulers.pack_table(sched, self.cfg.prediction_type, n, self.cfg.max_steps))
+            self.table.copy_(schedulers.pack_table(sched, self.cfg.prediction_type, n, self.cfg.max_steps, start,
+                                                   from_image=self.cfg.task == "img2img"))
             self._table_key = key
+
+    def _set_images(self, image, mask_image):
+        """Copy the call's image (and mask) into the static buffers, after checking them."""
+        task = self.cfg.task
+        if task == "txt2img":
+            if image is not None or mask_image is not None:
+                raise ValueError("task 'txt2img' takes no image or mask_image: use task 'img2img' or 'inpaint'")
+            return
+        if image is None or image.dtype != torch.uint8 or tuple(image.shape) != tuple(self.pixels.shape):
+            raise ValueError(f"task {task!r} needs image: uint8 {tuple(self.pixels.shape)} (B, 8h, 8w, RGB) at the "
+                             f"sampler's resolution, got "
+                             f"{None if image is None else (image.dtype, tuple(image.shape))}")
+        if task == "img2img":
+            if mask_image is not None:
+                raise ValueError("task 'img2img' takes no mask_image: use task 'inpaint'")
+        elif (mask_image is None or mask_image.dtype != torch.uint8
+              or tuple(mask_image.shape) != tuple(self.mask_image.shape)):
+            raise ValueError(f"task 'inpaint' needs mask_image: uint8 {tuple(self.mask_image.shape)} (B, 8h, 8w, "
+                             f"0..255), got {None if mask_image is None else (mask_image.dtype, tuple(mask_image.shape))}")
+        self.pixels.copy_(image)
+        if task == "inpaint":
+            self.mask_image.copy_(mask_image)
 
     def prepare(self, guidance_scale: Optional[float] = None):
         """Capture the graphs for the configured (or given) guidance scale ahead of the first sample()."""
         if not self.cfg.use_cuda_graph:
             return
-        _, _, g = self._options(None, None, guidance_scale)
+        n, sched, g, start = self._options(None, None, guidance_scale)
         saved = self._enter_eval()
         try:
             with torch.no_grad():
-                self._set_table(self.cfg.scheduler, self.cfg.num_inference_steps)
+                self._set_table(sched, n, start)
                 self._graphs_for(2 if g > 1.0 else 1)
         finally:
             self._restore_modes(saved)
 
     def sample(self, input_ids: torch.Tensor, negative_input_ids: Optional[torch.Tensor] = None, seed: int = 0,
                num_inference_steps: Optional[int] = None, scheduler: Optional[str] = None,
-               guidance_scale: Optional[float] = None) -> torch.Tensor:
+               guidance_scale: Optional[float] = None, image: Optional[torch.Tensor] = None,
+               mask_image: Optional[torch.Tensor] = None, strength: Optional[float] = None) -> torch.Tensor:
         """uint8 [B, 8h, 8w, 3] images (a view of `self.image`, overwritten by the next call) for the token
         ids [B, seq_len] of the prompts and of the negative prompts (the empty prompt's ids for plain
-        classifier-free guidance; unused when guidance_scale <= 1). `self.latents` holds the final latents."""
-        n, sched, g = self._options(num_inference_steps, scheduler, guidance_scale)
+        classifier-free guidance; unused when guidance_scale <= 1). `self.latents` holds the final latents.
+        img2img: image uint8 [B, 8h, 8w, 3], strength in (0, 1] (default cfg.strength); inpaint: image and
+        mask_image uint8 [B, 8h, 8w] (0..255, >= 128 repainted)."""
+        n, sched, g, start = self._options(num_inference_steps, scheduler, guidance_scale, strength)
+        k = n - start
         G = 2 if g > 1.0 else 1
         B = self.latents.shape[0]
         if tuple(input_ids.shape) != tuple(self.input_ids[B:].shape):
@@ -274,25 +360,28 @@ class LoraSampler:
                              f"{tuple(self.input_ids[B:].shape)}")
         if G == 2 and (negative_input_ids is None or tuple(negative_input_ids.shape) != tuple(input_ids.shape)):
             raise ValueError("guidance_scale > 1 needs negative_input_ids of the prompts' shape")
+        self._set_images(image, mask_image)
         saved = self._enter_eval()
         try:
             with torch.no_grad():
-                self._set_table(sched, n)
+                self._set_table(sched, n, start)
                 self.guidance.fill_(g)
                 self.input_ids[B:].copy_(input_ids)
                 if G == 2:
                     self.input_ids[:B].copy_(negative_input_ids)
                 if not self.cfg.external_noise:
                     self.generator.manual_seed(int(seed))
-                    self.noise[:n + 1].normal_(generator=self.generator)
+                    self.noise[:k + 1].normal_(generator=self.generator)
+                    if self.cfg.task != "txt2img":
+                        self.posterior_noise.normal_(generator=self.generator)
                 if self.cfg.use_cuda_graph:
                     ga, gb, gc = self._graphs_for(G)
                     ga.replay()
-                    for _ in range(n):
+                    for _ in range(k):
                         gb.replay()
                     gc.replay()
                 else:
-                    self._run_eager(G, n)
+                    self._run_eager(G, k)
         finally:
             self._restore_modes(saved)
         return self.image

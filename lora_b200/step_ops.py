@@ -15,6 +15,10 @@ and the two ends of a sampling step (lora_b200/sample.py):
 
   sample_step       guidance sum + the scheduler's update (folded coefficients) + the next UNet input
                     and timestep (+ the decoder input on the last step); init=True: the first input
+  sample_step_ch    the same into the 9-channel inpainting UNet's input (latent channels only)
+  sample_init       the start of an img2img / inpainting loop: posterior sample, add_noise, the first
+                    UNet input (+ the inpainting mask and masked-image latent channels)
+  pixels_ingest_inpaint  uint8 image + 0..255 mask -> the inpainting pipeline's masked image
   pixels_emit       decoded image -> (x / 2 + 0.5).clamp(0, 1) -> uint8 HWC, diffusers' post-processing
 
 and the latent cache of cli_lora_pti.py:141-151 (`cached_latents=True`): the VAE runs once per
@@ -177,6 +181,51 @@ def _dense_hw_strides(t: torch.Tensor, what: str):
     return sb, sc, sw
 
 
+def _sample_step_args(model_out, x, noise, table, guidance, step_index, counter, unet_in, timestep, vae_in,
+                      vae_scaling, init, unet_channels, what):
+    """The argument tuple of lb_sample_step / lb_sample_step_ch after sample_step's checks (unet_in has
+    `unet_channels` channels)."""
+    if not x.is_cuda:
+        raise _C.LoraB200Error(f"{what} needs CUDA tensors (no CPU path)")
+    if not vae_scaling > 0.0:
+        raise _C.LoraB200Error(f"{what}: vae_scaling must be positive, got {vae_scaling}")
+    B, C, H, W = x.shape
+    Cu = C if unet_channels is None else unet_channels
+    G = unet_in.shape[0] // B
+    if x.dtype != torch.float32 or not x.is_contiguous():
+        raise _C.LoraB200Error(f"{what}: x must be a contiguous float32 tensor")
+    if (tuple(unet_in.shape) != (G * B, Cu, H, W) or unet_in.shape[0] % B
+            or not unet_in.is_contiguous(memory_format=torch.channels_last)):
+        raise _C.LoraB200Error(f"{what}: unet_in must be a channels_last [G*B, {Cu}, {H}, {W}] tensor, "
+                               f"got {tuple(unet_in.shape)}")
+    if (table.dtype != torch.float32 or table.dim() != 2 or table.shape[1] != 8 or not table.is_contiguous()
+            or noise.dtype != torch.float32 or tuple(noise.shape) != (table.shape[0], B, C, H, W)
+            or not noise.is_contiguous()):
+        raise _C.LoraB200Error(f"{what}: table must be fp32 [rows, 8] and noise fp32 [rows, B, C, H, W]")
+    if step_index.dtype != torch.int32 or counter.dtype != torch.int32 or timestep.dtype != torch.float32:
+        raise _C.LoraB200Error(f"{what}: step_index / counter int32 [1], timestep fp32 [1]")
+    sb = sc = sp = 0
+    mdt = vdt = _C.LB_F32
+    vcl = 0
+    if not init:
+        if model_out is None or tuple(model_out.shape) != (G * B, C, H, W):
+            raise _C.LoraB200Error(f"{what}: model_out must be [{G * B}, {C}, {H}, {W}]")
+        sb, sc, sp = _dense_hw_strides(model_out, "model_out")
+        mdt = dtype_code(model_out.dtype)
+        if vae_in is None or tuple(vae_in.shape) != (B, C, H, W):
+            raise _C.LoraB200Error(f"{what}: vae_in must be [{B}, {C}, {H}, {W}]")
+        vcl = int(not vae_in.is_contiguous())
+        if vcl and not vae_in.is_contiguous(memory_format=torch.channels_last):
+            raise _C.LoraB200Error(f"{what}: vae_in must be contiguous or channels_last")
+        vdt = dtype_code(vae_in.dtype)
+        if guidance is None or guidance.dtype != torch.float32:
+            raise _C.LoraB200Error(f"{what}: guidance must be a float32 [1] tensor")
+    head = (ptr(model_out), mdt, sb, sc, sp, G, ptr(x), ptr(noise), ptr(table), table.shape[0], ptr(guidance),
+            ptr(step_index), ptr(counter), ptr(unet_in), dtype_code(unet_in.dtype))
+    tail = (ptr(timestep), ptr(vae_in), vdt, vcl, 1.0 / float(vae_scaling), B, C, H, W, int(init), stream_ptr())
+    return head, tail
+
+
 def sample_step(model_out: Optional[torch.Tensor], x: torch.Tensor, noise: torch.Tensor, table: torch.Tensor,
                 guidance: Optional[torch.Tensor], step_index: torch.Tensor, counter: torch.Tensor,
                 unet_in: torch.Tensor, timestep: torch.Tensor, vae_in: Optional[torch.Tensor],
@@ -190,45 +239,101 @@ def sample_step(model_out: Optional[torch.Tensor], x: torch.Tensor, noise: torch
     vae_in: [B, C, H, W] in the VAE's dtype, contiguous or channels_last, written on the last step as
     `1 / vae_scaling * x` (the pipeline's expression, the reciprocal rounded to fp32).
     init=True: x = z_0 * init_noise_sigma and the first UNet input and timestep; the index is reset."""
+    head, tail = _sample_step_args(model_out, x, noise, table, guidance, step_index, counter, unet_in, timestep,
+                                   vae_in, vae_scaling, init, None, "sample_step")
+    check(_C.lib.lb_sample_step(*head, *tail), "lb_sample_step")
+    ops._count()
+
+
+def sample_step_ch(model_out: Optional[torch.Tensor], x: torch.Tensor, noise: torch.Tensor, table: torch.Tensor,
+                   guidance: Optional[torch.Tensor], step_index: torch.Tensor, counter: torch.Tensor,
+                   unet_in: torch.Tensor, timestep: torch.Tensor, vae_in: Optional[torch.Tensor],
+                   vae_scaling: float, init: bool = False):
+    """sample_step into a UNet input of more channels than the latents (lb_sample_step_ch): unet_in is a
+    channels_last [G*B, C', H, W] tensor, C' >= C (the inpainting UNet's 2C + 1), and only its channels
+    [0, C) are written."""
+    Cu = unet_in.shape[1] if unet_in.dim() == 4 else -1
+    if Cu < x.shape[1]:
+        raise _C.LoraB200Error(f"sample_step_ch: unet_in has {Cu} channels, fewer than the latents' {x.shape[1]}")
+    head, tail = _sample_step_args(model_out, x, noise, table, guidance, step_index, counter, unet_in, timestep,
+                                   vae_in, vae_scaling, init, Cu, "sample_step_ch")
+    check(_C.lib.lb_sample_step_ch(*head, Cu, *tail), "lb_sample_step_ch")
+    ops._count()
+
+
+def sample_init(moments: Optional[torch.Tensor], posterior_noise: Optional[torch.Tensor], x: torch.Tensor,
+                noise: torch.Tensor, table: torch.Tensor, step_index: torch.Tensor, counter: torch.Tensor,
+                unet_in: torch.Tensor, timestep: torch.Tensor, scaling: float = 0.18215,
+                mask: Optional[torch.Tensor] = None):
+    """One launch of lb_sample_init, in place on preallocated buffers (nothing is allocated: capturable).
+
+    moments: `vae.encode(image).latent_dist.parameters` [B, 2C, h, w] in the VAE's dtype (NCHW or
+    channels_last) or None; posterior_noise: [B, C, h, w] standard normal in that dtype or fp32.
+    Without mask (img2img): x = add_noise(latent_dist.sample() * scaling, z_0, t_start) from row 0 of the
+    table (c_noise, s_start, t_start, c_lat); without moments: x = z_0 * c_noise. mask (inpainting): uint8
+    [B, 8h, 8w], 0..255, the pipeline's mask image; moments are then the masked image's, x = z_0 * c_noise,
+    and unet_in ([G*B, 2C + 1, h, w]) gets the binarised latent-grid mask in channel C and the masked
+    image's latents in channels C+1..2C. The first UNet input s_start * x goes to channels [0, C) of every
+    half; timestep, step_index and counter are set as lb_sample_step's init sets them."""
     if not x.is_cuda:
-        raise _C.LoraB200Error("sample_step needs CUDA tensors (no CPU path)")
-    if not vae_scaling > 0.0:
-        raise _C.LoraB200Error(f"sample_step: vae_scaling must be positive, got {vae_scaling}")
+        raise _C.LoraB200Error("sample_init needs CUDA tensors (no CPU path)")
     B, C, H, W = x.shape
-    G = unet_in.shape[0] // B
     if x.dtype != torch.float32 or not x.is_contiguous():
-        raise _C.LoraB200Error("sample_step: x must be a contiguous float32 tensor")
-    if (tuple(unet_in.shape) != (G * B, C, H, W) or unet_in.shape[0] % B
+        raise _C.LoraB200Error("sample_init: x must be a contiguous float32 tensor")
+    Cu = C if mask is None else 2 * C + 1
+    G = unet_in.shape[0] // B
+    if (tuple(unet_in.shape) != (G * B, Cu, H, W) or G not in (1, 2)
             or not unet_in.is_contiguous(memory_format=torch.channels_last)):
-        raise _C.LoraB200Error(f"sample_step: unet_in must be a channels_last [G*B, {C}, {H}, {W}] tensor, "
+        raise _C.LoraB200Error(f"sample_init: unet_in must be a channels_last [G*B, {Cu}, {H}, {W}] tensor, "
                                f"got {tuple(unet_in.shape)}")
     if (table.dtype != torch.float32 or table.dim() != 2 or table.shape[1] != 8 or not table.is_contiguous()
             or noise.dtype != torch.float32 or tuple(noise.shape) != (table.shape[0], B, C, H, W)
             or not noise.is_contiguous()):
-        raise _C.LoraB200Error("sample_step: table must be fp32 [rows, 8] and noise fp32 [rows, B, C, H, W]")
+        raise _C.LoraB200Error("sample_init: table must be fp32 [rows, 8] and noise fp32 [rows, B, C, H, W]")
     if step_index.dtype != torch.int32 or counter.dtype != torch.int32 or timestep.dtype != torch.float32:
-        raise _C.LoraB200Error("sample_step: step_index / counter int32 [1], timestep fp32 [1]")
-    sb = sc = sp = 0
-    mdt = vdt = _C.LB_F32
-    vcl = 0
-    if not init:
-        if model_out is None or tuple(model_out.shape) != (G * B, C, H, W):
-            raise _C.LoraB200Error(f"sample_step: model_out must be [{G * B}, {C}, {H}, {W}]")
-        sb, sc, sp = _dense_hw_strides(model_out, "model_out")
-        mdt = dtype_code(model_out.dtype)
-        if vae_in is None or tuple(vae_in.shape) != (B, C, H, W):
-            raise _C.LoraB200Error(f"sample_step: vae_in must be [{B}, {C}, {H}, {W}]")
-        vcl = int(not vae_in.is_contiguous())
-        if vcl and not vae_in.is_contiguous(memory_format=torch.channels_last):
-            raise _C.LoraB200Error("sample_step: vae_in must be contiguous or channels_last")
-        vdt = dtype_code(vae_in.dtype)
-        if guidance is None or guidance.dtype != torch.float32:
-            raise _C.LoraB200Error("sample_step: guidance must be a float32 [1] tensor")
-    check(_C.lib.lb_sample_step(ptr(model_out), mdt, sb, sc, sp, G, ptr(x), ptr(noise), ptr(table), table.shape[0],
-                                ptr(guidance), ptr(step_index), ptr(counter), ptr(unet_in),
-                                dtype_code(unet_in.dtype), ptr(timestep), ptr(vae_in), vdt, vcl, 1.0 / float(vae_scaling),
-                                B, C, H, W, int(init), stream_ptr()), "lb_sample_step")
+        raise _C.LoraB200Error("sample_init: step_index / counter int32 [1], timestep fp32 [1]")
+    mom, sb, sc, sp, md, pe, ed = None, 0, 0, 0, _C.LB_F32, None, _C.LB_F32
+    if moments is not None:
+        if tuple(moments.shape) != (B, 2 * C, H, W):
+            raise _C.LoraB200Error(f"sample_init: moments must be [{B}, {2 * C}, {H}, {W}], got {tuple(moments.shape)}")
+        if posterior_noise is None or tuple(posterior_noise.shape) != (B, C, H, W):
+            raise _C.LoraB200Error(f"sample_init: posterior_noise must be [{B}, {C}, {H}, {W}]")
+        if posterior_noise.dtype not in (moments.dtype, torch.float32) or not posterior_noise.is_contiguous():
+            raise _C.LoraB200Error("sample_init: posterior_noise must be contiguous, in the moments' dtype or fp32")
+        mom, (sb, sc, sp) = _moments_strides(moments)
+        md, pe, ed = dtype_code(mom.dtype), posterior_noise, dtype_code(posterior_noise.dtype)
+    if mask is not None:
+        if moments is None:
+            raise _C.LoraB200Error("sample_init: the inpainting mask needs the masked image's moments")
+        if mask.dtype != torch.uint8 or tuple(mask.shape) != (B, 8 * H, 8 * W) or not mask.is_contiguous():
+            raise _C.LoraB200Error(f"sample_init: mask must be a contiguous uint8 [{B}, {8 * H}, {8 * W}] tensor")
+    check(_C.lib.lb_sample_init(ptr(mom), md, sb, sc, sp, ptr(pe), ed, float(scaling), ptr(mask), ptr(noise),
+                                ptr(table), table.shape[0], ptr(x), ptr(step_index), ptr(counter), ptr(unet_in),
+                                dtype_code(unet_in.dtype), Cu, ptr(timestep), G, B, C, H, W, stream_ptr()),
+          "lb_sample_init")
     ops._count()
+
+
+def pixels_ingest_inpaint(pixels: torch.Tensor, mask: torch.Tensor, out_dtype: torch.dtype,
+                          channels_last: bool = True) -> torch.Tensor:
+    """The inpainting pipeline's masked image, one launch (lb_pixels_ingest_inpaint): [B, 3, H, W] of
+    `out_dtype`, channels_last or contiguous NCHW, = image * (mask < 0.5) with image = uint8 / 127.5 - 1
+    and mask = (uint8 / 255 >= 0.5) (prepare_mask_and_masked_image). pixels: uint8 [B, H, W, 3]; mask:
+    uint8 [B, H, W], 0..255 -- not pixels_ingest's 0 / 1 training mask."""
+    if not pixels.is_cuda:
+        raise _C.LoraB200Error("pixels_ingest_inpaint needs CUDA tensors (no CPU path)")
+    if pixels.dtype != torch.uint8 or pixels.dim() != 4 or pixels.shape[3] != 3:
+        raise _C.LoraB200Error(f"pixels must be uint8 [B, H, W, 3], got {pixels.dtype} {tuple(pixels.shape)}")
+    B, H, W, _ = pixels.shape
+    if mask.dtype != torch.uint8 or tuple(mask.shape) != (B, H, W):
+        raise _C.LoraB200Error(f"mask must be uint8 [{B}, {H}, {W}], got {mask.dtype} {tuple(mask.shape)}")
+    px, m = pixels.contiguous(), mask.contiguous()
+    fmt = torch.channels_last if channels_last else torch.contiguous_format
+    xm = torch.empty((B, 3, H, W), device=pixels.device, dtype=out_dtype, memory_format=fmt)
+    check(_C.lib.lb_pixels_ingest_inpaint(ptr(px), ptr(m), ptr(xm), dtype_code(out_dtype), int(channels_last),
+                                          B, H, W, stream_ptr()), "lb_pixels_ingest_inpaint")
+    ops._count()
+    return xm
 
 
 def pixels_emit(image: torch.Tensor, out: torch.Tensor):

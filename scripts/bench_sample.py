@@ -1,9 +1,13 @@
 """Sampling throughput: LoraSampler's graph replay, its eager path and the pipeline-style oracle loop
 (oracle/sample_ref.py), alternated in one process, on full-size host models with LoRA r=4 on the UNet
 and the text encoder, bf16 autocast, guidance 7:
-  SD1.5 512 px, Euler-ancestral, 50 steps, batch 1 and 4;  SD2.1 768-v, DDIM, 50 steps, batch 1.
+  SD1.5 512 px, Euler-ancestral, 50 steps, batch 1 and 4;  SD2.1 768-v, DDIM, 50 steps, batch 1;
+  SD1.5 512 px img2img, Euler-ancestral, 50 steps at strength 0.75 (37 steps run), batch 1;
+  SD1.5-inpainting shape (a 9-channel UNet), 512 px, Euler-ancestral, 50 steps, batch 1.
 Prints per workload: s/image and ms per denoising step, the decode's share of a graph-replayed call,
 liblora_b200 launches per denoising step (ops counter), peak memory, and the GPU's name and power limit.
+The img2img and inpainting workloads also print the share of graph A (text encoder, image ingest, VAE
+encoder and lb_sample_init) in a graph-replayed call, and the denoising steps run.
 Weights are random: the timings do not depend on them."""
 import argparse
 import json
@@ -28,7 +32,7 @@ def _gpu():
     return name, power
 
 
-def _models(sd2: bool):
+def _models(sd2: bool, in_channels: int = 4):
     import lora_b200 as L
     from lora_b200.host.clip import build_text_encoder
     from lora_b200.host.unet_sd15 import UNet2DConditionModel, UNetConfig
@@ -37,7 +41,9 @@ def _models(sd2: bool):
     import copy
     torch.manual_seed(0)
     with torch.device("cuda"):
-        unet = UNet2DConditionModel(UNetConfig.sd21() if sd2 else UNetConfig())
+        ucfg = UNetConfig.sd21() if sd2 else UNetConfig()
+        ucfg.in_channels = in_channels
+        unet = UNet2DConditionModel(ucfg)
         text = build_text_encoder(sd2=sd2)
         vae = AutoencoderKL(VAEConfig.sd(), with_decoder=True)
     for m in (unet, text, vae):
@@ -61,66 +67,95 @@ def _time(fn, reps):
     return (time.perf_counter() - t0) / reps
 
 
-def run(name, sd2, B, res, sched, pred, n, reps):
+def run(name, sd2, B, res, sched, pred, n, reps, task="txt2img", strength=0.75):
     import lora_b200 as L
     from lora_b200 import ops
+    from lora_b200.host import schedulers
     from lora_b200.sample import LoraSampler, SamplerConfig
+    from oracle import sample_image_ref as RI
     from oracle import sample_ref as R
-    unet, text, vae, unet_r, text_r = _models(sd2)
+    unet, text, vae, unet_r, text_r = _models(sd2, 9 if task == "inpaint" else 4)
     L.set_grouping(True)
     lat = (B, 4, res // 8, res // 8)
     cfg = dict(scheduler=sched, prediction_type=pred, num_inference_steps=n, max_steps=n, guidance_scale=7.0,
-               autocast_dtype=torch.bfloat16)
+               autocast_dtype=torch.bfloat16, task=task, strength=strength)
     sg = LoraSampler(unet, text, vae, SamplerConfig(**cfg), latent_shape=lat)
     se = LoraSampler(unet, text, vae, SamplerConfig(use_cuda_graph=False, **cfg), latent_shape=lat)
     ids = torch.randint(0, text.config.vocab_size, (B, 77), device="cuda")
     neg = torch.randint(0, text.config.vocab_size, (B, 77), device="cuda")
+    g = torch.Generator().manual_seed(0)
+    image = torch.randint(0, 256, (B, res, res, 3), generator=g, dtype=torch.uint8).cuda()
+    mask = torch.zeros(B, res, res, dtype=torch.uint8)
+    mask[:, res // 4:3 * res // 4, res // 4:3 * res // 4] = 255
+    mask = mask.cuda()
+    extra = {"txt2img": {}, "img2img": dict(image=image), "inpaint": dict(image=image, mask_image=mask)}[task]
+    k = n - schedulers.t_start(n, strength) if task == "img2img" else n        # denoising steps run
     torch.cuda.reset_peak_memory_stats()
     sg.prepare()
-    sg.sample(ids, neg)
-    se.sample(ids, neg)
-    noise = sg.noise[:n + 1].clone()
-    oracle = lambda: R.sample(unet_r, text_r, vae, R.make_scheduler(sched, pred), n, ids, neg, noise, 7.0,  # noqa: E731
-                              dtype=torch.float32, autocast_dtype=torch.bfloat16)
+    sg.sample(ids, neg, **extra)
+    se.sample(ids, neg, **extra)
+    noise = sg.noise[:k + 1].clone()
+    if task == "txt2img":
+        oracle = lambda: R.sample(unet_r, text_r, vae, R.make_scheduler(sched, pred), n, ids, neg, noise, 7.0,  # noqa: E731
+                                  dtype=torch.float32, autocast_dtype=torch.bfloat16)
+    elif task == "img2img":
+        peps = sg.posterior_noise.clone()
+        oracle = lambda: RI.sample_img2img(unet_r, text_r, vae, RI.make_scheduler(sched, pred), n, strength, ids,  # noqa: E731
+                                           neg, image, noise, peps, 7.0, dtype=torch.float32,
+                                           autocast_dtype=torch.bfloat16)
+    else:
+        peps = sg.posterior_noise.clone()
+        oracle = lambda: RI.sample_inpaint(unet_r, text_r, vae, RI.make_scheduler(sched, pred), n, ids, neg,  # noqa: E731
+                                           image, mask, noise, peps, 7.0, dtype=torch.float32,
+                                           autocast_dtype=torch.bfloat16)
     oracle()
     t = {"graph": [], "eager": [], "oracle": []}
     for _ in range(reps):                      # alternated: the three paths see the same machine state
-        t["graph"].append(_time(lambda: sg.sample(ids, neg), 1))
-        t["eager"].append(_time(lambda: se.sample(ids, neg), 1))
+        t["graph"].append(_time(lambda: sg.sample(ids, neg, **extra), 1))
+        t["eager"].append(_time(lambda: se.sample(ids, neg, **extra), 1))
         t["oracle"].append(_time(oracle, 1))
-    gc = sg._graphs[2][2]
+    ga, _, gc = sg._graphs[2]
     decode = _time(gc.replay, 3)
+    graph_a = _time(ga.replay, 3)
     with torch.no_grad():
         unet.eval()
         c0 = ops.LAUNCH_COUNT
         se._body_b(2)
         launches = ops.LAUNCH_COUNT - c0
         unet.train()
-    med = {k: sorted(v)[len(v) // 2] for k, v in t.items()}
-    return {"workload": name, "batch": B, "steps": n,
-            **{f"{k}_s_per_image": round(v / B, 4) for k, v in med.items()},
-            **{f"{k}_ms_per_step": round(1e3 * v / n, 3) for k, v in med.items()},
-            "decode_share_graph": round(decode / med["graph"], 4),
-            "launches_per_step": launches,
-            "peak_mib": round(torch.cuda.max_memory_allocated() / 2 ** 20)}
+    med = {key: sorted(v)[len(v) // 2] for key, v in t.items()}
+    out = {"workload": name, "batch": B, "steps": n,
+           **{f"{key}_s_per_image": round(v / B, 4) for key, v in med.items()},
+           **{f"{key}_ms_per_step": round(1e3 * v / k, 3) for key, v in med.items()},
+           "decode_share_graph": round(decode / med["graph"], 4),
+           "launches_per_step": launches,
+           "peak_mib": round(torch.cuda.max_memory_allocated() / 2 ** 20)}
+    if task != "txt2img":
+        out.update(task=task, denoising_steps=k, graph_a_share_graph=round(graph_a / med["graph"], 4))
+        if task == "img2img":
+            out["strength"] = strength
+    return out
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--steps", type=int, default=50)
-    ap.add_argument("--only", default=None, help="run one workload (sd15_b1, sd15_b4, sd21_768v)")
+    ap.add_argument("--only", default=None,
+                    help="run one workload (sd15_b1, sd15_b4, sd21_768v, sd15_img2img, sd15_inpaint)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_sample.py needs a CUDA device")
     name, power = _gpu()
     work = [("sd15_b1", False, 1, 512, "euler_ancestral", "epsilon"),
             ("sd15_b4", False, 4, 512, "euler_ancestral", "epsilon"),
-            ("sd21_768v", True, 1, 768, "ddim", "v_prediction")]
+            ("sd21_768v", True, 1, 768, "ddim", "v_prediction"),
+            ("sd15_img2img", False, 1, 512, "euler_ancestral", "epsilon", "img2img"),
+            ("sd15_inpaint", False, 1, 512, "euler_ancestral", "epsilon", "inpaint")]
     for w in work:
         if a.only and w[0] != a.only:
             continue
-        r = run(*w, a.steps, a.reps)
+        r = run(*w[:6], a.steps, a.reps, *w[6:])
         r.update(gpu=name, power_limit=power)
         print(json.dumps(r), flush=True)
 
