@@ -575,6 +575,22 @@ int lb_sample_step_ch(const void* model_out, int model_dtype, long long stride_b
                       int unet_channels, float* timestep, void* vae_in, int vae_dtype, int vae_channels_last,
                       float vae_inv_scaling, int B, int C, int H, int W, int init, void* stream);
 
+/* lb_sample_step_ch for a multistep scheduler (DPM-Solver++(2M), host/schedulers.py), one launch. The
+ * arguments are lb_sample_step_ch's with x0_hist in place of noise and no init (the loop starts with
+ * lb_sample_step(init = 1) or lb_sample_init, which reset step_index and counter). Row 1 + i of the table
+ * is (a, b, d, s_next, t_next, last, p, q); x0_hist is fp32 NCHW [B, C, H, W]:
+ *   m = m_u + g (m_c - m_u)  (G = 1: m = model_out);  x0 = p x + q m;  x' = a x + b x0 + d x0_hist
+ *   (x0_hist is not read when d = 0);  x0_hist = x0;  x = x'
+ *   unet_in channels [0, C) of every half = s_next * x';  *timestep = t_next;  last: vae_in = vae_inv_scaling x'
+ * Each element of x and x0_hist is read and written by the thread that owns it, so both update in place.
+ * The step index advances as in lb_sample_step. Allocates nothing; capturable. Refusals as
+ * lb_sample_step_ch's (x0_hist == NULL: LB_ERR_SHAPE). */
+int lb_sample_step_ms(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                      long long stride_p, int G, float* x, float* x0_hist, const float* table, int table_rows,
+                      const float* guidance, int* step_index, unsigned int* counter, void* unet_in, int unet_dtype,
+                      int unet_channels, float* timestep, void* vae_in, int vae_dtype, int vae_channels_last,
+                      float vae_inv_scaling, int B, int C, int H, int W, void* stream);
+
 /* The start of an img2img or inpainting sampling loop, one launch (diffusers' StableDiffusionImg2Img-
  * Pipeline.prepare_latents / StableDiffusionInpaintPipeline.prepare_mask_latents). Row 0 of the table is
  * (c_noise, s_start, t_start, c_lat, ...) (host/schedulers.pack_table); noise slice 0 is z_0.

@@ -18,7 +18,9 @@
 //                         first UNet input from the initial noise
 //   lb_sample_step_ch     the same into a UNet input of more channels than the latents (the 9-channel
 //                         inpainting UNet): only the latent channels are written
-//   lb_sample_init        the start of an img2img or inpainting loop: the posterior sample of the encoded
+//   lb_sample_step_ms     the same for a multistep scheduler (DPM-Solver++(2M)): the data prediction, the
+//                         update from it and the previous step's, and that history kept in place
+//   lb_sample_init       the start of an img2img or inpainting loop: the posterior sample of the encoded
 //                         image, scheduler.add_noise at the first kept timestep, the first UNet input,
 //                         and for inpainting the constant mask and masked-image channels
 //   lb_pixels_ingest_inpaint  uint8 image + uint8 0..255 mask -> the inpainting pipeline's masked image
@@ -261,13 +263,20 @@ masked_mse_kernel(const void* __restrict__ pred, int pred_dt, long long sb, long
 // init: x = z_0 * init_noise_sigma (row 0: (sigma, s_0, t_0)), the first UNet input and timestep, and the
 // step index and arrival counter reset. Every block reads *step_index; the last block to arrive
 // advances it, so one captured launch replays as every step in turn.
+// MS (the multistep family, lb_sample_step_ms; no init, no noise): row 1 + i is
+// (a, b, d, s_next, t_next, last, p, q) and, with h = x0_hist [B, C, P] fp32 NCHW,
+//   x0 = p x + q m_hat        (the data prediction: convert_model_output of DPM-Solver++)
+//   x' = a x + b x0 + d h     (h unread when d = 0);  then h = x0, in place
+// Each element of x and h is read and written by the one thread that owns it.
+template <bool MS>
 __global__ void __launch_bounds__(256)
 sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long sc, long long sp, int G,
-                   float* __restrict__ x, const float* __restrict__ noise, const float* __restrict__ table,
-                   int rows, const float* __restrict__ guidance, int* __restrict__ step_index,
-                   unsigned int* __restrict__ counter, void* __restrict__ unet_in, int udt, int Cu,
-                   float* __restrict__ timestep, void* __restrict__ vae_in, int vdt, int vae_cl, float vae_inv_scaling,
-                   int B, int C, int P, int init) {
+                   float* __restrict__ x, const float* __restrict__ noise, float* __restrict__ x0_hist,
+                   const float* __restrict__ table, int rows, const float* __restrict__ guidance,
+                   int* __restrict__ step_index, unsigned int* __restrict__ counter, void* __restrict__ unet_in,
+                   int udt, int Cu, float* __restrict__ timestep, void* __restrict__ vae_in, int vdt, int vae_cl,
+                   float vae_inv_scaling, int B, int C, int P, int init_arg) {
+  const bool init = !MS && init_arg;
   __shared__ int s_row;
   __shared__ bool last_block;
   if (threadIdx.x == 0) {
@@ -280,15 +289,16 @@ sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long
   const long long slice = static_cast<long long>(B) * C * P;
   if (i < static_cast<long long>(B) * P) {
     const int b = static_cast<int>(i / P), px = static_cast<int>(i % P);
-    float s_next, alpha = 0.f, beta = 0.f, gamma = 0.f, g = 0.f;
+    float s_next, alpha = 0.f, beta = 0.f, gamma = 0.f, g = 0.f, p = 0.f, q = 0.f;
     bool last = false;
     if (init) {
       s_next = row[1];
     } else {
       alpha = row[0]; beta = row[1]; gamma = row[2]; s_next = row[3]; last = row[5] != 0.f;
       g = *guidance;
+      if (MS) { p = row[6]; q = row[7]; }
     }
-    const float* z = noise + (init ? 0ll : s_row * slice);
+    const float* z = MS ? nullptr : noise + (init ? 0ll : s_row * slice);
     for (int c = 0; c < C; ++c) {
       const long long xi = (static_cast<long long>(b) * C + c) * P + px;
       float xn;
@@ -300,8 +310,16 @@ sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long
           const float mc = ld_any(mo, (B + b) * sb + c * sc + px * sp, mdt);
           m = fmaf(g, mc - m, m);
         }
-        xn = fmaf(alpha, x[xi], beta * m);
-        if (gamma != 0.f) xn = fmaf(gamma, z[xi], xn);
+        if (MS) {
+          const float xc = x[xi];
+          const float x0 = fmaf(p, xc, q * m);
+          xn = fmaf(alpha, xc, beta * x0);
+          if (gamma != 0.f) xn = fmaf(gamma, x0_hist[xi], xn);
+          x0_hist[xi] = x0;
+        } else {
+          xn = fmaf(alpha, x[xi], beta * m);
+          if (gamma != 0.f) xn = fmaf(gamma, z[xi], xn);
+        }
       }
       x[xi] = xn;
       const float u = __fmul_rn(s_next, xn);
@@ -511,25 +529,27 @@ extern "C" int lb_pixels_ingest_inpaint(const void* pixels, const unsigned char*
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
+// MS: the multistep launch (lb_sample_step_ms): x0_hist in place of noise, never init
+template <bool MS>
 static int launch_sample_step(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
-                              long long stride_p, int G, float* x, const float* noise, const float* table,
-                              int table_rows, const float* guidance, int* step_index, unsigned int* counter,
-                              void* unet_in, int unet_dtype, int unet_channels, float* timestep, void* vae_in,
-                              int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B, int C, int H,
-                              int W, int init, void* stream) {
+                              long long stride_p, int G, float* x, const float* noise, float* x0_hist,
+                              const float* table, int table_rows, const float* guidance, int* step_index,
+                              unsigned int* counter, void* unet_in, int unet_dtype, int unet_channels,
+                              float* timestep, void* vae_in, int vae_dtype, int vae_channels_last,
+                              float vae_inv_scaling, int B, int C, int H, int W, int init, void* stream) {
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || (G != 1 && G != 2) || table_rows < 2) return LB_ERR_SHAPE;
   if (unet_channels < C) return LB_ERR_SHAPE;
   if (!float_dtype(unet_dtype) || !float_dtype(vae_dtype) || (!init && !float_dtype(model_dtype)))
     return LB_ERR_DTYPE;
-  if (x == nullptr || noise == nullptr || table == nullptr || step_index == nullptr || counter == nullptr ||
-      unet_in == nullptr || timestep == nullptr)
+  if (x == nullptr || (MS ? x0_hist == nullptr : noise == nullptr) || table == nullptr || step_index == nullptr ||
+      counter == nullptr || unet_in == nullptr || timestep == nullptr)
     return LB_ERR_SHAPE;
   if (!init && (model_out == nullptr || guidance == nullptr || vae_in == nullptr || !(vae_inv_scaling > 0.f)))
     return LB_ERR_SHAPE;
   const long long n = static_cast<long long>(B) * H * W;
-  sample_step_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows, guidance, step_index,
-      counter, unet_in, unet_dtype, unet_channels, timestep, vae_in, vae_dtype, vae_channels_last != 0,
+  sample_step_kernel<MS><<<static_cast<int>((n + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, x0_hist, table, table_rows, guidance,
+      step_index, counter, unet_in, unet_dtype, unet_channels, timestep, vae_in, vae_dtype, vae_channels_last != 0,
       vae_inv_scaling, B, C, H * W, init != 0);
   return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
@@ -540,9 +560,10 @@ extern "C" int lb_sample_step(const void* model_out, int model_dtype, long long 
                               void* unet_in, int unet_dtype, float* timestep, void* vae_in, int vae_dtype,
                               int vae_channels_last, float vae_inv_scaling, int B, int C, int H, int W, int init,
                               void* stream) {
-  return launch_sample_step(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows,
-                            guidance, step_index, counter, unet_in, unet_dtype, C, timestep, vae_in, vae_dtype,
-                            vae_channels_last, vae_inv_scaling, B, C, H, W, init, stream);
+  return launch_sample_step<false>(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, nullptr,
+                                   table, table_rows, guidance, step_index, counter, unet_in, unet_dtype, C,
+                                   timestep, vae_in, vae_dtype, vae_channels_last, vae_inv_scaling, B, C, H, W, init,
+                                   stream);
 }
 
 extern "C" int lb_sample_step_ch(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
@@ -551,9 +572,22 @@ extern "C" int lb_sample_step_ch(const void* model_out, int model_dtype, long lo
                                  void* unet_in, int unet_dtype, int unet_channels, float* timestep, void* vae_in,
                                  int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B, int C, int H,
                                  int W, int init, void* stream) {
-  return launch_sample_step(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, table, table_rows,
-                            guidance, step_index, counter, unet_in, unet_dtype, unet_channels, timestep, vae_in,
-                            vae_dtype, vae_channels_last, vae_inv_scaling, B, C, H, W, init, stream);
+  return launch_sample_step<false>(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, noise, nullptr,
+                                   table, table_rows, guidance, step_index, counter, unet_in, unet_dtype,
+                                   unet_channels, timestep, vae_in, vae_dtype, vae_channels_last, vae_inv_scaling, B,
+                                   C, H, W, init, stream);
+}
+
+extern "C" int lb_sample_step_ms(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                                 long long stride_p, int G, float* x, float* x0_hist, const float* table,
+                                 int table_rows, const float* guidance, int* step_index, unsigned int* counter,
+                                 void* unet_in, int unet_dtype, int unet_channels, float* timestep, void* vae_in,
+                                 int vae_dtype, int vae_channels_last, float vae_inv_scaling, int B, int C, int H,
+                                 int W, void* stream) {
+  return launch_sample_step<true>(model_out, model_dtype, stride_b, stride_c, stride_p, G, x, nullptr, x0_hist,
+                                  table, table_rows, guidance, step_index, counter, unet_in, unet_dtype,
+                                  unet_channels, timestep, vae_in, vae_dtype, vae_channels_last, vae_inv_scaling, B,
+                                  C, H, W, 0, stream);
 }
 
 extern "C" int lb_sample_init(const void* moments, int moments_dtype, long long stride_b, long long stride_c,

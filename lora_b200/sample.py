@@ -1,6 +1,6 @@
 """Sampling from LoRA-patched models: the denoising loop of diffusers' StableDiffusionPipeline
-(classifier-free guidance, Euler-ancestral or DDIM, the VAE decode and the uint8 post-processing) over
-the same host models and fused LoRA kernels the training steps use.
+(classifier-free guidance, Euler-ancestral, DDIM or DPM-Solver++(2M), the VAE decode and the uint8
+post-processing) over the same host models and fused LoRA kernels the training steps use.
 
     from lora_b200.sample import LoraSampler, SamplerConfig
     s = LoraSampler(unet, text_encoder, vae, SamplerConfig(scheduler="euler_ancestral", guidance_scale=7.0),
@@ -29,12 +29,17 @@ A `sample()` replays three CUDA graphs, with no host sync and no allocation betw
   B  one denoising step: the UNet at batch G*B, then lb_sample_step (guidance sum, the scheduler's update
      as folded coefficients, the next UNet input and timestep). Replayed N times: the step index lives
      on the device and the kernel advances it. img2img runs the last k = n - t_start steps of the
-     n-step schedule (host/schedulers.t_start: int(n * strength) steps), so B is replayed k times;
+     n-step schedule (host/schedulers.t_start: int(n * strength) steps), so B is replayed k times.
+     A multistep scheduler (DPM-Solver++(2M), "dpmsolver_multistep") runs lb_sample_step_ms in place of
+     lb_sample_step: it also keeps the previous step's data prediction in the static `x0_hist`;
   C  the VAE decoder and lb_pixels_emit.
 `use_cuda_graph=False` runs the same code eagerly. The number of steps (up to `max_steps`), the
 scheduler, the guidance scale, the seed, the strength, the image and the mask may change per call:
 they rewrite device tables and buffers. A guidance
 scale <= 1 runs without the unconditional half (G = 1), as the pipeline does; that is a capture of its own.
+So is each scheduler family (schedulers.family: "single-step" for Euler-ancestral and DDIM, "multistep"
+for DPM-Solver++): switching between Euler-ancestral and DDIM costs no capture, the first call of the
+other family one, and later calls none.
 The graphs are captured again only when something baked into a launch changes: a site's scale, a
 selector, the set of sites or their parameter storage, the grouping policy (`captures` counts them).
 
@@ -52,14 +57,15 @@ import torch.nn as nn
 
 from . import _C, ops
 from .host import schedulers
-from .step_ops import pixels_emit, pixels_ingest, pixels_ingest_inpaint, sample_init, sample_step, sample_step_ch
+from .step_ops import (pixels_emit, pixels_ingest, pixels_ingest_inpaint, sample_init, sample_step, sample_step_ch,
+                       sample_step_ms)
 
 _SITE_NAMES = ("LoraInjectedLinear", "LoraInjectedConv2d")
 
 
 @dataclass
 class SamplerConfig:
-    scheduler: str = "euler_ancestral"         # "euler_ancestral" | "ddim"
+    scheduler: str = "euler_ancestral"         # "euler_ancestral" | "ddim" | "dpmsolver_multistep"
     num_inference_steps: int = 50
     guidance_scale: float = 7.5
     prediction_type: str = "epsilon"           # the UNet's: "epsilon" | "v_prediction" (SD 2.x 768-v)
@@ -124,6 +130,7 @@ class LoraSampler:
         self.input_ids = torch.zeros((2 * B, seq_len), device=dev, dtype=torch.long)    # [negative ; prompt]
         self.noise = torch.zeros((rows, B, C, h, w), device=dev, dtype=torch.float32)
         self.latents = torch.zeros(latent_shape, device=dev, dtype=torch.float32)
+        self.x0_hist = torch.zeros(latent_shape, device=dev, dtype=torch.float32)      # multistep: last x0
         self.table = torch.zeros((rows, schedulers.TABLE_COLS), device=dev, dtype=torch.float32)
         self.guidance = torch.zeros(1, device=dev, dtype=torch.float32)
         self.step_index = torch.zeros(1, device=dev, dtype=torch.int32)
@@ -143,7 +150,7 @@ class LoraSampler:
             self.mask_image = torch.zeros((B, 8 * h, 8 * w), device=dev, dtype=torch.uint8)
         self._ehs = {}
         self._table_key = None
-        self._graphs = {}             # G -> (A, B, C)
+        self._graphs = {}             # (G, scheduler family) -> (A, B, C)
         self._fingerprint = None
         self._factor_bufs = []
         self.captures = 0
@@ -223,9 +230,13 @@ class LoraSampler:
                     self._counter, self.unet_in[G], self.timestep, self.cfg.vae_scaling,
                     mask=self.mask_image if task == "inpaint" else None)
 
-    def _body_b(self, G: int):
+    def _body_b(self, G: int, family: str = "single-step"):
         with self._autocast():
             out = self.unet(self.unet_in[G], self.timestep, self._ehs[G]).sample
+        if family == "multistep":
+            sample_step_ms(out, self.latents, self.x0_hist, self.table, self.guidance, self.step_index,
+                           self._counter, self.unet_in[G], self.timestep, self.vae_in, self.cfg.vae_scaling)
+            return
         step = sample_step_ch if self.cfg.task == "inpaint" else sample_step
         step(out, self.latents, self.noise, self.table, self.guidance, self.step_index, self._counter,
              self.unet_in[G], self.timestep, self.vae_in, self.cfg.vae_scaling)
@@ -233,20 +244,20 @@ class LoraSampler:
     def _body_c(self):
         pixels_emit(self.vae.decode(self.vae_in).sample, self.image)
 
-    def _run_eager(self, G: int, n: int):
+    def _run_eager(self, G: int, n: int, family: str = "single-step"):
         self._collect_factor_buffers()
         self._body_a(G)
         for _ in range(n):
-            self._body_b(G)
+            self._body_b(G, family)
         self._body_c()
 
     # ------------------------------------------------------------------ capture
-    def _capture(self, G: int):
+    def _capture(self, G: int, family: str):
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(max(1, self.cfg.graph_warmup)):
-                self._run_eager(G, 1)
+                self._run_eager(G, 1, family)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self._collect_factor_buffers()
@@ -255,22 +266,22 @@ class LoraSampler:
             self._body_a(G)
         gb = torch.cuda.CUDAGraph()
         with torch.cuda.graph(gb, pool=ga.pool()):
-            self._body_b(G)
+            self._body_b(G, family)
         gc = torch.cuda.CUDAGraph()
         with torch.cuda.graph(gc, pool=ga.pool()):
             self._body_c()
         torch.cuda.synchronize()
-        self._graphs[G] = (ga, gb, gc)
+        self._graphs[(G, family)] = (ga, gb, gc)
         self.captures += 1
 
-    def _graphs_for(self, G: int):
+    def _graphs_for(self, G: int, family: str):
         fp = self._fingerprint_now()
         if fp != self._fingerprint:
             self._graphs.clear()
             self._fingerprint = fp
-        if G not in self._graphs:
-            self._capture(G)
-        return self._graphs[G]
+        if (G, family) not in self._graphs:
+            self._capture(G, family)
+        return self._graphs[(G, family)]
 
     # ------------------------------------------------------------------ modes
     def _enter_eval(self):
@@ -338,7 +349,7 @@ class LoraSampler:
         try:
             with torch.no_grad():
                 self._set_table(sched, n, start)
-                self._graphs_for(2 if g > 1.0 else 1)
+                self._graphs_for(2 if g > 1.0 else 1, schedulers.family(sched))
         finally:
             self._restore_modes(saved)
 
@@ -354,6 +365,7 @@ class LoraSampler:
         n, sched, g, start = self._options(num_inference_steps, scheduler, guidance_scale, strength)
         k = n - start
         G = 2 if g > 1.0 else 1
+        family = schedulers.family(sched)
         B = self.latents.shape[0]
         if tuple(input_ids.shape) != tuple(self.input_ids[B:].shape):
             raise ValueError(f"input_ids of shape {tuple(input_ids.shape)}: the sampler takes "
@@ -375,13 +387,13 @@ class LoraSampler:
                     if self.cfg.task != "txt2img":
                         self.posterior_noise.normal_(generator=self.generator)
                 if self.cfg.use_cuda_graph:
-                    ga, gb, gc = self._graphs_for(G)
+                    ga, gb, gc = self._graphs_for(G, family)
                     ga.replay()
                     for _ in range(k):
                         gb.replay()
                     gc.replay()
                 else:
-                    self._run_eager(G, k)
+                    self._run_eager(G, k, family)
         finally:
             self._restore_modes(saved)
         return self.image

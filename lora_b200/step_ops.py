@@ -16,6 +16,8 @@ and the two ends of a sampling step (lora_b200/sample.py):
   sample_step       guidance sum + the scheduler's update (folded coefficients) + the next UNet input
                     and timestep (+ the decoder input on the last step); init=True: the first input
   sample_step_ch    the same into the 9-channel inpainting UNet's input (latent channels only)
+  sample_step_ms    the same for a multistep scheduler (DPM-Solver++(2M)): the data prediction x0, the
+                    update from it and the previous step's x0, and that history kept in a device buffer
   sample_init       the start of an img2img / inpainting loop: posterior sample, add_noise, the first
                     UNet input (+ the inpainting mask and masked-image latent channels)
   pixels_ingest_inpaint  uint8 image + 0..255 mask -> the inpainting pipeline's masked image
@@ -182,9 +184,9 @@ def _dense_hw_strides(t: torch.Tensor, what: str):
 
 
 def _sample_step_args(model_out, x, noise, table, guidance, step_index, counter, unet_in, timestep, vae_in,
-                      vae_scaling, init, unet_channels, what):
+                      vae_scaling, init, unet_channels, what, x0_hist=None):
     """The argument tuple of lb_sample_step / lb_sample_step_ch after sample_step's checks (unet_in has
-    `unet_channels` channels)."""
+    `unet_channels` channels). With x0_hist (lb_sample_step_ms) the history takes the noise's place."""
     if not x.is_cuda:
         raise _C.LoraB200Error(f"{what} needs CUDA tensors (no CPU path)")
     if not vae_scaling > 0.0:
@@ -198,9 +200,14 @@ def _sample_step_args(model_out, x, noise, table, guidance, step_index, counter,
             or not unet_in.is_contiguous(memory_format=torch.channels_last)):
         raise _C.LoraB200Error(f"{what}: unet_in must be a channels_last [G*B, {Cu}, {H}, {W}] tensor, "
                                f"got {tuple(unet_in.shape)}")
-    if (table.dtype != torch.float32 or table.dim() != 2 or table.shape[1] != 8 or not table.is_contiguous()
-            or noise.dtype != torch.float32 or tuple(noise.shape) != (table.shape[0], B, C, H, W)
-            or not noise.is_contiguous()):
+    if table.dtype != torch.float32 or table.dim() != 2 or table.shape[1] != 8 or not table.is_contiguous():
+        raise _C.LoraB200Error(f"{what}: table must be fp32 [rows, 8]" +
+                               ("" if x0_hist is not None else " and noise fp32 [rows, B, C, H, W]"))
+    if x0_hist is not None:
+        if x0_hist.dtype != torch.float32 or tuple(x0_hist.shape) != (B, C, H, W) or not x0_hist.is_contiguous():
+            raise _C.LoraB200Error(f"{what}: x0_hist must be a contiguous fp32 [{B}, {C}, {H}, {W}] tensor")
+        noise = x0_hist
+    elif noise.dtype != torch.float32 or tuple(noise.shape) != (table.shape[0], B, C, H, W) or not noise.is_contiguous():
         raise _C.LoraB200Error(f"{what}: table must be fp32 [rows, 8] and noise fp32 [rows, B, C, H, W]")
     if step_index.dtype != torch.int32 or counter.dtype != torch.int32 or timestep.dtype != torch.float32:
         raise _C.LoraB200Error(f"{what}: step_index / counter int32 [1], timestep fp32 [1]")
@@ -258,6 +265,27 @@ def sample_step_ch(model_out: Optional[torch.Tensor], x: torch.Tensor, noise: to
     head, tail = _sample_step_args(model_out, x, noise, table, guidance, step_index, counter, unet_in, timestep,
                                    vae_in, vae_scaling, init, Cu, "sample_step_ch")
     check(_C.lib.lb_sample_step_ch(*head, Cu, *tail), "lb_sample_step_ch")
+    ops._count()
+
+
+def sample_step_ms(model_out: torch.Tensor, x: torch.Tensor, x0_hist: torch.Tensor, table: torch.Tensor,
+                   guidance: torch.Tensor, step_index: torch.Tensor, counter: torch.Tensor, unet_in: torch.Tensor,
+                   timestep: torch.Tensor, vae_in: torch.Tensor, vae_scaling: float):
+    """One launch of lb_sample_step_ms, in place on preallocated buffers (nothing is allocated: capturable).
+
+    The arguments of sample_step_ch with x0_hist (fp32 contiguous [B, C, H, W]) in place of noise and no
+    init: the loop starts with sample_step(init=True) or sample_init. table rows are
+    (a, b, d, s_next, t_next, last, p, q) (host/schedulers.pack_table for a multistep scheduler):
+    x0 = p x + q m_hat, x = a x + b x0 + d x0_hist (x0_hist unread when d = 0), then x0_hist = x0.
+    unet_in may have more channels than the latents; only channels [0, C) are written."""
+    Cu = unet_in.shape[1] if unet_in.dim() == 4 else -1
+    if Cu < x.shape[1]:
+        raise _C.LoraB200Error(f"sample_step_ms: unet_in has {Cu} channels, fewer than the latents' {x.shape[1]}")
+    if x0_hist is None:
+        raise _C.LoraB200Error("sample_step_ms needs the x0_hist buffer")
+    head, tail = _sample_step_args(model_out, x, None, table, guidance, step_index, counter, unet_in, timestep,
+                                   vae_in, vae_scaling, False, Cu, "sample_step_ms", x0_hist=x0_hist)
+    check(_C.lib.lb_sample_step_ms(*head, Cu, *tail[:-2], tail[-1]), "lb_sample_step_ms")   # no init argument
     ops._count()
 
 

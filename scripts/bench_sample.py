@@ -3,11 +3,16 @@
 and the text encoder, bf16 autocast, guidance 7:
   SD1.5 512 px, Euler-ancestral, 50 steps, batch 1 and 4;  SD2.1 768-v, DDIM, 50 steps, batch 1;
   SD1.5 512 px img2img, Euler-ancestral, 50 steps at strength 0.75 (37 steps run), batch 1;
-  SD1.5-inpainting shape (a 9-channel UNet), 512 px, Euler-ancestral, 50 steps, batch 1.
-Prints per workload: s/image and ms per denoising step, the decode's share of a graph-replayed call,
+  SD1.5-inpainting shape (a 9-channel UNet), 512 px, Euler-ancestral, 50 steps, batch 1;
+  DPM-Solver++(2M): SD1.5 512 px 20 and 25 steps, SD2.1 768-v 25 steps, SD1.5 512 px img2img 25 steps at
+  strength 0.75 (18 steps run), batch 1.
+Prints per workload: s/image and ms per denoising step (the call's time over its steps), the time of
+one replay of the denoising-step graph alone, the decode's share of a graph-replayed call,
 liblora_b200 launches per denoising step (ops counter), peak memory, and the GPU's name and power limit.
 The img2img and inpainting workloads also print the share of graph A (text encoder, image ingest, VAE
-encoder and lb_sample_init) in a graph-replayed call, and the denoising steps run.
+encoder and lb_sample_init) in a graph-replayed call, and the denoising steps run. The DPM-Solver++
+workloads also print the peak memory once the same graph sampler holds the captures of both scheduler
+families (one Euler-ancestral call after the timed ones).
 Weights are random: the timings do not depend on them."""
 import argparse
 import json
@@ -67,6 +72,13 @@ def _time(fn, reps):
     return (time.perf_counter() - t0) / reps
 
 
+def _ref_scheduler(mod, sched, pred):
+    """The oracle scheduler of that name: oracle/sample_dpm_ref.py's DPM-Solver++, otherwise oracle module
+    `mod`'s (sample_ref or sample_image_ref)."""
+    from oracle.sample_dpm_ref import RefDPMSolverMultistep
+    return RefDPMSolverMultistep(pred) if sched == "dpmsolver_multistep" else mod.make_scheduler(sched, pred)
+
+
 def run(name, sd2, B, res, sched, pred, n, reps, task="txt2img", strength=0.75):
     import lora_b200 as L
     from lora_b200 import ops
@@ -96,16 +108,16 @@ def run(name, sd2, B, res, sched, pred, n, reps, task="txt2img", strength=0.75):
     se.sample(ids, neg, **extra)
     noise = sg.noise[:k + 1].clone()
     if task == "txt2img":
-        oracle = lambda: R.sample(unet_r, text_r, vae, R.make_scheduler(sched, pred), n, ids, neg, noise, 7.0,  # noqa: E731
+        oracle = lambda: R.sample(unet_r, text_r, vae, _ref_scheduler(R, sched, pred), n, ids, neg, noise, 7.0,  # noqa: E731
                                   dtype=torch.float32, autocast_dtype=torch.bfloat16)
     elif task == "img2img":
         peps = sg.posterior_noise.clone()
-        oracle = lambda: RI.sample_img2img(unet_r, text_r, vae, RI.make_scheduler(sched, pred), n, strength, ids,  # noqa: E731
+        oracle = lambda: RI.sample_img2img(unet_r, text_r, vae, _ref_scheduler(RI, sched, pred), n, strength, ids,  # noqa: E731
                                            neg, image, noise, peps, 7.0, dtype=torch.float32,
                                            autocast_dtype=torch.bfloat16)
     else:
         peps = sg.posterior_noise.clone()
-        oracle = lambda: RI.sample_inpaint(unet_r, text_r, vae, RI.make_scheduler(sched, pred), n, ids, neg,  # noqa: E731
+        oracle = lambda: RI.sample_inpaint(unet_r, text_r, vae, _ref_scheduler(RI, sched, pred), n, ids, neg,  # noqa: E731
                                            image, mask, noise, peps, 7.0, dtype=torch.float32,
                                            autocast_dtype=torch.bfloat16)
     oracle()
@@ -114,22 +126,32 @@ def run(name, sd2, B, res, sched, pred, n, reps, task="txt2img", strength=0.75):
         t["graph"].append(_time(lambda: sg.sample(ids, neg, **extra), 1))
         t["eager"].append(_time(lambda: se.sample(ids, neg, **extra), 1))
         t["oracle"].append(_time(oracle, 1))
-    ga, _, gc = sg._graphs[2]
+    family = schedulers.family(sched)
+    ga, gb, gc = sg._graphs[(2, family)]
     decode = _time(gc.replay, 3)
     graph_a = _time(ga.replay, 3)
+    # graph B alone (the UNet forward and the one step launch), replayed as many times as a call does; the
+    # step index runs past the table, whose last row the kernel then repeats: the same work per replay
+    denoise_step = _time(gb.replay, k)
     with torch.no_grad():
         unet.eval()
         c0 = ops.LAUNCH_COUNT
-        se._body_b(2)
+        se._body_b(2, family)
         launches = ops.LAUNCH_COUNT - c0
         unet.train()
     med = {key: sorted(v)[len(v) // 2] for key, v in t.items()}
     out = {"workload": name, "batch": B, "steps": n,
            **{f"{key}_s_per_image": round(v / B, 4) for key, v in med.items()},
            **{f"{key}_ms_per_step": round(1e3 * v / k, 3) for key, v in med.items()},
+           "graph_b_ms_per_replay": round(1e3 * denoise_step, 3),
            "decode_share_graph": round(decode / med["graph"], 4),
            "launches_per_step": launches,
            "peak_mib": round(torch.cuda.max_memory_allocated() / 2 ** 20)}
+    if family == "multistep":
+        out["scheduler"] = sched
+        sg.sample(ids, neg, scheduler="euler_ancestral", **extra)          # the other family's captures
+        torch.cuda.synchronize()
+        out.update(captures=sg.captures, peak_mib_both_families=round(torch.cuda.max_memory_allocated() / 2 ** 20))
     if task != "txt2img":
         out.update(task=task, denoising_steps=k, graph_a_share_graph=round(graph_a / med["graph"], 4))
         if task == "img2img":
@@ -142,7 +164,8 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--only", default=None,
-                    help="run one workload (sd15_b1, sd15_b4, sd21_768v, sd15_img2img, sd15_inpaint)")
+                    help="comma-separated workloads (sd15_b1, sd15_b4, sd21_768v, sd15_img2img, sd15_inpaint, "
+                         "sd15_dpm20, sd15_dpm25, sd21_768v_dpm25, sd15_img2img_dpm25)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_sample.py needs a CUDA device")
@@ -151,11 +174,17 @@ def main():
             ("sd15_b4", False, 4, 512, "euler_ancestral", "epsilon"),
             ("sd21_768v", True, 1, 768, "ddim", "v_prediction"),
             ("sd15_img2img", False, 1, 512, "euler_ancestral", "epsilon", "img2img"),
-            ("sd15_inpaint", False, 1, 512, "euler_ancestral", "epsilon", "inpaint")]
+            ("sd15_inpaint", False, 1, 512, "euler_ancestral", "epsilon", "inpaint"),
+            ("sd15_dpm20", False, 1, 512, "dpmsolver_multistep", "epsilon", "txt2img", 20),
+            ("sd15_dpm25", False, 1, 512, "dpmsolver_multistep", "epsilon", "txt2img", 25),
+            ("sd21_768v_dpm25", True, 1, 768, "dpmsolver_multistep", "v_prediction", "txt2img", 25),
+            ("sd15_img2img_dpm25", False, 1, 512, "dpmsolver_multistep", "epsilon", "img2img", 25)]
+    only = set(a.only.split(",")) if a.only else None
     for w in work:
-        if a.only and w[0] != a.only:
+        if only and w[0] not in only:
             continue
-        r = run(*w[:6], a.steps, a.reps, *w[6:])
+        steps = w[7] if len(w) > 7 else a.steps           # the DPM-Solver++ rows fix their step counts
+        r = run(*w[:6], steps, a.reps, *w[6:7])
         r.update(gpu=name, power_limit=power)
         print(json.dumps(r), flush=True)
 
