@@ -591,6 +591,23 @@ int lb_sample_step_ms(const void* model_out, int model_dtype, long long stride_b
                       int unet_channels, float* timestep, void* vae_in, int vae_dtype, int vae_channels_last,
                       float vae_inv_scaling, int B, int C, int H, int W, void* stream);
 
+/* Either sampling step with guidance rescale (diffusers' rescale_noise_cfg, the `guidance_rescale` of
+ * StableDiffusionPipeline / StableDiffusionXLPipeline), one launch. The arguments are lb_sample_step_ch's
+ * without init, plus x0_hist and guidance_rescale (a DEVICE fp32 [1], phi, so phi changes per call without
+ * a recapture). x0_hist == NULL: lb_sample_step_ch's single-step update, reading noise; x0_hist != NULL:
+ * lb_sample_step_ms's multistep update (noise is not read). Per sample b, over its C*H*W elements:
+ *   m = m_u + g (m_c - m_u);  r_b = std(m_c) / std(m)  (unbiased);  m = phi (m r_b) + (1 - phi) m
+ * evaluated as m * fl32(1 + phi (r_b - 1)), the statistics accumulated in fp64 in a fixed order (replays
+ * are bit-reproducible). At phi = 0 every output equals lb_sample_step_ch's / lb_sample_step_ms's bit
+ * for bit. The step index advances as in lb_sample_step. Allocates nothing; capturable.
+ * G != 2, guidance_rescale == NULL, B > 65535 or lb_sample_step_ch's bad shapes: LB_ERR_SHAPE. */
+int lb_sample_step_rescale(const void* model_out, int model_dtype, long long stride_b, long long stride_c,
+                           long long stride_p, int G, float* x, const float* noise, float* x0_hist,
+                           const float* table, int table_rows, const float* guidance,
+                           const float* guidance_rescale, int* step_index, unsigned int* counter, void* unet_in,
+                           int unet_dtype, int unet_channels, float* timestep, void* vae_in, int vae_dtype,
+                           int vae_channels_last, float vae_inv_scaling, int B, int C, int H, int W, void* stream);
+
 /* The start of an img2img or inpainting sampling loop, one launch (diffusers' StableDiffusionImg2Img-
  * Pipeline.prepare_latents / StableDiffusionInpaintPipeline.prepare_mask_latents). Row 0 of the table is
  * (c_noise, s_start, t_start, c_lat, ...) (host/schedulers.pack_table); noise slice 0 is z_0.

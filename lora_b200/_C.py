@@ -82,6 +82,8 @@ def _load():
                                f32, i32, i32, i32, i32, i32, vp], i32),
         "lb_sample_step_ms": ([vp, i32, ll, ll, ll, i32, vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp, vp, i32, i32,
                                f32, i32, i32, i32, i32, vp], i32),
+        "lb_sample_step_rescale": ([vp, i32, ll, ll, ll, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp,
+                                    i32, i32, f32, i32, i32, i32, i32, vp], i32),
         "lb_sample_init": ([vp, i32, ll, ll, ll, vp, i32, f32, vp, vp, vp, i32, vp, vp, vp, vp, i32, i32, vp, i32, i32,
                             i32, i32, i32, vp], i32),
         "lb_pixels_ingest_inpaint": ([vp, vp, vp, i32, i32, i32, i32, i32, vp], i32),
@@ -164,7 +166,7 @@ EXPORTED = [n for n in ("lb_abi_version", "lb_lora_linear_fwd", "lb_lora_wgrad",
                         "lb_lora_linear_fwd_dropout", "lb_lora_conv2d_fwd_dropout", "lb_debug_set_pdl", "lb_svd_workspace_bytes", "lb_svd_truncated_batched",
                         "lb_optim_step_fused", "lb_step_prologue", "lb_step_prologue_v", "lb_masked_mse_fwd_bwd",
                         "lb_pixels_ingest", "lb_step_prologue_posterior", "lb_sample_step", "lb_pixels_emit",
-                        "lb_sample_step_ch", "lb_sample_step_ms", "lb_sample_init", "lb_pixels_ingest_inpaint",
+                        "lb_sample_step_ch", "lb_sample_step_ms", "lb_sample_step_rescale", "lb_sample_init", "lb_pixels_ingest_inpaint",
                         "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight")]
 
 

@@ -20,6 +20,8 @@
 //                         inpainting UNet): only the latent channels are written
 //   lb_sample_step_ms     the same for a multistep scheduler (DPM-Solver++(2M)): the data prediction, the
 //                         update from it and the previous step's, and that history kept in place
+//   lb_sample_step_rescale  either step (single-step or multistep) with guidance rescale: the per-sample
+//                         std ratio of the conditional and guided predictions, in the same one launch
 //   lb_sample_init       the start of an img2img or inpainting loop: the posterior sample of the encoded
 //                         image, scheduler.add_noise at the first kept timestep, the first UNet input,
 //                         and for inpainting the constant mask and masked-image channels
@@ -30,10 +32,13 @@
 // ten small torch kernels per step and their intermediates), not bandwidth.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "lora_b200.h"
+
+namespace cg = cooperative_groups;
 
 namespace lbglue {
 
@@ -349,6 +354,142 @@ sample_step_kernel(const void* __restrict__ mo, int mdt, long long sb, long long
   }
 }
 
+// lb_sample_step_rescale: sample_step_kernel's step (G = 2) with guidance rescale ("Common Diffusion Noise
+// Schedules are Flawed", diffusers' rescale_noise_cfg) between the guidance sum and the update:
+//   m_hat = m_u + g (m_c - m_u);  r_b = std(m_c[b]) / std(m_hat[b]) (unbiased, over C x P; the (n - 1)
+//   cancels in the ratio);  m_hat <- k_b m_hat,  k_b = fl32(1 + phi (r_b - 1)) = phi r_b + (1 - phi)
+// k_b is exactly 1 at phi = 0 (set so, whatever r_b is), and m_hat * 1 is m_hat bit for bit: the update
+// then equals sample_step_kernel's, whose float operations this kernel repeats in the same order.
+//
+// The statistics of sample b need every element of b before any element can be updated, so the launch
+// is one 8-CTA thread-block cluster per sample (8 is the portable cluster size; grid (8, B)). Its CTAs
+// stride over the sample's pixels twice. Pass 1 sums (m_c, m_c^2, m_hat, m_hat^2) in fp64 per thread,
+// then over the warp by shuffles, over the CTA in warp order, and over the cluster through distributed
+// shared memory in rank order: a fixed order, so replays are bit-reproducible. A cluster barrier needs no
+// grid-wide co-residency (a cooperative launch would) and keeps the whole exchange on chip. Pass 2
+// re-reads the model output (L2-resident: 256 KiB at 128 x 128 latents in bf16) and applies the update.
+// The step index advances as in sample_step_kernel: every CTA reads it first, the last CTA to arrive
+// advances it, so one captured launch replays as every step. MS selects lb_sample_step_ms's update.
+constexpr int RS_CLUSTER = 8;
+
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+template <bool MS>
+__global__ void __cluster_dims__(RS_CLUSTER, 1, 1) __launch_bounds__(256)
+sample_step_rescale_kernel(const void* __restrict__ mo, int mdt, long long sb, long long sc, long long sp,
+                           float* __restrict__ x, const float* __restrict__ noise, float* __restrict__ x0_hist,
+                           const float* __restrict__ table, int rows, const float* __restrict__ guidance,
+                           const float* __restrict__ guidance_rescale, int* __restrict__ step_index,
+                           unsigned int* __restrict__ counter, void* __restrict__ unet_in, int udt, int Cu,
+                           float* __restrict__ timestep, void* __restrict__ vae_in, int vdt, int vae_cl,
+                           float vae_inv_scaling, int B, int C, int P) {
+  cg::cluster_group cluster = cg::this_cluster();
+  __shared__ int s_row;
+  __shared__ double s_warp[8][4];
+  __shared__ double s_part[4];
+  __shared__ float s_k;
+  __shared__ bool last_block;
+  if (threadIdx.x == 0) {
+    const int k = 1 + *step_index;
+    s_row = k < 0 ? 0 : (k >= rows ? rows - 1 : k);
+  }
+  __syncthreads();
+  const float* row = table + 8ll * s_row;
+  const int b = blockIdx.y;
+  const int stride = RS_CLUSTER * 256;
+  const int first = static_cast<int>(cluster.block_rank()) * 256 + threadIdx.x;
+  const float g = *guidance;
+  const long long ub = static_cast<long long>(b) * sb, cb = static_cast<long long>(B + b) * sb;
+
+  double acc[4] = {0.0, 0.0, 0.0, 0.0};       // sum m_c, sum m_c^2, sum m_hat, sum m_hat^2
+  for (int px = first; px < P; px += stride) {
+    for (int c = 0; c < C; ++c) {
+      const long long o = c * sc + px * sp;
+      const float mu = ld_any(mo, ub + o, mdt), mc = ld_any(mo, cb + o, mdt);
+      const double dc = mc, dh = fmaf(g, mc - mu, mu);
+      acc[0] += dc;
+      acc[1] += dc * dc;
+      acc[2] += dh;
+      acc[3] += dh * dh;
+    }
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const double v = warp_sum(acc[j]);
+    if (lane == 0) s_warp[warp][j] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < 4) {
+    double v = 0.0;
+    for (int w = 0; w < 8; ++w) v += s_warp[w][threadIdx.x];
+    s_part[threadIdx.x] = v;
+  }
+  cluster.sync();
+  if (threadIdx.x == 0) {
+    double a[4] = {0.0, 0.0, 0.0, 0.0};
+    for (unsigned int r = 0; r < RS_CLUSTER; ++r) {
+      const double* part = cluster.map_shared_rank(s_part, r);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) a[j] += part[j];
+    }
+    const double n = static_cast<double>(C) * P;
+    const double ss_c = a[1] - a[0] * a[0] / n, ss_h = a[3] - a[2] * a[2] / n;
+    const double phi = *guidance_rescale;
+    s_k = phi == 0.0 ? 1.f : static_cast<float>(1.0 + phi * (sqrt(ss_c / ss_h) - 1.0));
+  }
+  cluster.sync();            // s_k is set, and no CTA leaves while another still reads its s_part
+
+  const float kf = s_k;
+  const float alpha = row[0], beta = row[1], gamma = row[2], s_next = row[3];
+  const bool last = row[5] != 0.f;
+  const float p = MS ? row[6] : 0.f, q = MS ? row[7] : 0.f;
+  const long long slice = static_cast<long long>(B) * C * P;
+  const float* z = MS ? nullptr : noise + s_row * slice;
+  for (int px = first; px < P; px += stride) {
+    const long long i = static_cast<long long>(b) * P + px;
+    for (int c = 0; c < C; ++c) {
+      const long long xi = (static_cast<long long>(b) * C + c) * P + px;
+      const long long o = c * sc + px * sp;
+      float m = ld_any(mo, ub + o, mdt);
+      const float mc = ld_any(mo, cb + o, mdt);
+      m = fmaf(g, mc - m, m);
+      m = __fmul_rn(m, kf);
+      float xn;
+      if (MS) {
+        const float xc = x[xi];
+        const float x0 = fmaf(p, xc, q * m);
+        xn = fmaf(alpha, xc, beta * x0);
+        if (gamma != 0.f) xn = fmaf(gamma, x0_hist[xi], xn);
+        x0_hist[xi] = x0;
+      } else {
+        xn = fmaf(alpha, x[xi], beta * m);
+        if (gamma != 0.f) xn = fmaf(gamma, z[xi], xn);
+      }
+      x[xi] = xn;
+      const float u = __fmul_rn(s_next, xn);
+      for (int h = 0; h < 2; ++h) st_any(unet_in, (static_cast<long long>(h * B + b) * P + px) * Cu + c, udt, u);
+      if (last) st_any(vae_in, vae_cl ? i * C + c : xi, vdt, __fmul_rn(vae_inv_scaling, xn));
+    }
+  }
+  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *timestep = row[4];
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last_block = atomicAdd(counter, 1u) == gridDim.x * gridDim.y - 1;
+  }
+  __syncthreads();
+  if (last_block && threadIdx.x == 0) {
+    *step_index += 1;
+    *counter = 0u;
+    __threadfence();
+  }
+}
+
 // The start of an img2img or inpainting sampling loop (StableDiffusionImg2ImgPipeline /
 // StableDiffusionInpaintPipeline), element (b, c, p) of the latents [B, C, P], from row 0 of the table:
 // (c_noise, s_start, t_start, c_lat). With moments and no mask (img2img):
@@ -588,6 +729,36 @@ extern "C" int lb_sample_step_ms(const void* model_out, int model_dtype, long lo
                                   table, table_rows, guidance, step_index, counter, unet_in, unet_dtype,
                                   unet_channels, timestep, vae_in, vae_dtype, vae_channels_last, vae_inv_scaling, B,
                                   C, H, W, 0, stream);
+}
+
+extern "C" int lb_sample_step_rescale(const void* model_out, int model_dtype, long long stride_b,
+                                      long long stride_c, long long stride_p, int G, float* x, const float* noise,
+                                      float* x0_hist, const float* table, int table_rows, const float* guidance,
+                                      const float* guidance_rescale, int* step_index, unsigned int* counter,
+                                      void* unet_in, int unet_dtype, int unet_channels, float* timestep,
+                                      void* vae_in, int vae_dtype, int vae_channels_last, float vae_inv_scaling,
+                                      int B, int C, int H, int W, void* stream) {
+  if (B <= 0 || B > 65535 || C <= 0 || H <= 0 || W <= 0 || G != 2 || table_rows < 2 || unet_channels < C)
+    return LB_ERR_SHAPE;
+  if (static_cast<long long>(H) * W > 0x7fffffffll - RS_CLUSTER * 256) return LB_ERR_SHAPE;
+  if (!float_dtype(model_dtype) || !float_dtype(unet_dtype) || !float_dtype(vae_dtype)) return LB_ERR_DTYPE;
+  if (model_out == nullptr || x == nullptr || (x0_hist == nullptr && noise == nullptr) || table == nullptr ||
+      guidance == nullptr || guidance_rescale == nullptr || step_index == nullptr || counter == nullptr ||
+      unet_in == nullptr || timestep == nullptr || vae_in == nullptr || !(vae_inv_scaling > 0.f))
+    return LB_ERR_SHAPE;
+  const dim3 grid(RS_CLUSTER, B);
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (x0_hist)
+    sample_step_rescale_kernel<true><<<grid, 256, 0, s>>>(
+        model_out, model_dtype, stride_b, stride_c, stride_p, x, nullptr, x0_hist, table, table_rows, guidance,
+        guidance_rescale, step_index, counter, unet_in, unet_dtype, unet_channels, timestep, vae_in, vae_dtype,
+        vae_channels_last != 0, vae_inv_scaling, B, C, H * W);
+  else
+    sample_step_rescale_kernel<false><<<grid, 256, 0, s>>>(
+        model_out, model_dtype, stride_b, stride_c, stride_p, x, noise, nullptr, table, table_rows, guidance,
+        guidance_rescale, step_index, counter, unet_in, unet_dtype, unet_channels, timestep, vae_in, vae_dtype,
+        vae_channels_last != 0, vae_inv_scaling, B, C, H * W);
+  return cudaGetLastError() == cudaSuccess ? LB_OK : LB_ERR_CUDA;
 }
 
 extern "C" int lb_sample_init(const void* moments, int moments_dtype, long long stride_b, long long stride_c,

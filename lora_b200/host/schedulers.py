@@ -66,6 +66,19 @@ and lb_sample_step_ms keeps h on the device. The table row is (a, b, d, s_next, 
   img2img       add_noise as DDIM's: sqrt(acp[t]) x + sqrt(1 - acp[t]) z (float32 tables)
 Karras sigmas (use_karras_sigmas, diffusers 0.15+) follow other rules and are not provided.
 
+Euler ("euler": EulerDiscreteScheduler with the scheduler config SDXL base ships: scaled_linear 0.00085 ->
+0.012, timestep_spacing="leading", steps_offset=1, linear interpolation, no Karras sigmas, s_churn = 0)
+is single-step and noiseless (gamma = 0). The name means this config for every UNet: SD 1.x's
+scheduler config would space the timesteps "linspace" in diffusers. No copy of diffusers is installed
+here; the rules below are restated from its source, and oracle/sample_xl_ref.RefEulerDiscrete restates
+the scheduler op by op.
+  timesteps     (arange(n) * (1000 // n)).round() reversed, plus 1, float32: n = 30 gives 958 925 ... 34 1
+  sigmas        ((1 - acp) / acp) ** 0.5, np.interp at the timesteps, then [.., 0.0], as float32
+  init_noise_sigma = (max(sigmas) ** 2 + 1) ** 0.5 ("leading" spacing);  scale_model_input as Euler-a's
+  step i        x0 as Euler-ancestral's;  x' = x + (x - x0) / sigma_i * (sigma_{i+1} - sigma_i)
+  img2img       add_noise as Euler-ancestral's: x + z * sigma[t_start]
+The three older schedulers keep the tables above (SD's scheduler configs) for SDXL UNets too.
+
 DDPM / PNDM sampling are not provided: DDPM's strided-variance rule changed between diffusers
 releases, and no copy of them is installed to pin it against.
 """
@@ -74,7 +87,7 @@ import math
 import numpy as np
 import torch
 
-SCHEDULERS = ("euler_ancestral", "ddim", "dpmsolver_multistep")
+SCHEDULERS = ("euler_ancestral", "ddim", "dpmsolver_multistep", "euler")
 MULTISTEP = ("dpmsolver_multistep",)        # run by lb_sample_step_ms, with the x0 history
 PREDICTION_TYPES = ("epsilon", "v_prediction")
 NUM_TRAIN_TIMESTEPS = 1000
@@ -101,25 +114,31 @@ def alphas_cumprod() -> torch.Tensor:
 
 
 def timesteps(scheduler: str, n: int) -> np.ndarray:
-    """The scheduler's timesteps for n inference steps (float64 for Euler-ancestral, int64 for DDIM and
-    DPM-Solver++)."""
+    """The scheduler's timesteps for n inference steps (float64 for Euler-ancestral, float32 for Euler,
+    int64 for DDIM and DPM-Solver++)."""
     if scheduler == "euler_ancestral":
         return np.linspace(0, NUM_TRAIN_TIMESTEPS - 1, n, dtype=float)[::-1].copy()
+    if scheduler == "euler":
+        ts = (np.arange(0, n) * (NUM_TRAIN_TIMESTEPS // n)).round()[::-1].copy().astype(np.float32)
+        return ts + np.float32(1)
     if scheduler == "dpmsolver_multistep":
         return np.linspace(0, NUM_TRAIN_TIMESTEPS - 1, n + 1).round()[::-1][:-1].copy().astype(np.int64)
     ratio = NUM_TRAIN_TIMESTEPS // n
     return (np.arange(0, n) * ratio).round()[::-1].copy().astype(np.int64) + 1
 
 
-def euler_sigmas(n: int) -> np.ndarray:
-    """EulerAncestralDiscreteScheduler.sigmas after set_timesteps(n): float32, n + 1 values."""
+def euler_sigmas(n: int, scheduler: str = "euler_ancestral") -> np.ndarray:
+    """EulerAncestralDiscreteScheduler.sigmas (or, scheduler="euler", EulerDiscreteScheduler's) after
+    set_timesteps(n): float32, n + 1 values."""
     acp = alphas_cumprod()
     base = np.array(((1 - acp) / acp) ** 0.5)
-    s = np.interp(timesteps("euler_ancestral", n), np.arange(0, len(base)), base)
+    s = np.interp(timesteps(scheduler, n), np.arange(0, len(base)), base)
     return np.concatenate([s, [0.0]]).astype(np.float32)
 
 
 def init_noise_sigma(scheduler: str, n: int) -> float:
+    if scheduler == "euler":
+        return float((float(euler_sigmas(n, "euler").max()) ** 2 + 1) ** 0.5)
     return float(euler_sigmas(n).max()) if scheduler == "euler_ancestral" else 1.0
 
 
@@ -162,19 +181,22 @@ def coefficients(scheduler: str, prediction_type: str, n: int, t_start: int = 0)
     ts = timesteps(scheduler, n).astype(np.float64)
     steps = np.zeros((n, 5), dtype=np.float64)
     v = prediction_type == "v_prediction"
-    if scheduler == "euler_ancestral":
-        sig = euler_sigmas(n).astype(np.float64)
+    if scheduler in ("euler_ancestral", "euler"):
+        sig = euler_sigmas(n, scheduler).astype(np.float64)
         for i in range(n):
             s, s_to = sig[i], sig[i + 1]
-            up = math.sqrt(s_to ** 2 * (s ** 2 - s_to ** 2) / s ** 2)
-            down = math.sqrt(s_to ** 2 - up ** 2)
+            if scheduler == "euler":                   # s_churn = 0: no noise, the step ends at sigma_{i+1}
+                up, down = 0.0, s_to
+            else:
+                up = math.sqrt(s_to ** 2 * (s ** 2 - s_to ** 2) / s ** 2)
+                down = math.sqrt(s_to ** 2 - up ** 2)
             d = down - s
             if v:
                 alpha, beta = 1.0 + d * s / (s ** 2 + 1), d / math.sqrt(s ** 2 + 1)
             else:
                 alpha, beta = 1.0, d
             steps[i] = (alpha, beta, up, 1.0 / math.sqrt(s_to ** 2 + 1), ts[i + 1] if i + 1 < n else 0.0)
-        return (float(sig.max()), 1.0 / math.sqrt(sig[0] ** 2 + 1), ts[0]), steps
+        return (init_noise_sigma(scheduler, n), 1.0 / math.sqrt(sig[0] ** 2 + 1), ts[0]), steps
     acp = alphas_cumprod().double().numpy()
     ratio = NUM_TRAIN_TIMESTEPS // n
     for i in range(n):
@@ -204,10 +226,11 @@ def t_start(n: int, strength: float) -> int:
 
 def add_noise_coefficients(scheduler: str, n: int, start: int):
     """(c_lat, c_noise): the float32 scalars scheduler.add_noise(x, z, timesteps[start]) evaluates as
-    c_lat * x + c_noise * z (Euler-ancestral: 1 and sigma[start]; DDIM and DPM-Solver++: sqrt(acp[t]) and
-    sqrt(1 - acp[t]), each rounded to float32 as torch computes them from the float32 alphas_cumprod)."""
-    if scheduler == "euler_ancestral":
-        return np.float32(1.0), euler_sigmas(n)[start]
+    c_lat * x + c_noise * z (Euler-ancestral and Euler: 1 and sigma[start]; DDIM and DPM-Solver++:
+    sqrt(acp[t]) and sqrt(1 - acp[t]), each rounded to float32 as torch computes them from the float32
+    alphas_cumprod)."""
+    if scheduler in ("euler_ancestral", "euler"):
+        return np.float32(1.0), euler_sigmas(n, scheduler)[start]
     acp = alphas_cumprod().numpy()
     t = int(timesteps(scheduler, n)[start])
     return np.sqrt(acp[t]), np.sqrt(np.float32(1.0) - acp[t])

@@ -37,9 +37,12 @@ A `sample()` replays three CUDA graphs, with no host sync and no allocation betw
 scheduler, the guidance scale, the seed, the strength, the image and the mask may change per call:
 they rewrite device tables and buffers. A guidance
 scale <= 1 runs without the unconditional half (G = 1), as the pipeline does; that is a capture of its own.
-So is each scheduler family (schedulers.family: "single-step" for Euler-ancestral and DDIM, "multistep"
-for DPM-Solver++): switching between Euler-ancestral and DDIM costs no capture, the first call of the
-other family one, and later calls none.
+So is each scheduler family (schedulers.family: "single-step" for Euler-ancestral, Euler and DDIM,
+"multistep" for DPM-Solver++): switching between Euler-ancestral and DDIM costs no capture, the first call
+of the other family one, and later calls none. Guidance rescale (`guidance_rescale` phi > 0 with
+guidance; diffusers' rescale_noise_cfg) runs lb_sample_step_rescale in place of the step launch, in either
+family: a capture of its own, while phi itself is a device scalar and changes per call. LoraXLSampler
+(below) samples SDXL.
 The graphs are captured again only when something baked into a launch changes: a site's scale, a
 selector, the set of sites or their parameter storage, the grouping policy (`captures` counts them).
 
@@ -58,7 +61,7 @@ import torch.nn as nn
 from . import _C, ops
 from .host import schedulers
 from .step_ops import (pixels_emit, pixels_ingest, pixels_ingest_inpaint, sample_init, sample_step, sample_step_ch,
-                       sample_step_ms)
+                       sample_step_ms, sample_step_rescale)
 
 _SITE_NAMES = ("LoraInjectedLinear", "LoraInjectedConv2d")
 
@@ -82,6 +85,9 @@ class SamplerConfig:
     # a UNet of 2C + 1 input channels); with external_noise the caller fills `self.posterior_noise` too
     task: str = "txt2img"
     strength: float = 0.8                      # img2img: the part of the schedule run (the pipeline's default)
+    # phi of rescale_noise_cfg ("Common Diffusion Noise Schedules are Flawed"), in [0, 1]; applied under
+    # classifier-free guidance only (G = 2), by lb_sample_step_rescale; 0 runs the plain step launches
+    guidance_rescale: float = 0.0
 
 
 TASKS = ("txt2img", "img2img", "inpaint")
@@ -91,14 +97,24 @@ def _sites(*models):
     return [m for model in models for m in model.modules() if type(m).__name__ in _SITE_NAMES]
 
 
+def _check_phi(phi: float) -> float:
+    phi = float(phi)
+    if not 0.0 <= phi <= 1.0:
+        raise ValueError(f"guidance_rescale must be in [0, 1], got {phi}")
+    return phi
+
+
 class LoraSampler:
+    _sdxl = False             # LoraXLSampler: the UNet takes the SDXL "text_time" conditioning
+
     def __init__(self, unet: nn.Module, text_encoder: nn.Module, vae: nn.Module, cfg: SamplerConfig,
                  latent_shape=(1, 4, 64, 64), seq_len: int = 77, device=None):
         schedulers.check(cfg.scheduler, cfg.prediction_type)
         ucfg = getattr(unet, "cfg", None) or getattr(unet, "config", None)
-        if getattr(ucfg, "addition_embed_type", None) is not None:
+        if not self._sdxl and getattr(ucfg, "addition_embed_type", None) is not None:
             raise ValueError("LoraSampler does not sample SDXL UNets (addition_embed_type "
-                             f"{ucfg.addition_embed_type!r}): their pooled and time-id conditioning is not supported")
+                             f"{ucfg.addition_embed_type!r}): sample them with LoraXLSampler")
+        _check_phi(cfg.guidance_rescale)
         B, C, h, w = latent_shape
         if cfg.task not in TASKS:
             raise ValueError(f"unknown task {cfg.task!r}: one of {TASKS}")
@@ -133,6 +149,7 @@ class LoraSampler:
         self.x0_hist = torch.zeros(latent_shape, device=dev, dtype=torch.float32)      # multistep: last x0
         self.table = torch.zeros((rows, schedulers.TABLE_COLS), device=dev, dtype=torch.float32)
         self.guidance = torch.zeros(1, device=dev, dtype=torch.float32)
+        self.guidance_rescale = torch.zeros(1, device=dev, dtype=torch.float32)      # phi
         self.step_index = torch.zeros(1, device=dev, dtype=torch.int32)
         self._counter = torch.zeros(1, device=dev, dtype=torch.int32)
         self.timestep = torch.zeros(1, device=dev, dtype=torch.float32)
@@ -150,7 +167,7 @@ class LoraSampler:
             self.mask_image = torch.zeros((B, 8 * h, 8 * w), device=dev, dtype=torch.uint8)
         self._ehs = {}
         self._table_key = None
-        self._graphs = {}             # (G, scheduler family) -> (A, B, C)
+        self._graphs = {}             # (G, scheduler family[, "rescale"]) -> (A, B, C)
         self._fingerprint = None
         self._factor_bufs = []
         self.captures = 0
@@ -160,7 +177,7 @@ class LoraSampler:
         """Everything of the models that a captured launch holds as a constant or an address."""
         from .grouping import get_grouping
         sig = []
-        for m in _sites(self.unet, self.text_encoder):
+        for m in _sites(*self._lora_models()):
             base = m.linear if hasattr(m, "linear") else m.conv
             sel = getattr(m.selector, "weight", None)
             sig.append((id(m), float(m.scale), m.r, id(sel), None if sel is None else sel.data_ptr(),
@@ -173,7 +190,7 @@ class LoraSampler:
         """The 16-bit padded down-factor copies the sites' forward reads (modules._SiteState.down): held
         here so that the addresses graph B captured stay valid, and re-cast by `_refresh_factors`."""
         bufs = []
-        for m in _sites(self.unet, self.text_encoder):
+        for m in _sites(*self._lora_models()):
             if m.r > ops.MAX_RANK:        # rank chunks cast their factors inside every forward
                 continue
             tab = None
@@ -204,17 +221,28 @@ class LoraSampler:
                                                    _C.dtype_code(dt), _C.stream_ptr()), "lb_refresh_shadows")
             ops._count()
 
+    def _lora_models(self):
+        """The models whose LoRA sites the sampler covers (fingerprint, factor refresh, eval mode)."""
+        return (self.unet, self.text_encoder)
+
     # ------------------------------------------------------------------ the three bodies
     def _autocast(self):
         dt = self.cfg.autocast_dtype
         return torch.autocast("cuda", dtype=dt) if dt is not None else torch.autocast("cuda", enabled=False)
 
-    def _body_a(self, G: int):
-        self._refresh_factors()
+    def _encode(self, G: int):
+        """The conditioning of the G halves (under the autocast): [negative ; prompt] hidden states."""
         B = self.latents.shape[0]
         ids = self.input_ids if G == 2 else self.input_ids[B:]
+        self._ehs[G] = self.text_encoder(ids)[0].to(self.model_dtype)
+
+    def _unet(self, G: int):
+        return self.unet(self.unet_in[G], self.timestep, self._ehs[G]).sample
+
+    def _body_a(self, G: int):
+        self._refresh_factors()
         with self._autocast():
-            self._ehs[G] = self.text_encoder(ids)[0].to(self.model_dtype)
+            self._encode(G)
         task = self.cfg.task
         if task == "txt2img":
             sample_step(None, self.latents, self.noise, self.table, None, self.step_index, self._counter,
@@ -230,9 +258,15 @@ class LoraSampler:
                     self._counter, self.unet_in[G], self.timestep, self.cfg.vae_scaling,
                     mask=self.mask_image if task == "inpaint" else None)
 
-    def _body_b(self, G: int, family: str = "single-step"):
+    def _body_b(self, G: int, family: str = "single-step", rescale: bool = False):
         with self._autocast():
-            out = self.unet(self.unet_in[G], self.timestep, self._ehs[G]).sample
+            out = self._unet(G)
+        if rescale:                   # G = 2, either family: lb_sample_step_rescale
+            ms = family == "multistep"
+            sample_step_rescale(out, self.latents, None if ms else self.noise, self.x0_hist if ms else None,
+                                self.table, self.guidance, self.guidance_rescale, self.step_index, self._counter,
+                                self.unet_in[G], self.timestep, self.vae_in, self.cfg.vae_scaling)
+            return
         if family == "multistep":
             sample_step_ms(out, self.latents, self.x0_hist, self.table, self.guidance, self.step_index,
                            self._counter, self.unet_in[G], self.timestep, self.vae_in, self.cfg.vae_scaling)
@@ -244,20 +278,25 @@ class LoraSampler:
     def _body_c(self):
         pixels_emit(self.vae.decode(self.vae_in).sample, self.image)
 
-    def _run_eager(self, G: int, n: int, family: str = "single-step"):
+    def _run_eager(self, G: int, n: int, family: str = "single-step", rescale: bool = False):
         self._collect_factor_buffers()
         self._body_a(G)
         for _ in range(n):
-            self._body_b(G, family)
+            self._body_b(G, family, rescale)
         self._body_c()
 
     # ------------------------------------------------------------------ capture
-    def _capture(self, G: int, family: str):
+    def _key(self, G: int, family: str, rescale: bool):
+        """The capture key: guidance mode, scheduler family, and the rescale launch when it runs."""
+        return (G, family) + (("rescale",) if rescale else ())
+
+    def _capture(self, key):
+        G, family, rescale = key[0], key[1], "rescale" in key[2:]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(max(1, self.cfg.graph_warmup)):
-                self._run_eager(G, 1, family)
+                self._run_eager(G, 1, family, rescale)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self._collect_factor_buffers()
@@ -266,27 +305,28 @@ class LoraSampler:
             self._body_a(G)
         gb = torch.cuda.CUDAGraph()
         with torch.cuda.graph(gb, pool=ga.pool()):
-            self._body_b(G, family)
+            self._body_b(G, family, rescale)
         gc = torch.cuda.CUDAGraph()
         with torch.cuda.graph(gc, pool=ga.pool()):
             self._body_c()
         torch.cuda.synchronize()
-        self._graphs[(G, family)] = (ga, gb, gc)
+        self._graphs[key] = (ga, gb, gc)
         self.captures += 1
 
-    def _graphs_for(self, G: int, family: str):
+    def _graphs_for(self, key):
         fp = self._fingerprint_now()
         if fp != self._fingerprint:
             self._graphs.clear()
             self._fingerprint = fp
-        if (G, family) not in self._graphs:
-            self._capture(G, family)
-        return self._graphs[(G, family)]
+        if key not in self._graphs:
+            self._capture(key)
+        return self._graphs[key]
 
     # ------------------------------------------------------------------ modes
     def _enter_eval(self):
-        saved = [(m, m.training) for model in (self.unet, self.text_encoder, self.vae) for m in model.modules()]
-        for model in (self.unet, self.text_encoder, self.vae):
+        models = self._lora_models() + (self.vae,)
+        saved = [(m, m.training) for model in models for m in model.modules()]
+        for model in models:
             model.eval()
         return saved
 
@@ -340,32 +380,36 @@ class LoraSampler:
         if task == "inpaint":
             self.mask_image.copy_(mask_image)
 
-    def prepare(self, guidance_scale: Optional[float] = None):
-        """Capture the graphs for the configured (or given) guidance scale ahead of the first sample()."""
+    def prepare(self, guidance_scale: Optional[float] = None, guidance_rescale: Optional[float] = None):
+        """Capture the graphs for the configured (or given) guidance scale and rescale ahead of the first
+        sample()."""
         if not self.cfg.use_cuda_graph:
             return
         n, sched, g, start = self._options(None, None, guidance_scale)
+        phi = _check_phi(self.cfg.guidance_rescale if guidance_rescale is None else guidance_rescale)
+        G = 2 if g > 1.0 else 1
         saved = self._enter_eval()
         try:
             with torch.no_grad():
                 self._set_table(sched, n, start)
-                self._graphs_for(2 if g > 1.0 else 1, schedulers.family(sched))
+                self._graphs_for(self._key(G, schedulers.family(sched), G == 2 and phi > 0.0))
         finally:
             self._restore_modes(saved)
 
     def sample(self, input_ids: torch.Tensor, negative_input_ids: Optional[torch.Tensor] = None, seed: int = 0,
                num_inference_steps: Optional[int] = None, scheduler: Optional[str] = None,
                guidance_scale: Optional[float] = None, image: Optional[torch.Tensor] = None,
-               mask_image: Optional[torch.Tensor] = None, strength: Optional[float] = None) -> torch.Tensor:
+               mask_image: Optional[torch.Tensor] = None, strength: Optional[float] = None,
+               guidance_rescale: Optional[float] = None) -> torch.Tensor:
         """uint8 [B, 8h, 8w, 3] images (a view of `self.image`, overwritten by the next call) for the token
         ids [B, seq_len] of the prompts and of the negative prompts (the empty prompt's ids for plain
         classifier-free guidance; unused when guidance_scale <= 1). `self.latents` holds the final latents.
         img2img: image uint8 [B, 8h, 8w, 3], strength in (0, 1] (default cfg.strength); inpaint: image and
-        mask_image uint8 [B, 8h, 8w] (0..255, >= 128 repainted)."""
+        mask_image uint8 [B, 8h, 8w] (0..255, >= 128 repainted). guidance_rescale: phi in [0, 1] (default
+        cfg.guidance_rescale), applied when guidance_scale > 1."""
         n, sched, g, start = self._options(num_inference_steps, scheduler, guidance_scale, strength)
-        k = n - start
+        phi = _check_phi(self.cfg.guidance_rescale if guidance_rescale is None else guidance_rescale)
         G = 2 if g > 1.0 else 1
-        family = schedulers.family(sched)
         B = self.latents.shape[0]
         if tuple(input_ids.shape) != tuple(self.input_ids[B:].shape):
             raise ValueError(f"input_ids of shape {tuple(input_ids.shape)}: the sampler takes "
@@ -373,27 +417,173 @@ class LoraSampler:
         if G == 2 and (negative_input_ids is None or tuple(negative_input_ids.shape) != tuple(input_ids.shape)):
             raise ValueError("guidance_scale > 1 needs negative_input_ids of the prompts' shape")
         self._set_images(image, mask_image)
+
+        def write_ids():
+            self.input_ids[B:].copy_(input_ids)
+            if G == 2:
+                self.input_ids[:B].copy_(negative_input_ids)
+
+        return self._generate(n, sched, g, start, phi, seed, write_ids)
+
+    def _generate(self, n: int, sched: str, g: float, start: int, phi: float, seed: int, write_inputs):
+        """The call's tables, scalars, inputs (write_inputs()) and noise, then the graphs (or the eager
+        path): the part of sample() every sampler shares."""
+        k = n - start
+        G = 2 if g > 1.0 else 1
+        rescale = G == 2 and phi > 0.0
+        key = self._key(G, schedulers.family(sched), rescale)
         saved = self._enter_eval()
         try:
             with torch.no_grad():
                 self._set_table(sched, n, start)
                 self.guidance.fill_(g)
-                self.input_ids[B:].copy_(input_ids)
-                if G == 2:
-                    self.input_ids[:B].copy_(negative_input_ids)
+                if rescale:
+                    self.guidance_rescale.fill_(phi)
+                write_inputs()
                 if not self.cfg.external_noise:
                     self.generator.manual_seed(int(seed))
                     self.noise[:k + 1].normal_(generator=self.generator)
                     if self.cfg.task != "txt2img":
                         self.posterior_noise.normal_(generator=self.generator)
                 if self.cfg.use_cuda_graph:
-                    ga, gb, gc = self._graphs_for(G, family)
+                    ga, gb, gc = self._graphs_for(key)
                     ga.replay()
                     for _ in range(k):
                         gb.replay()
                     gc.replay()
                 else:
-                    self._run_eager(G, k, family)
+                    self._run_eager(G, k, key[1], rescale)
         finally:
             self._restore_modes(saved)
         return self.image
+
+
+def _int_ids(t: torch.Tensor, shape, what: str):
+    if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{what} of shape {None if not isinstance(t, torch.Tensor) else tuple(t.shape)}: the "
+                         f"sampler takes {tuple(shape)}")
+    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+        raise ValueError(f"{what} must be integer token ids, got {t.dtype}")
+
+
+def _pair(v, what: str):
+    if v is None or len(v) != 2:
+        raise ValueError(f"{what} must be a pair (height, width) or (top, left), got {v!r}")
+    return float(v[0]), float(v[1])
+
+
+class LoraXLSampler(LoraSampler):
+    """Sampling from LoRA-patched SDXL models: the denoising loop of diffusers' StableDiffusionXLPipeline
+    (txt2img) and StableDiffusionXLImg2ImgPipeline (img2img, requires_aesthetics_score=False) over the
+    LoraSampler machinery -- the same three graphs, schedulers, step launches and per-call options.
+
+        s = LoraXLSampler(unet, text_encoder, text_encoder_2, vae,
+                          SamplerConfig(scheduler="euler", num_inference_steps=30, guidance_scale=5.0,
+                                        vae_scaling=0.13025, autocast_dtype=torch.bfloat16),
+                          latent_shape=(1, 4, 128, 128))
+        img = s.sample(input_ids, input_ids_2, seed=0)        # uint8 [B, 1024, 1024, 3] on the device
+
+    The conditioning is the pipeline's encode_prompt (LoraXLTrainStep._predict's): both encoders'
+    penultimate hidden states concatenated ([G*B, 77, 2048]), encoder 2's text_embeds as the pooled
+    conditioning, and `time_ids` [G*B, 6] fp32 (original size, crop top-left, target size) from a static
+    buffer written per call, which costs no capture. With guidance and no negative ids the negative
+    embeddings and pooled embeddings are zeros (force_zeros_for_empty_prompt, SDXL base's setting); with
+    both negative id tensors they are encoded. Zeroed or encoded negatives is a capture key of its own, like
+    the scheduler family and guidance rescale (`SamplerConfig.guidance_rescale` or sample(guidance_rescale=)).
+
+    Refused before any CUDA call: a non-SDXL UNet, encoders that do not fit it, task "inpaint", and an
+    fp16 VAE (SDXL's VAE overflows in fp16; diffusers upcasts it, this sampler asks for fp32 or bf16)."""
+    _sdxl = True
+
+    def __init__(self, unet: nn.Module, text_encoder: nn.Module, text_encoder_2: nn.Module, vae: nn.Module,
+                 cfg: SamplerConfig, latent_shape=(1, 4, 128, 128), seq_len: int = 77, device=None):
+        from .train import _check_xl_models
+        ucfg = getattr(unet, "cfg", None) or getattr(unet, "config", None)
+        if getattr(ucfg, "addition_embed_type", None) != "text_time":
+            raise ValueError("LoraXLSampler samples SDXL UNets (addition_embed_type='text_time'); sample SD 1.x / "
+                             "2.x UNets with LoraSampler")
+        _check_xl_models(unet, text_encoder, text_encoder_2)
+        if cfg.task == "inpaint":
+            raise ValueError("LoraXLSampler does not inpaint: tasks 'txt2img' and 'img2img' only")
+        if any(p.dtype == torch.float16 for p in vae.parameters()):
+            raise ValueError("the SDXL VAE overflows in fp16 (diffusers' SDXL VAE config sets force_upcast): pass it "
+                             "in fp32 or bf16")
+        self.text_encoder_2 = text_encoder_2
+        super().__init__(unet, text_encoder, vae, cfg, latent_shape=latent_shape, seq_len=seq_len, device=device)
+        B, _, h, w = latent_shape
+        dev = self.device
+        self.input_ids_2 = torch.zeros((2 * B, seq_len), device=dev, dtype=torch.long)    # [negative ; prompt]
+        self.time_ids = torch.tensor([[8.0 * h, 8.0 * w, 0.0, 0.0, 8.0 * h, 8.0 * w]] * (2 * B), device=dev,
+                                     dtype=torch.float32)
+        self._added = {}
+        self._zero_negatives = True
+
+    def _lora_models(self):
+        return (self.unet, self.text_encoder, self.text_encoder_2)
+
+    def _key(self, G: int, family: str, rescale: bool):
+        zeros = G == 2 and self._zero_negatives
+        return super()._key(G, family, rescale) + (("zero_negatives",) if zeros else ())
+
+    def _encode(self, G: int):
+        B = self.latents.shape[0]
+        zeros = G == 2 and self._zero_negatives
+        lo = B if G == 1 or zeros else 0
+        out1 = self.text_encoder(self.input_ids[lo:], output_hidden_states=True)
+        out2 = self.text_encoder_2(self.input_ids_2[lo:], output_hidden_states=True)
+        ehs = torch.cat([out1.hidden_states[-2], out2.hidden_states[-2]], dim=-1)
+        pooled = out2.text_embeds
+        if zeros:
+            ehs = torch.cat([torch.zeros_like(ehs), ehs])
+            pooled = torch.cat([torch.zeros_like(pooled), pooled])
+        self._ehs[G] = ehs.to(self.model_dtype)
+        self._added[G] = {"text_embeds": pooled, "time_ids": self.time_ids[(2 - G) * B:]}
+
+    def _unet(self, G: int):
+        return self.unet(self.unet_in[G], self.timestep, self._ehs[G], added_cond_kwargs=self._added[G]).sample
+
+    def prepare(self, guidance_scale: Optional[float] = None, guidance_rescale: Optional[float] = None,
+                encoded_negatives: bool = False):
+        """LoraSampler.prepare, for zeroed (the default call's) or encoded negative prompts."""
+        self._zero_negatives = not encoded_negatives
+        super().prepare(guidance_scale, guidance_rescale)
+
+    def sample(self, input_ids: torch.Tensor, input_ids_2: torch.Tensor,
+               negative_input_ids: Optional[torch.Tensor] = None, negative_input_ids_2: Optional[torch.Tensor] = None,
+               seed: int = 0, original_size=None, crops_coords_top_left=(0, 0), target_size=None,
+               guidance_rescale: Optional[float] = None, num_inference_steps: Optional[int] = None,
+               scheduler: Optional[str] = None, guidance_scale: Optional[float] = None,
+               image: Optional[torch.Tensor] = None, strength: Optional[float] = None) -> torch.Tensor:
+        """uint8 [B, 8h, 8w, 3] images (a view of `self.image`) for the two tokenizers' ids [B, seq_len] of
+        the prompts. The negative prompts' ids come as a pair or not at all (zeroed negatives).
+        original_size and target_size default to (8h, 8w); with crops_coords_top_left they make each
+        sample's time ids. img2img: image uint8 [B, 8h, 8w, 3] and strength, as LoraSampler.sample."""
+        n, sched, g, start = self._options(num_inference_steps, scheduler, guidance_scale, strength)
+        phi = _check_phi(self.cfg.guidance_rescale if guidance_rescale is None else guidance_rescale)
+        G = 2 if g > 1.0 else 1
+        B = self.latents.shape[0]
+        shape = tuple(self.input_ids[B:].shape)
+        _int_ids(input_ids, shape, "input_ids")
+        _int_ids(input_ids_2, shape, "input_ids_2")
+        if (negative_input_ids is None) != (negative_input_ids_2 is None):
+            raise ValueError("give both negative_input_ids and negative_input_ids_2, or neither (zeroed negatives)")
+        encoded = negative_input_ids is not None
+        if encoded:
+            _int_ids(negative_input_ids, shape, "negative_input_ids")
+            _int_ids(negative_input_ids_2, shape, "negative_input_ids_2")
+        _, _, h, w = self.latents.shape
+        sizes = (_pair((8 * h, 8 * w) if original_size is None else original_size, "original_size")
+                 + _pair(crops_coords_top_left, "crops_coords_top_left")
+                 + _pair((8 * h, 8 * w) if target_size is None else target_size, "target_size"))
+        self._set_images(image, None)
+        self._zero_negatives = not encoded
+
+        def write_inputs():
+            self.input_ids[B:].copy_(input_ids)
+            self.input_ids_2[B:].copy_(input_ids_2)
+            if G == 2 and encoded:
+                self.input_ids[:B].copy_(negative_input_ids)
+                self.input_ids_2[:B].copy_(negative_input_ids_2)
+            self.time_ids.copy_(torch.tensor(sizes, dtype=torch.float32).expand(2 * B, 6))
+
+        return self._generate(n, sched, g, start, phi, seed, write_inputs)

@@ -289,6 +289,37 @@ def sample_step_ms(model_out: torch.Tensor, x: torch.Tensor, x0_hist: torch.Tens
     ops._count()
 
 
+def sample_step_rescale(model_out: torch.Tensor, x: torch.Tensor, noise: Optional[torch.Tensor],
+                        x0_hist: Optional[torch.Tensor], table: torch.Tensor, guidance: torch.Tensor,
+                        guidance_rescale: torch.Tensor, step_index: torch.Tensor, counter: torch.Tensor,
+                        unet_in: torch.Tensor, timestep: torch.Tensor, vae_in: torch.Tensor, vae_scaling: float):
+    """One launch of lb_sample_step_rescale, in place on preallocated buffers (nothing is allocated:
+    capturable): a classifier-free-guided step (model_out [2B, C, H, W]) with guidance rescale.
+
+    guidance_rescale: a device fp32 [1] holding phi. x0_hist None: sample_step_ch's single-step update,
+    reading `noise`; x0_hist given: sample_step_ms's multistep update (noise unused, may be None).
+    Per sample, m_hat = m_u + g (m_c - m_u) is scaled by phi * std(m_c) / std(m_hat) + (1 - phi) before
+    the update (diffusers' rescale_noise_cfg); at phi = 0 the result equals sample_step_ch's /
+    sample_step_ms's bit for bit."""
+    Cu = unet_in.shape[1] if unet_in.dim() == 4 else -1
+    if Cu < x.shape[1]:
+        raise _C.LoraB200Error(f"sample_step_rescale: unet_in has {Cu} channels, fewer than the latents' "
+                               f"{x.shape[1]}")
+    if unet_in.shape[0] != 2 * x.shape[0]:
+        raise _C.LoraB200Error("sample_step_rescale: guidance rescale needs classifier-free guidance (G = 2): "
+                               f"unet_in has {unet_in.shape[0]} rows for {x.shape[0]} latents")
+    if (guidance_rescale is None or guidance_rescale.dtype != torch.float32 or guidance_rescale.numel() != 1
+            or guidance_rescale.device != x.device):
+        raise _C.LoraB200Error("sample_step_rescale: guidance_rescale must be a float32 [1] tensor on x's device")
+    head, tail = _sample_step_args(model_out, x, noise, table, guidance, step_index, counter, unet_in, timestep,
+                                   vae_in, vae_scaling, False, Cu, "sample_step_rescale", x0_hist=x0_hist)
+    # head[7] is the noise, or x0_hist in its place: split it into the two pointers; phi follows guidance
+    pair = (ptr(None), head[7]) if x0_hist is not None else (head[7], ptr(None))
+    head = head[:7] + pair + head[8:11] + (ptr(guidance_rescale),) + head[11:]
+    check(_C.lib.lb_sample_step_rescale(*head, Cu, *tail[:-2], tail[-1]), "lb_sample_step_rescale")
+    ops._count()
+
+
 def sample_init(moments: Optional[torch.Tensor], posterior_noise: Optional[torch.Tensor], x: torch.Tensor,
                 noise: torch.Tensor, table: torch.Tensor, step_index: torch.Tensor, counter: torch.Tensor,
                 unet_in: torch.Tensor, timestep: torch.Tensor, scaling: float = 0.18215,
