@@ -39,6 +39,7 @@ import torch
 import torch.nn as nn
 
 import test_kernels_gpu as KG
+from test_kernels_gpu import acc_tol, check_branch, check_rel, check_t, n_sms, tprime, ulp16
 from oracle import lora_ops as O
 
 DEV = "cuda"
@@ -141,10 +142,6 @@ def _ops():
     return ops
 
 
-def n_sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
 def make_member(M, K, N, r, dt, seed, scale, bias=False, diag=False, x=None):
     """KG.make_case's operands on the device; x: the family's shared input (None: the member's own)."""
     x_, W, A, B, b, d = KG.make_case(M, K, N, r, dt, seed, bias=bias, diag=diag)
@@ -162,51 +159,6 @@ def make_family(M, K, Ns, dt, seed, bias):
 
 def shapes(mems):
     return [(m.x.shape[0], m.x.shape[1], m.W.shape[0]) for m in mems]
-
-
-def acc_tol(K):
-    """Bound for a tensor-core reduction over K (module docstring)."""
-    return max(1e-5, K / 16 * 2.0 ** -24)
-
-
-def ulp16(dt):
-    return 2.0 ** -8 if dt == BF else 2.0 ** -11
-
-
-def regions(M, N, bn):
-    """(name, rows, cols): the whole tensor, the last 128-row tile, the last bn-column tile."""
-    return [("all", slice(None), slice(None)), ("last row tile", slice((M - 1) // 128 * 128, None), slice(None)),
-            ("last column tile", slice(None), slice((N - 1) // bn * bn, None))]
-
-
-def check_rel(got, ref, tol, bn, what):
-    got, ref = got.detach().to(DEV, F64), ref.detach().to(DEV, F64)
-    for name, rs, cs in regions(*ref.shape, bn):
-        e = KG.rel_err(got[rs, cs], ref[rs, cs])
-        assert e < tol, f"{what} [{name}]: rel {e:.3e} >= {tol:.1e}"
-
-
-def check_branch(got, ref, base, bn, what):
-    """err <= 2^-7 ||ref - base|| + 1e-5 ||ref|| on every region (base: the frozen GEMM + bias)."""
-    got, ref, base = (t.detach().to(DEV, F64) for t in (got, ref, base))
-    for name, rs, cs in regions(*ref.shape, bn):
-        g, r_, b_ = got[rs, cs], ref[rs, cs], base[rs, cs]
-        err, bound = float((g - r_).norm()), 2.0 ** -7 * float((r_ - b_).norm()) + 1e-5 * float(r_.norm())
-        assert err <= bound, f"{what} [{name}]: err {err:.3e} > {bound:.3e}"
-
-
-def check_t(T, t_ref, r, K, what):
-    """T side output: rel < acc_tol(K) on the whole tensor and the last row tile, padded columns zero."""
-    check_rel(T[:, :r], t_ref, acc_tol(K), r, what)
-    assert torch.count_nonzero(T[:, r:]) == 0, f"{what}: padded rank columns written"
-
-
-def tprime(T, r, scale, diag, dt):
-    """T' as the drain forms it: fp32 T * fp32(scale * diag), rounded to the 16-bit operand type."""
-    coef = torch.full((r,), scale, dtype=F32, device=DEV)
-    if diag is not None:
-        coef = coef * diag.float()
-    return (T[:, :r] * coef).to(dt).to(F64)
 
 
 def problems(mems, dt, tiled=False, scale0=False):

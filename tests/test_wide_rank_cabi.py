@@ -76,3 +76,25 @@ def test_rank_pad():
     for r in (0, 65):
         with pytest.raises(LoraB200Error):
             ops.rank_pad(r)
+
+
+def test_linear_entry_points_refuse_bad_outputs_pointers_and_dropout_without_gpu(L):
+    """lb_lora_linear_fwd / _dropout: output pitch, misaligned operands, drop_p and its seed, output type."""
+    buf = ctypes.create_string_buffer(4096)
+    base = (ctypes.addressof(buf) + 255) & ~255
+    p, q = ctypes.c_void_p(base), ctypes.c_void_p(base + 8)        # q: 8-byte aligned, not 16
+    fwd = lambda X=p, W=p, D=p, Y=p, T=None, T_in=None, N=64, dt=0, odt=0: L.lb_lora_linear_fwd(
+        X, W, None, D, p, 4, 1, None, 1.0, Y, T, T_in, 8, 64, N, 4, 16, dt, odt, None)
+    assert fwd(N=60) == -1 and fwd(N=60, dt=1, odt=1) == -1            # 16-bit output: N % 8
+    assert fwd(N=62, odt=2) == -1                                      # fp32 output: N % 4
+    for arg in ("W", "D", "Y", "T", "T_in"):
+        assert fwd(**{arg: q}) == -4, arg
+    assert fwd(dt=0, odt=1) == -3 and fwd(dt=1, odt=0) == -3           # neither the operand type nor fp32
+    drop = lambda drop_p, seed=p, N=64, odt=0, Y=p, T=None: L.lb_lora_linear_fwd_dropout(
+        p, p, None, p, p, 4, 1, None, 1.0, Y, T, 8, 64, N, 4, 16, 0, odt, drop_p, seed, None)
+    for bad in (1.0, 1.5, -0.1, float("nan")):
+        assert drop(bad) == -1, bad
+    assert drop(0.1, seed=None) == -1
+    assert drop(0.1, N=60) == -1 and drop(0.1, N=62, odt=2) == -1
+    assert drop(0.1, Y=q) == -4 and drop(0.1, T=q) == -4
+    assert drop(0.1, odt=1) == -3
