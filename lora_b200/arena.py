@@ -156,8 +156,7 @@ class LoraArena:
                 taps = kh * kw
                 ktot = taps * cin
                 # down16 [RP, taps*Cin], K index = tap*Cin + c  <- A[r,Cin,kh,kw]
-                for t in range(taps):
-                    rows.append((o_dn + t, cin * taps, taps, r, cin, sh_off + t * cin, ktot, rp))
+                rows += ops.conv_tap_rows(o_dn, sh_off, r, cin, taps, rp)
                 self._shadow_slots.append((s, "down", sh_off, ktot, rp)); sh_off += rp * ktot
                 rows.append((o_up, 1, r, r, cout, sh_off, cout, rp))
                 self._shadow_slots.append((s, "upT", sh_off, cout, rp)); sh_off += rp * cout

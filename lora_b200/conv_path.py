@@ -7,9 +7,10 @@ raises LoraB200Error (there is no eager fallback).
 """
 import torch
 
-from . import ops
+from . import dropout_path, ops
 from ._C import LoraB200Error
-from .modules import _LOW, _SiteState, _compute_dtype, _fp32_master, _key, _out_dtype
+from .modules import (_SiteState, _active_dropout, _compute_dtype, _dx_dtype, _factor_grads, _fp32_master,
+                      _grad_targets, _out_dtype)
 
 
 def _geometry(conv):
@@ -26,42 +27,6 @@ def _geometry(conv):
     return kh, kw, ph, pw
 
 
-def _frozen_conv(st: _SiteState, weight, dtype, need_bwd: bool):
-    k = _key(weight, tag="conv")
-    ent = st.w.get(dtype)
-    if ent is not None and ent[0] != k:
-        ent = None
-    have_f = ent is not None
-    have_b = ent is not None and ent[2] is not None
-    if not have_f or (need_bwd and not have_b):
-        f, b = ops.cast_conv_weight(weight, dtype, not have_f, need_bwd)
-        ent = (k, ent[1] if have_f else f, b if need_bwd else None)
-        st.w[dtype] = ent
-    return ent[1], ent[2]
-
-
-def _down16(st: _SiteState, A, dtype):
-    k = _key(A)
-    ent = st.down.get(dtype)
-    if ent is None or ent[0] != k:
-        if not hasattr(st, "conv_tables"):
-            st.conv_tables = {}
-        ent = (k, ops.conv_down16(A, dtype, st.conv_tables))
-        st.down[dtype] = ent
-    return ent[1]
-
-
-def _upT16(st: _SiteState, B, dtype):
-    k = _key(B)
-    ent = st.upT.get(dtype)
-    if ent is None or ent[0] != k:
-        cout, r = B.shape[0], B.shape[1]
-        src = _fp32_master(B)
-        ent = (k, ops.cast_rows_pad16(src, 1, r, r, cout, dtype))
-        st.upT[dtype] = ent
-    return ent[1]
-
-
 def _nhwc16(x, dtype):
     if x.dtype != dtype:
         x = x.to(dtype)
@@ -69,6 +34,9 @@ def _nhwc16(x, dtype):
 
 
 class _FusedLoraConv2dFn(torch.autograd.Function):
+    """autograd node for one LoRA conv site; with an active nn.Dropout the branch is masked in the
+    forward's drain and the backward recomputes the mask from the saved seed (dropout_path.py)."""
+
     @staticmethod
     def forward(ctx, x, A, B, mod):
         if not x.is_cuda:
@@ -81,60 +49,56 @@ class _FusedLoraConv2dFn(torch.autograd.Function):
         cdt = _compute_dtype(x)
         odt = _out_dtype(x, cdt)
         r = mod.r
-        need_bwd = any(ctx.needs_input_grad[:3])
         x16 = _nhwc16(x, cdt)
-        w_f, _ = _frozen_conv(st, conv.weight, cdt, False)
+        w_f, _ = st.frozen_conv(conv.weight, cdt, False)
         b32 = st.bias32(conv.bias)
-        down16 = _down16(st, A, cdt)
-        B32 = _fp32_master(B)
+        down16 = st.conv_down16(A, cdt)
         diag = mod._selector_diag()
         scale = float(mod.scale)
-        y, T = ops.fused_conv2d(x16, w_f, b32, down16, B32, 0, r, 1, 0, diag, scale, r,
-                                conv.out_channels, kh, kw, ph, pw, False, odt, need_bwd)
-        ctx.mod, ctx.cdt, ctx.scale, ctx.diag = mod, cdt, scale, diag
-        ctx.geom = (kh, kw, ph, pw)
-        ctx.x_dtype = x.dtype
-        ctx.save_for_backward(x16, T, A, B)
+        p = _active_dropout(mod)
+        seed = dropout_path._fresh_seed(mod, x.device) if p > 0.0 else None
+        want_t = p > 0.0 or any(ctx.needs_input_grad[:3])
+        y, T = ops.fused_conv2d(x16, w_f, b32, down16, _fp32_master(B), 0, r, 1, 0, diag, scale, r,
+                                conv.out_channels, kh, kw, ph, pw, False, odt, want_t, drop_p=p, seed=seed)
+        ctx.mod, ctx.cdt, ctx.scale, ctx.p, ctx.diag = mod, cdt, scale, p, diag
+        ctx.geom, ctx.x_dtype = (kh, kw, ph, pw), x.dtype
+        ctx.save_for_backward(x16, T, A, B, *([] if seed is None else [seed]))
         return y
 
     @staticmethod
     def backward(ctx, gy):
         mod = ctx.mod
         st: _SiteState = mod._lb
-        x16, T, A, B = ctx.saved_tensors
+        x16, T, A, B, *seed = ctx.saved_tensors
         conv = mod.conv
         kh, kw, ph, pw = ctx.geom
         taps = kh * kw
-        cin, cout, r = conv.in_channels, conv.out_channels, mod.r
+        cin, cout, r, p = conv.in_channels, conv.out_channels, mod.r, ctx.p
         cdt = ctx.cdt
         gy16 = _nhwc16(gy, cdt)
         n, _, h, w = gy16.shape
-        _, w_b = _frozen_conv(st, conv.weight, cdt, True)
-        upT16 = _upT16(st, B, cdt)
+        gy2d = gy16.permute(0, 2, 3, 1).reshape(n * h * w, cout)       # NHWC bytes as [pixels, Cout]
+        _, w_b = st.frozen_conv(conv.weight, cdt, True)
+        upT16 = st.upT16(B, cdt)
         A32 = _fp32_master(A)
-        dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
         # dX = conv_T(gY, W) + conv_T((gY.B)*s*d, A); "up" = A read flipped: element (c, tap g, j)
         # at A[j, c, taps-1-g]  ->  base offset taps-1, up_rs = taps, up_cs = cin*taps, up_gs = -1
-        # (rank pads 32 / 64: the entry computes dTs = gY.B first and runs the taps through it)
+        # (rank pads 32 / 64: the entry computes dTs = gY.B first and runs the taps through it);
+        # with dropout one masked pass gives dTs = (mask o gY / (1-p)) . B first and dX takes it (T_in)
+        t_in = ops.dropout_dt(gy2d, _fp32_master(B), r, 1, p, seed[0], r) if p > 0.0 else None
         dX, dTs = ops.fused_conv2d(gy16, w_b, None, upT16, A32, taps - 1, taps, cin * taps, -1,
                                    ctx.diag, ctx.scale, r, cin, kh, kw, kh - 1 - ph, kw - 1 - pw,
-                                   True, dx_dtype, True)
+                                   True, _dx_dtype(ctx.x_dtype), t_in is None, t_in=t_in)
+        dTs = dTs if t_in is None else t_in
         need_x, need_a, need_b = ctx.needs_input_grad[:3]
-        sink = st.grad_sink
-        dA = dB = None
+        tA, tB, deferrable = _grad_targets(st, need_a, need_b, (r, cin * taps), (cout, r), gy.device)
         if need_a:
-            tgt = sink[0] if sink is not None else torch.zeros((r, cin * taps), device=gy.device,
-                                                               dtype=torch.float32)
-            ops.wgrad_conv(x16, dTs, ctx.diag, ctx.scale, tgt, r, cin, h, w, kh, kw, ph, pw, deferrable=sink is not None)
-            if sink is None:
-                dA = tgt.view_as(A).to(A.dtype)
-        if need_b:
-            tgt = sink[1] if sink is not None else torch.zeros((cout, r), device=gy.device,
-                                                               dtype=torch.float32)
-            gy2d = gy16.permute(0, 2, 3, 1).reshape(n * h * w, cout)       # NHWC bytes as [pixels, Cout]
-            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tgt, 1, r, r, deferrable=sink is not None)
-            if sink is None:
-                dB = tgt.view_as(B).to(B.dtype)
+            ops.wgrad_conv(x16, dTs, ctx.diag, ctx.scale, tA, r, cin, h, w, kh, kw, ph, pw, deferrable=deferrable)
+        if need_b and p > 0.0:      # dB reduces the masked gY
+            ops.wgrad_masked(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, p, seed[0], deferrable=deferrable)
+        elif need_b:
+            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, deferrable=deferrable)
+        dA, dB = _factor_grads(tA, tB, deferrable, A, B)
         dx = dX.to(ctx.x_dtype) if need_x else None
         return dx, dA, dB, None
 
@@ -143,7 +107,4 @@ def lora_conv2d(mod, x):
     if mod.r > ops.MAX_RANK:
         raise LoraB200Error(f"LoraInjectedConv2d: LoRA rank {mod.r} > {ops.MAX_RANK} is not supported by the "
                             "fused conv kernel (linear sites run as rank chunks, rank_chunks.py)")
-    if mod.training and mod.dropout.p > 0.0:
-        from .dropout_path import lora_conv2d_dropout
-        return lora_conv2d_dropout(mod, x)
     return _FusedLoraConv2dFn.apply(x, mod.lora_down.weight, mod.lora_up.weight, mod)

@@ -20,7 +20,8 @@ from typing import List, Optional
 import torch
 
 from . import ops
-from .modules import _LOW, _SiteState, _compute_dtype, _fp32_master, _out_dtype
+from .modules import (_SiteState, _active_dropout, _compute_dtype, _dx_dtype, _factor_grads, _fp32_master,
+                      _grad_targets, _out_dtype, _rows, _split_mode)
 
 _ENABLED = False
 
@@ -84,10 +85,7 @@ def _key(x: torch.Tensor):
 
 
 def _plain(site, x) -> bool:
-    from . import modules
-    if site.training and site.dropout.p > 0.0:
-        return False
-    if (modules._FP32_MODE == "split" and x.dtype == torch.float32 and not torch.is_autocast_enabled("cuda")):
+    if _active_dropout(site) or _split_mode(x):
         return False
     return x.is_cuda and site.linear.in_features == x.shape[-1]
 
@@ -98,9 +96,7 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
         cdt = _compute_dtype(x)
         odt = _out_dtype(x, cdt)
         K = x.shape[-1]
-        x2d = x.reshape(-1, K)
-        if x2d.dtype != cdt or not x2d.is_contiguous():
-            x2d = x2d.to(cdt).contiguous()
+        x2d = _rows(x, K, cdt)
         need_bwd = any(ctx.needs_input_grad)
         probs, meta = [], []
         for i, m in enumerate(members):
@@ -127,7 +123,7 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
         Ts = saved[1:1 + ctx.n_T]
         factors = saved[1 + ctx.n_T:]
         K = x2d.shape[1]
-        dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
+        dx_dtype = _dx_dtype(ctx.x_dtype)
         live = [i for i, g in enumerate(gys) if g is not None]
         probs, g2ds = [], {}
         for i in live:
@@ -135,10 +131,7 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
             A, B = factors[2 * i], factors[2 * i + 1]
             st: _SiteState = m._lb
             N = m.linear.out_features
-            g2d = gys[i].reshape(-1, N)
-            if g2d.dtype != cdt or not g2d.is_contiguous():
-                g2d = g2d.to(cdt).contiguous()
-            g2ds[i] = g2d
+            g2d = g2ds[i] = _rows(gys[i], N, cdt)
             _, wt16 = st.frozen(m.linear.weight, cdt, need_t=True)
             diag, scale = ctx.meta[i]
             probs.append((g2d, wt16, None, st.upT16(B, cdt), _fp32_master(A), 1, K, diag, scale, m.r))
@@ -155,25 +148,18 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
                 N, r = m.linear.out_features, m.r
                 diag, scale = ctx.meta[i]
                 need_a, need_b = ctx.needs_input_grad[2 + 2 * i], ctx.needs_input_grad[3 + 2 * i]
-                sink = st.grad_sink
-                tA = tB = None
-                if need_a:
-                    tA = sink[0] if sink is not None else torch.zeros((r, K), device=x2d.device, dtype=torch.float32)
-                if need_b:
-                    tB = sink[1] if sink is not None else torch.zeros((N, r), device=x2d.device, dtype=torch.float32)
+                tA, tB, deferrable = _grad_targets(st, need_a, need_b, (r, K), (N, r), x2d.device)
                 if need_a and need_b:
                     multi.append((dTs[j], tA, g2ds[i], Ts[i], tB, diag, scale, r))
                 elif need_a:
-                    ops.wgrad(x2d, dTs[j], diag, scale, tA, K, 1, r, deferrable=sink is not None)
+                    ops.wgrad(x2d, dTs[j], diag, scale, tA, K, 1, r, deferrable=deferrable)
                 elif need_b:
-                    ops.wgrad(g2ds[i], Ts[i], diag, scale, tB, 1, r, r, deferrable=sink is not None)
-                temps.append((i, sink, tA, tB, A, B, need_a, need_b))
+                    ops.wgrad(g2ds[i], Ts[i], diag, scale, tB, 1, r, r, deferrable=deferrable)
+                temps.append((i, tA, tB, deferrable, A, B))
             if multi:
                 ops.wgrad_multi(x2d, multi, deferrable=all_sink)   # every dA/dB of the family: one launch
-            for (i, sink, tA, tB, A, B, need_a, need_b) in temps:
-                if sink is None:
-                    grads[2 * i] = tA.to(A.dtype).view_as(A) if need_a else None
-                    grads[2 * i + 1] = tB.to(B.dtype).view_as(B) if need_b else None
+            for (i, tA, tB, deferrable, A, B) in temps:
+                grads[2 * i], grads[2 * i + 1] = _factor_grads(tA, tB, deferrable, A, B)
             if ctx.needs_input_grad[0]:
                 acc = dXs[0]
                 for extra in dXs[1:]:

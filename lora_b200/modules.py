@@ -24,7 +24,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import dropout_path, ops
 from ._C import LoraB200Error
 
 _LOW = (torch.bfloat16, torch.float16)
@@ -106,8 +106,7 @@ def invalidate_caches(model: nn.Module):
             st.down.clear()
             st.upT.clear()
             st.bias = None
-            if hasattr(st, "w3"):      # precise_path.py's split-bf16 copies
-                st.w3 = None
+            st.w3 = None
 
 
 class _SiteState:
@@ -117,10 +116,12 @@ class _SiteState:
     (lora.py:290,302-303,706-711; cli_svd.py:52-53)."""
 
     def __init__(self):
-        self.w = {}        # dtype -> (key, w16, wt16)
+        self.w = {}        # dtype -> (key, w16, wt16); a conv site: (key, forward operand, dX operand)
         self.bias = None   # (key, bias fp32)
-        self.down = {}     # dtype -> (key, down16 [RP,K]), RP = ops.rank_pad(r)
+        self.down = {}     # dtype -> (key, down16 [RP,K]), RP = ops.rank_pad(r); a conv site: K = taps*Cin
         self.upT = {}      # dtype -> (key, upT16 [RP,N])
+        self.w3 = None     # (key, W, W^T or None) as split-bf16 [.., 3K] (precise_path.py)
+        self.conv_tables = {}  # ops.conv_tap_table's tables: they follow the factor's shape, never its values
         self.grad_sink = None  # (gA view, gB view) when the arena owns the gradients
         self.parent = None     # weakref to the module this site was injected into (grouping.py)
 
@@ -166,6 +167,21 @@ class _SiteState:
             self.w[slot] = ent
         return ent[1], ent[2]
 
+    def frozen_conv(self, weight: torch.Tensor, dtype, need_bwd: bool):
+        """16-bit operands of a frozen conv weight (ops.cast_conv_weight): (forward [Cout, taps*Cin],
+        input-gradient [Cin, taps*Cout] or None)."""
+        k = _key(weight, tag="conv")
+        ent = self.w.get(dtype)
+        if ent is not None and ent[0] != k:
+            ent = None
+        have_f = ent is not None
+        have_b = ent is not None and ent[2] is not None
+        if not have_f or (need_bwd and not have_b):
+            f, b = ops.cast_conv_weight(weight, dtype, not have_f, need_bwd)
+            ent = (k, ent[1] if have_f else f, b if need_bwd else None)
+            self.w[dtype] = ent
+        return ent[1], ent[2]
+
     def bias32(self, bias: Optional[torch.Tensor]):
         if bias is None:
             return None
@@ -180,21 +196,26 @@ class _SiteState:
         ent = self.down.get(dtype)
         if ent is None or ent[0] != k:
             r, K = a2d.shape
-            src = a2d.detach()
-            src = src if src.dtype == torch.float32 and src.is_contiguous() else src.float().contiguous()
-            ent = (k, ops.cast_rows_pad16(src, K, 1, r, K, dtype))
+            ent = (k, ops.cast_rows_pad16(_fp32_master(a2d), K, 1, r, K, dtype))
             self.down[dtype] = ent
         return ent[1]
 
-    def upT16(self, b2d: torch.Tensor, dtype):
-        """B [N,r] fp32 master -> B^T [RP,N] 16-bit, rows r.. zero."""
-        k = _key(b2d)
+    def conv_down16(self, a4d: torch.Tensor, dtype):
+        """A [r,Cin,kh,kw] fp32 master -> [RP, taps*Cin] 16-bit, tap-major (ops.conv_down16)."""
+        k = _key(a4d)
+        ent = self.down.get(dtype)
+        if ent is None or ent[0] != k:
+            ent = (k, ops.conv_down16(a4d, dtype, self.conv_tables))
+            self.down[dtype] = ent
+        return ent[1]
+
+    def upT16(self, b: torch.Tensor, dtype):
+        """B [N,r] (a conv site: [Cout,r,1,1]) fp32 master -> B^T [RP,N] 16-bit, rows r.. zero."""
+        k = _key(b)
         ent = self.upT.get(dtype)
         if ent is None or ent[0] != k:
-            N, r = b2d.shape
-            src = b2d.detach()
-            src = src if src.dtype == torch.float32 and src.is_contiguous() else src.float().contiguous()
-            ent = (k, ops.cast_rows_pad16(src, 1, r, r, N, dtype))
+            N, r = b.shape[0], b.shape[1]
+            ent = (k, ops.cast_rows_pad16(_fp32_master(b), 1, r, r, N, dtype))
             self.upT[dtype] = ent
         return ent[1]
 
@@ -206,9 +227,54 @@ def _fp32_master(w: torch.Tensor) -> torch.Tensor:
     return d
 
 
+# ---- what every site's autograd function shares (fused linear / conv, precise, rank chunks, grouped)
+def _rows(t: torch.Tensor, C: int, cdt) -> torch.Tensor:
+    """t as contiguous [M, C] rows of dtype cdt (the x2d / gy2d operands)."""
+    t2d = t.reshape(-1, C)
+    if t2d.dtype != cdt or not t2d.is_contiguous():
+        t2d = t2d.to(cdt).contiguous()
+    return t2d
+
+
+def _dx_dtype(x_dtype: torch.dtype) -> torch.dtype:
+    """dX is computed in the activation's own 16-bit type, else in fp32."""
+    return x_dtype if x_dtype in _LOW else torch.float32
+
+
+def _grad_targets(st: _SiteState, need_a: bool, need_b: bool, a_shape, b_shape, device):
+    """(tA, tB, deferrable): where dA / dB accumulate. With an arena these are its gradient views,
+    which feed only the optimizer, so their reductions may be deferred (ops.wgrad_defer_begin);
+    otherwise fresh fp32 zeros. A target is None when its factor needs no gradient."""
+    sink = st.grad_sink
+    if sink is not None:
+        return (sink[0] if need_a else None), (sink[1] if need_b else None), True
+    z = lambda shape: torch.zeros(shape, device=device, dtype=torch.float32)
+    return (z(a_shape) if need_a else None), (z(b_shape) if need_b else None), False
+
+
+def _factor_grads(tA, tB, deferrable: bool, A: torch.Tensor, B: torch.Tensor):
+    """(dA, dB) for autograd: None when the targets are the arena's (the gradients are in place)."""
+    if deferrable:
+        return None, None
+    return (None if tA is None else tA.to(A.dtype).view_as(A)), (None if tB is None else tB.to(B.dtype).view_as(B))
+
+
+def _active_dropout(mod) -> float:
+    """p of the site's nn.Dropout when it acts (training mode and p > 0), else 0."""
+    p = float(mod.dropout.p)
+    return p if mod.training and p > 0.0 else 0.0
+
+
+def _split_mode(x: torch.Tensor) -> bool:
+    """Whether the fp32-faithful split-bf16 policy (set_fp32_mode("split")) applies to this input."""
+    return _FP32_MODE == "split" and x.dtype == torch.float32 and not torch.is_autocast_enabled("cuda")
+
+
 class _FusedLoraLinearFn(torch.autograd.Function):
     """autograd node for one LoRA linear site. Inputs A, B are passed so that autograd knows the
-    factors are used; W and bias are frozen (train_lora_dreambooth.py:595) and never get grads."""
+    factors are used; W and bias are frozen (train_lora_dreambooth.py:595) and never get grads.
+    With an active nn.Dropout the forward masks the branch in the kernel's drain and the backward
+    recomputes the same mask from the saved seed (dropout_path.py)."""
 
     @staticmethod
     def forward(ctx, x, A, B, mod):
@@ -218,71 +284,67 @@ class _FusedLoraLinearFn(torch.autograd.Function):
             raise LoraB200Error("LoraInjectedLinear.forward: lora_b200 runs on CUDA tensors only")
         cdt = _compute_dtype(x)
         odt = _out_dtype(x, cdt)
-        K = lin.in_features
-        N = lin.out_features
-        r = mod.r
-        x2d = x.reshape(-1, K)
-        if x2d.dtype != cdt or not x2d.is_contiguous():
-            x2d = x2d.to(cdt).contiguous()
-        need_bwd = any(ctx.needs_input_grad[:3])
+        K, N, r = lin.in_features, lin.out_features, mod.r
+        x2d = _rows(x, K, cdt)
         w16, _ = st.frozen(lin.weight, cdt, need_t=False)
         b32 = st.bias32(lin.bias)
-        A32 = _fp32_master(A)
-        B32 = _fp32_master(B)
         down16 = st.down16(A, cdt)
         diag = mod._selector_diag()
         scale = float(mod.scale)
-        drop = mod.dropout.p if (mod.training and mod.dropout.p > 0.0) else 0.0
-        if drop > 0.0:
-            raise LoraB200Error("dropout>0 in training mode is handled by _FusedLoraLinearDropoutFn")
-        y, T = ops.fused_linear(x2d, w16, b32, down16, B32, r, 1, diag, scale, r, odt, need_bwd)
-        ctx.mod = mod
-        ctx.cdt = cdt
-        ctx.scale = scale
-        ctx.x_shape = x.shape
-        ctx.x_dtype = x.dtype
-        ctx.diag = diag
-        ctx.save_for_backward(x2d, T, A, B)
+        p = _active_dropout(mod)
+        seed = dropout_path._fresh_seed(mod, x.device) if p > 0.0 else None
+        want_t = p > 0.0 or any(ctx.needs_input_grad[:3])
+        y, T = ops.fused_linear(x2d, w16, b32, down16, _fp32_master(B), r, 1, diag, scale, r, odt, want_t,
+                                drop_p=p, seed=seed)
+        ctx.mod, ctx.cdt, ctx.scale, ctx.p, ctx.diag = mod, cdt, scale, p, diag
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.save_for_backward(x2d, T, A, B, *([] if seed is None else [seed]))
         return y.view(*x.shape[:-1], N)
 
     @staticmethod
     def backward(ctx, gy):
         mod = ctx.mod
         st: _SiteState = mod._lb
-        x2d, T, A, B = ctx.saved_tensors
+        x2d, T, A, B, *seed = ctx.saved_tensors
         lin = mod.linear
-        K, N, r = lin.in_features, lin.out_features, mod.r
+        K, N, r, p = lin.in_features, lin.out_features, mod.r, ctx.p
         cdt = ctx.cdt
-        gy2d = gy.reshape(-1, N)
-        if gy2d.dtype != cdt or not gy2d.is_contiguous():
-            gy2d = gy2d.to(cdt).contiguous()
+        gy2d = _rows(gy, N, cdt)
         _, wt16 = st.frozen(lin.weight, cdt, need_t=True)
         upT16 = st.upT16(B, cdt)
         A32 = _fp32_master(A)
-        # dX = gY.W + ((gY.B) * s*d).A ; dTs = gY.B   (same fused kernel, transposed operands)
-        dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
+        # dX = gY.W + (dTs * s*d).A, dTs = gY.B   (same fused kernel, transposed operands); with dropout
+        # one masked pass gives dTs = (mask o gY / (1-p)) . B first and the dX kernel takes it (T_in)
+        t_in = ops.dropout_dt(gy2d, _fp32_master(B), r, 1, p, seed[0], r) if p > 0.0 else None
         dX, dTs = ops.fused_linear(gy2d, wt16, None, upT16, A32, 1, K, ctx.diag, ctx.scale, r,
-                                   dx_dtype, True)
-        need_x, need_a, need_b = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        sink = st.grad_sink
-        dA = dB = None
-        tA = tB = None
-        if need_a:
-            tA = sink[0] if sink is not None else torch.zeros((r, K), device=gy.device, dtype=torch.float32)
-        if need_b:
-            tB = sink[1] if sink is not None else torch.zeros((N, r), device=gy.device, dtype=torch.float32)
-        deferrable = sink is not None      # straight into the arena: nothing downstream waits for it
-        if need_a and need_b:
+                                   _dx_dtype(ctx.x_dtype), t_in is None, t_in=t_in)
+        dTs = dTs if t_in is None else t_in
+        need_x, need_a, need_b = ctx.needs_input_grad[:3]
+        tA, tB, deferrable = _grad_targets(st, need_a, need_b, (r, K), (N, r), gy.device)
+        if need_a and need_b and p == 0.0:
             ops.wgrad_pair(x2d, dTs, tA, gy2d, T, tB, ctx.diag, ctx.scale, r, deferrable=deferrable)
-        elif need_a:
-            ops.wgrad(x2d, dTs, ctx.diag, ctx.scale, tA, K, 1, r, deferrable=deferrable)
-        elif need_b:
-            ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, deferrable=deferrable)
-        if sink is None:
-            dA = tA.to(A.dtype).view_as(A) if need_a else None
-            dB = tB.to(B.dtype).view_as(B) if need_b else None
+        else:
+            if need_a:
+                ops.wgrad(x2d, dTs, ctx.diag, ctx.scale, tA, K, 1, r, deferrable=deferrable)
+            if need_b and p > 0.0:      # dB reduces the masked gY
+                ops.wgrad_masked(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, p, seed[0], deferrable=deferrable)
+            elif need_b:
+                ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r, deferrable=deferrable)
+        dA, dB = _factor_grads(tA, tB, deferrable, A, B)
         dx = dX.view(ctx.x_shape).to(ctx.x_dtype) if need_x else None
         return dx, dA, dB, None
+
+
+def _selector_diag(self) -> Optional[torch.Tensor]:
+    sel = self.selector
+    if isinstance(sel, nn.Identity):
+        return None
+    w = sel.weight.detach()
+    return torch.diagonal(w.reshape(self.r, self.r)).to(torch.float32).contiguous()
+
+
+def realize_as_lora(self):
+    return self.lora_up.weight.data * self.scale, self.lora_down.weight.data
 
 
 class LoraInjectedLinear(nn.Module):
@@ -307,34 +369,24 @@ class LoraInjectedLinear(nn.Module):
         nn.init.zeros_(self.lora_up.weight)
         self._lb = _SiteState()
 
-    def _selector_diag(self) -> Optional[torch.Tensor]:
-        sel = self.selector
-        if isinstance(sel, nn.Identity):
-            return None
-        w = sel.weight.detach()
-        return torch.diagonal(w.reshape(self.r, self.r)).to(torch.float32).contiguous()
+    _selector_diag = _selector_diag
+    realize_as_lora = realize_as_lora
 
     def forward(self, input):
         ops.wgrad_segment_boundary()
         if self.r > ops.MAX_RANK:   # joined LoRAs above rank 64 (lora_manager.py:13-71): rank chunks of 64
             from .rank_chunks import lora_linear_chunked
             return lora_linear_chunked(self, input)
-        if self.training and self.dropout.p > 0.0:
-            from .dropout_path import lora_linear_dropout
-            return lora_linear_dropout(self, input)
-        if (_FP32_MODE == "split" and input.dtype == torch.float32 and self.linear.weight.dtype == torch.float32
-                and not torch.is_autocast_enabled("cuda")):
-            from .precise_path import lora_linear_precise
-            return lora_linear_precise(self, input)
-        from . import grouping
-        if grouping._ENABLED and self._lb.parent is not None:
-            out = grouping.forward_maybe_grouped(self, input)
-            if out is not None:
-                return out
+        if not _active_dropout(self):
+            if _split_mode(input) and self.linear.weight.dtype == torch.float32:
+                from .precise_path import lora_linear_precise
+                return lora_linear_precise(self, input)
+            from . import grouping
+            if grouping._ENABLED and self._lb.parent is not None:
+                out = grouping.forward_maybe_grouped(self, input)
+                if out is not None:
+                    return out
         return _FusedLoraLinearFn.apply(input, self.lora_down.weight, self.lora_up.weight, self)
-
-    def realize_as_lora(self):
-        return self.lora_up.weight.data * self.scale, self.lora_down.weight.data
 
     def set_selector_from_diag(self, diag: torch.Tensor):
         assert diag.shape == (self.r,)
@@ -373,20 +425,13 @@ class LoraInjectedConv2d(nn.Module):
         nn.init.zeros_(self.lora_up.weight)
         self._lb = _SiteState()
 
-    def _selector_diag(self) -> Optional[torch.Tensor]:
-        sel = self.selector
-        if isinstance(sel, nn.Identity):
-            return None
-        w = sel.weight.detach()
-        return torch.diagonal(w.reshape(self.r, self.r)).to(torch.float32).contiguous()
+    _selector_diag = _selector_diag
+    realize_as_lora = realize_as_lora
 
     def forward(self, input):
         ops.wgrad_segment_boundary()
         from .conv_path import lora_conv2d
         return lora_conv2d(self, input)
-
-    def realize_as_lora(self):
-        return self.lora_up.weight.data * self.scale, self.lora_down.weight.data
 
     def set_selector_from_diag(self, diag: torch.Tensor):
         assert diag.shape == (self.r,)

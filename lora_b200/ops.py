@@ -113,12 +113,14 @@ def _req_cuda(*ts):
             raise _C.LoraB200Error("lora_b200 kernels need CUDA tensors (no CPU path)")
 
 
-def cast_rows_pad16(src: torch.Tensor, rs: int, cs: int, r: int, C: int, dtype) -> torch.Tensor:
-    """fp32 factor -> zero-padded 16-bit [rank_pad(r), C] operand (see lb_cast_rows_pad)."""
+def cast_rows_pad16(src: torch.Tensor, rs: int, cs: int, r: int, C: int, dtype,
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 factor -> zero-padded 16-bit [rank_pad(r), C] operand (see lb_cast_rows_pad); `out`: re-cast
+    into that existing operand in place."""
     _req_cuda(src)
-    rp = rank_pad(r) if r >= 1 else R_PAD
-    out = torch.empty((rp, C), device=src.device, dtype=dtype)
-    check(_C.lib.lb_cast_rows_pad(ptr(src), rs, cs, ptr(out), r, rp, C, dtype_code(dtype), stream_ptr()),
+    if out is None:
+        out = torch.empty((rank_pad(r) if r >= 1 else R_PAD, C), device=src.device, dtype=dtype)
+    check(_C.lib.lb_cast_rows_pad(ptr(src), rs, cs, ptr(out), r, out.shape[0], C, dtype_code(dtype), stream_ptr()),
           "lb_cast_rows_pad")
     _count()
     return out
@@ -256,23 +258,37 @@ def cast_conv_weight(w: torch.Tensor, dtype, want_fwd: bool, want_bwd: bool):
     return f, b
 
 
-def conv_down16(a4d: torch.Tensor, dtype, table_cache: dict) -> torch.Tensor:
-    """A [r,Cin,kh,kw] fp32 -> [rank_pad(r), kh*kw*Cin] 16-bit with K ordered tap-major, channel-minor."""
-    _req_cuda(a4d)
+def conv_tap_rows(src_off: int, dst_off: int, r: int, cin: int, taps: int, rp: int):
+    """lb_refresh_shadows rows that re-cast a conv down factor A [r,Cin,kh,kw] (fp32, `src_off` elements
+    into the source) to its [rp, taps*Cin] 16-bit operand (`dst_off` into the destination), whose K
+    index is tap-major, channel-minor: one row per tap."""
+    return [(src_off + t, cin * taps, taps, r, cin, dst_off + t * cin, taps * cin, rp) for t in range(taps)]
+
+
+def conv_tap_table(a4d: torch.Tensor, table_cache: dict) -> torch.Tensor:
+    """conv_down16's row table for a down factor shaped like a4d, built once per shape and device
+    into `table_cache` (an upload: build it before a graph capture that re-casts through it)."""
     r, cin, kh, kw = a4d.shape
-    taps = kh * kw
-    rp = rank_pad(r)
-    key = (r, cin, taps, a4d.device)
+    key = (r, cin, kh * kw, a4d.device)
     tab = table_cache.get(key)
     if tab is None:
-        rows = [(t, cin * taps, taps, r, cin, t * cin, taps * cin, rp) for t in range(taps)]
-        tab = torch.tensor(rows, device=a4d.device, dtype=torch.int64)
+        tab = torch.tensor(conv_tap_rows(0, 0, r, cin, kh * kw, rank_pad(r)), device=a4d.device, dtype=torch.int64)
         table_cache[key] = tab
+    return tab
+
+
+def conv_down16(a4d: torch.Tensor, dtype, table_cache: dict, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """A [r,Cin,kh,kw] fp32 -> [rank_pad(r), kh*kw*Cin] 16-bit with K ordered tap-major, channel-minor;
+    `out`: re-cast into that existing operand in place."""
+    _req_cuda(a4d)
+    r, cin, kh, kw = a4d.shape
+    tab = conv_tap_table(a4d, table_cache)
     src = a4d.detach()
     if src.dtype != torch.float32 or not src.is_contiguous():
         src = src.float().contiguous()
-    out = torch.empty((rp, taps * cin), device=a4d.device, dtype=dtype)
-    check(_C.lib.lb_refresh_shadows(ptr(src), ptr(tab), taps, cin, ptr(out), dtype_code(dtype), stream_ptr()),
+    if out is None:
+        out = torch.empty((rank_pad(r), kh * kw * cin), device=a4d.device, dtype=dtype)
+    check(_C.lib.lb_refresh_shadows(ptr(src), ptr(tab), kh * kw, cin, ptr(out), dtype_code(dtype), stream_ptr()),
           "lb_refresh_shadows")
     _count()
     return out

@@ -17,7 +17,7 @@ import torch
 
 from . import _C, ops
 from ._C import LoraB200Error, check, ptr, stream_ptr
-from .modules import _SiteState, _fp32_master, _key
+from .modules import _SiteState, _factor_grads, _fp32_master, _grad_targets, _key, _rows
 
 
 def _split(src2d: torch.Tensor, pattern: int, rows_pad: int = 0) -> torch.Tensor:
@@ -35,7 +35,7 @@ def _split(src2d: torch.Tensor, pattern: int, rows_pad: int = 0) -> torch.Tensor
 
 def _frozen3(st: _SiteState, weight: torch.Tensor, need_t: bool):
     k = _key(weight)
-    ent = getattr(st, "w3", None)
+    ent = st.w3
     if ent is None or ent[0] != k:
         ent = (k, _split(weight, 1), None)
     if need_t and ent[2] is None:
@@ -52,9 +52,7 @@ class _PreciseLoraLinearFn(torch.autograd.Function):
         st: _SiteState = mod._lb
         lin = mod.linear
         K, N, r = lin.in_features, lin.out_features, mod.r
-        x2d = x.reshape(-1, K)
-        if not x2d.is_contiguous():
-            x2d = x2d.contiguous()
+        x2d = _rows(x, K, torch.float32)
         need_bwd = any(ctx.needs_input_grad[:3])
         w3, _ = _frozen3(st, lin.weight, False)
         b32 = st.bias32(lin.bias)
@@ -74,29 +72,21 @@ class _PreciseLoraLinearFn(torch.autograd.Function):
         x2d, T, A, B = ctx.saved_tensors
         lin = mod.linear
         K, N, r = lin.in_features, lin.out_features, mod.r
-        gy2d = gy.reshape(-1, N).float()
-        if not gy2d.is_contiguous():
-            gy2d = gy2d.contiguous()
+        gy2d = _rows(gy, N, torch.float32)
         _, wt3 = _frozen3(st, lin.weight, True)
         upT3 = _split(_fp32_master(B).t().contiguous(), 1, rows_pad=ops.rank_pad(r))   # B^T [r,N] -> [RP,3N]
         dX, dTs = ops.fused_linear(_split(gy2d, 0), wt3, None, upT3, _fp32_master(A), 1, K, ctx.diag,
                                    ctx.scale, r, torch.float32, True)
         need_x, need_a, need_b = ctx.needs_input_grad[:3]
-        sink = st.grad_sink
-        tA = tB = dA = dB = None
-        if need_a:
-            tA = sink[0] if sink is not None else torch.zeros((r, K), device=gy.device, dtype=torch.float32)
-        if need_b:
-            tB = sink[1] if sink is not None else torch.zeros((N, r), device=gy.device, dtype=torch.float32)
+        tA, tB, sunk = _grad_targets(st, need_a, need_b, (r, K), (N, r), gy.device)
+        # launched at once, never queued: `sunk` only decides what autograd gets back
         if need_a and need_b:
             ops.wgrad_pair(x2d, dTs, tA, gy2d, T, tB, ctx.diag, ctx.scale, r)
         elif need_a:
             ops.wgrad(x2d, dTs, ctx.diag, ctx.scale, tA, K, 1, r)
         elif need_b:
             ops.wgrad(gy2d, T, ctx.diag, ctx.scale, tB, 1, r, r)
-        if sink is None:
-            dA = tA.to(A.dtype).view_as(A) if need_a else None
-            dB = tB.to(B.dtype).view_as(B) if need_b else None
+        dA, dB = _factor_grads(tA, tB, sunk, A, B)
         return (dX.view(ctx.x_shape) if need_x else None), dA, dB, None
 
 

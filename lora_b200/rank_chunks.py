@@ -15,7 +15,8 @@ import torch
 
 from . import ops
 from ._C import LoraB200Error
-from .modules import _LOW, _SiteState, _compute_dtype, _fp32_master, _out_dtype
+from .modules import (_SiteState, _active_dropout, _compute_dtype, _dx_dtype, _factor_grads, _fp32_master,
+                      _grad_targets, _out_dtype, _rows)
 
 CH = 64
 
@@ -29,16 +30,14 @@ class _ChunkedLoraLinearFn(torch.autograd.Function):
     def forward(ctx, x, A, B, mod):
         if not x.is_cuda:
             raise LoraB200Error("LoraInjectedLinear.forward: lora_b200 runs on CUDA tensors only")
-        if mod.training and mod.dropout.p > 0.0:
+        if _active_dropout(mod):
             raise LoraB200Error("LoRA rank > 64 with active dropout is not supported (train with r <= 64, "
                                 "or call .eval() / set dropout.p = 0 on joined LoRAs)")
         st: _SiteState = mod._lb
         lin = mod.linear
         cdt, K, N, r = _compute_dtype(x), lin.in_features, lin.out_features, mod.r
         odt = _out_dtype(x, cdt)
-        x2d = x.reshape(-1, K)
-        if x2d.dtype != cdt or not x2d.is_contiguous():
-            x2d = x2d.to(cdt).contiguous()
+        x2d = _rows(x, K, cdt)
         w16, _ = st.frozen(lin.weight, cdt, need_t=False, tiled=False)
         b32 = st.bias32(lin.bias)
         A32, B32 = _fp32_master(A), _fp32_master(B)
@@ -69,19 +68,12 @@ class _ChunkedLoraLinearFn(torch.autograd.Function):
         x2d, A, B, *Ts = ctx.saved_tensors
         lin = mod.linear
         K, N, r, cdt = lin.in_features, lin.out_features, mod.r, ctx.cdt
-        gy2d = gy.reshape(-1, N)
-        if gy2d.dtype != cdt or not gy2d.is_contiguous():
-            gy2d = gy2d.to(cdt).contiguous()
+        gy2d = _rows(gy, N, cdt)
         _, wt16 = st.frozen(lin.weight, cdt, need_t=True, tiled=False)
         A32, B32 = _fp32_master(A), _fp32_master(B)
-        dx_dtype = ctx.x_dtype if ctx.x_dtype in _LOW else torch.float32
+        dx_dtype = _dx_dtype(ctx.x_dtype)
         need_x, need_a, need_b = ctx.needs_input_grad[:3]
-        sink = st.grad_sink
-        tA = tB = None
-        if need_a:
-            tA = sink[0] if sink is not None else torch.zeros((r, K), device=gy.device, dtype=torch.float32)
-        if need_b:
-            tB = sink[1] if sink is not None else torch.zeros((N, r), device=gy.device, dtype=torch.float32)
+        tA, tB, sunk = _grad_targets(st, need_a, need_b, (r, K), (N, r), gy.device)
         seed0 = torch.zeros(1, device=gy.device, dtype=torch.int64)
         dX = None
         for c, (j0, j1) in enumerate(_chunks(r)):
@@ -97,10 +89,7 @@ class _ChunkedLoraLinearFn(torch.autograd.Function):
                 ops.wgrad(x2d, dT, dg, ctx.scale, tA[j0:], K, 1, rc)
             if need_b:
                 ops.wgrad(gy2d, Ts[c], dg, ctx.scale, tB[:, j0:], 1, r, rc)
-        dA = dB = None
-        if sink is None:
-            dA = tA.to(A.dtype).view_as(A) if need_a else None
-            dB = tB.to(B.dtype).view_as(B) if need_b else None
+        dA, dB = _factor_grads(tA, tB, sunk, A, B)
         dx = dX.view(ctx.x_shape).to(ctx.x_dtype) if need_x else None
         return dx, dA, dB, None
 

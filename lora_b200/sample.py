@@ -58,7 +58,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from . import _C, ops
+from . import ops
 from .host import schedulers
 from .step_ops import (pixels_emit, pixels_ingest, pixels_ingest_inpaint, sample_init, sample_step, sample_step_ch,
                        sample_step_ms, sample_step_rescale)
@@ -170,6 +170,7 @@ class LoraSampler:
         self._graphs = {}             # (G, scheduler family[, "rescale"]) -> (A, B, C)
         self._fingerprint = None
         self._factor_bufs = []
+        self._conv_tables = {}        # ops.conv_tap_table's row tables of the conv sites' down factors
         self.captures = 0
 
     # ------------------------------------------------------------------ what a capture bakes in
@@ -193,33 +194,22 @@ class LoraSampler:
         for m in _sites(*self._lora_models()):
             if m.r > ops.MAX_RANK:        # rank chunks cast their factors inside every forward
                 continue
-            tab = None
-            if type(m).__name__ == "LoraInjectedConv2d":      # the tap-major row table of ops.conv_down16
-                r, cin, kh, kw = m.lora_down.weight.shape
-                taps, rp = kh * kw, ops.rank_pad(r)
-                tab = torch.tensor([(t, cin * taps, taps, r, cin, t * cin, taps * cin, rp) for t in range(taps)],
-                                   device=self.device, dtype=torch.int64)
+            if type(m).__name__ == "LoraInjectedConv2d":      # its re-cast walks a row table: upload it now
+                ops.conv_tap_table(m.lora_down.weight, self._conv_tables)
             for dt, (_, buf) in list(m._lb.down.items()):
-                bufs.append((m, dt, buf, tab))
+                bufs.append((m, dt, buf))
         self._factor_bufs = bufs
 
     def _refresh_factors(self):
         """Re-cast every held down-factor copy from the factor's current value (an arena step, an
         in-place optimizer update and a `.data` edit all leave the fused forward's copy stale)."""
-        for m, dt, buf, tab in self._factor_bufs:
+        for m, dt, buf in self._factor_bufs:
             a = m.lora_down.weight.detach()
-            if a.dtype != torch.float32 or not a.is_contiguous():
-                a = a.float().contiguous()
-            r = m.r
             if type(m).__name__ == "LoraInjectedLinear":
-                K = a.shape[1]
-                _C.check(_C.lib.lb_cast_rows_pad(_C.ptr(a), K, 1, _C.ptr(buf), r, buf.shape[0], K, _C.dtype_code(dt),
-                                                 _C.stream_ptr()), "lb_cast_rows_pad")
+                a = a if a.dtype == torch.float32 and a.is_contiguous() else a.float().contiguous()
+                ops.cast_rows_pad16(a, a.shape[1], 1, m.r, a.shape[1], dt, out=buf)
             else:
-                _, cin, kh, kw = a.shape
-                _C.check(_C.lib.lb_refresh_shadows(_C.ptr(a), _C.ptr(tab), kh * kw, cin, _C.ptr(buf),
-                                                   _C.dtype_code(dt), _C.stream_ptr()), "lb_refresh_shadows")
-            ops._count()
+                ops.conv_down16(a, dt, self._conv_tables, out=buf)
 
     def _lora_models(self):
         """The models whose LoRA sites the sampler covers (fingerprint, factor refresh, eval mode)."""

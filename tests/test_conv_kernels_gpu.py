@@ -2,8 +2,8 @@
 and of its factor-gradient reductions (lb_lora_wgrad_conv, lb_lora_wgrad) against float64 references:
 oracle/lora_ops.py and plain float64 F.conv2d / conv2d_input / conv2d_weight, evaluated on the GPU.
 
-The kernels are called as the autograd glue calls them (conv_path.py forward and backward,
-dropout_path.py), at every SD1.5 512-px conv site and at ragged shapes. The census is chosen so that
+The kernels are called as the autograd glue calls them (conv_path.py forward and backward, with and
+without dropout), at every SD1.5 512-px conv site and at ragged shapes. The census is chosen so that
 it reaches every launch branch of conv2d_fwd_impl; `conv_plan` restates that selection and an
 unmarked CPU test checks the coverage.
 
@@ -509,7 +509,7 @@ def test_conv_split_plan_inside_a_cuda_graph():
 @pytest.mark.parametrize("case", DROP_CASES, ids=lambda c: "n{}_{}x{}_{}to{}_k{}_r{}_{}_p{}".format(
     *c[:7], str(c[7])[6:], c[8]))
 def test_conv_dropout_matches_oracle_with_the_exact_mask(case):
-    """Forward (masked drain) and backward (dropout_path.py: masked dT pass, dX from T_in, dA, masked
+    """Forward (masked drain) and backward (conv_path.py with p > 0: masked dT pass, dX from T_in, dA, masked
     dB) against the oracle fed the mask of oracle/dropmask.py."""
     ops = _ops()
     n, H, W, cin, cout, k, r, dt, p = case
@@ -540,7 +540,7 @@ def test_conv_dropout_matches_oracle_with_the_exact_mask(case):
             check_branch(y, ref, base, "dropout forward vs oracle")
             T = t
 
-    # backward, as dropout_path._LoraConv2dDropoutFn.backward
+    # backward, as conv_path._FusedLoraConv2dFn.backward with p > 0
     gy2d = nchw_to_rows(gy)
     dTs = ops.dropout_dt(gy2d, B, r, 1, p, seed_t, r)
     dts_ref = torch.einsum("nohw,oj->njhw", gy.to(F64) * mask / (1.0 - p), B.to(F64))
@@ -567,7 +567,7 @@ def test_conv_dropout_matches_oracle_with_the_exact_mask(case):
 @gpu
 @pytest.mark.parametrize("r", [4, 40])
 def test_linear_dropout_matches_oracle_with_the_exact_mask(r):
-    """The same for a linear site (fused_linear with drop_p; dropout_path._LoraLinearDropoutFn)."""
+    """The same for a linear site (fused_linear with drop_p; modules._FusedLoraLinearFn with p > 0)."""
     ops = _ops()
     M, K, N, p, scale, dt = 333, 320, 640, 0.25, 1.5, BF
     g = torch.Generator().manual_seed(r)

@@ -612,9 +612,9 @@ def test_linear_launch_matches_float64(case, dt):
 
 # ==================================================================================== T_in
 def tin_operands(M, K, N, r, dt, seed):
-    """The dX launch of dropout_path.py: gY [M, N] on W^T (wt16) and B^T (upT16), up = A read
-    transposed, and a dTs that is NOT gY . B16: independent values, padded columns included (the
-    kernel must ignore columns >= r)."""
+    """The dX launch of a dropout site's backward (modules._FusedLoraLinearFn): gY [M, N] on W^T (wt16)
+    and B^T (upT16), up = A read transposed, and a dTs that is NOT gY . B16: independent values, padded
+    columns included (the kernel must ignore columns >= r)."""
     ops = _ops()
     x, W, A, B, _, d = device_case(M, K, N, r, dt, seed, False, True)
     g = torch.Generator().manual_seed(seed)
@@ -665,7 +665,7 @@ def linear_mask(seed, p, M, N):
 @pytest.mark.parametrize("case", DROP_CASES, ids=lambda c: c[0])
 def test_dropout_launch_matches_oracle_with_the_exact_mask(case, dt):
     """Forward (masked drain) with fp32 and 16-bit output against the model and the oracle fed the
-    mask of oracle/dropmask.py; with `chain`, the backward of dropout_path._LoraLinearDropoutFn:
+    mask of oracle/dropmask.py; with `chain`, the backward of modules._FusedLoraLinearFn with p > 0:
     masked dT pass, dX from T_in, dA, masked dB."""
     ops = _ops()
     name, M, K, N, r, p, chain = case
