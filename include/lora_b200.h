@@ -91,6 +91,38 @@ int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W
                                float* const* T_out, const int* M, const int* K, const int* N,
                                const int* r, int in_dtype, int out_dtype, void* stream);
 
+/* Per-sample LoRA coefficients (forward only): lb_lora_linear_fwd without T_out / T_in, where the
+ * rank-r activations of output row m are scaled by a row of the fp32 table coef [samples, coef_ld]
+ * (device memory, coef_ld >= r) instead of by scale * diag:
+ *     Y[m,:] = X[m,:] . W^T (+ bias) + ((X[m,:] . down^T) * coef[s(m), 0:r]) . up^T,
+ *     s(m) = (m / rows_per_sample) % samples
+ * rows_per_sample = the rows of one batch element (77 tokens, H*W pixels, 1); the modulo maps every
+ * copy of a sample in a batch of k * samples (the [uncond ; cond] halves of classifier-free guidance)
+ * to the same coefficient row. Each image of a batch gets its own LoRA scale and selector mix in the
+ * same launch; the table's values may change between graph replays. Every forward plan of
+ * lb_lora_linear_fwd runs (r_pad 16 / 32 / 64, split-K, 16-bit or fp32 outputs); a table whose rows
+ * all equal fl32(scale * diag) gives lb_lora_linear_fwd's result bit for bit. Not for dropout or
+ * backward. */
+int lb_lora_linear_fwd_ps(const void* X, const void* W, const float* bias, const void* down,
+                          const float* up, long long up_rs, long long up_cs, const float* coef,
+                          int coef_ld, int rows_per_sample, int samples, void* Y, int M, int K, int N,
+                          int r, int r_pad, int in_dtype, int out_dtype, void* stream);
+
+/* The L2 split-K factor lb_lora_linear_fwd / lb_lora_linear_fwd_ps pick for a dropout-free forward of
+ * this shape on the current device (1: a plan without L2 split-K). Split plans add their partials at
+ * L2 in arrival order, so their results may differ in the last bits from run to run; every other plan
+ * repeats its bits. LB_ERR_SHAPE for a bad shape. */
+int lb_lora_linear_fwd_split_k(int M, int K, int N, int r_pad);
+
+/* lb_lora_linear_fwd_grouped with per-sample coefficients (see lb_lora_linear_fwd_ps): one table per
+ * problem, coef / coef_ld / rows_per_sample / samples are host arrays of length n (r <= 16). */
+int lb_lora_linear_fwd_grouped_ps(int n, const void* const* X, const void* const* W,
+                                  const float* const* bias, const void* const* down16,
+                                  const float* const* up, const long long* up_rs, const long long* up_cs,
+                                  const float* const* coef, const int* coef_ld, const int* rows_per_sample,
+                                  const int* samples, void* const* Y, const int* M, const int* K,
+                                  const int* N, const int* r, int in_dtype, int out_dtype, void* stream);
+
 /* Benchmark/profiling knob: tile schedule of lb_lora_linear_fwd.
  *   mode = schedule + 4 * block_n + 16 * split
  *   schedule: 0 = auto (default), 1 and 2 = one tile per CTA, 3 = split-K with the partials
@@ -222,6 +254,19 @@ int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const float* bias, 
                                int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
                                int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
                                void* stream);
+
+/* The L2 split-K factor lb_lora_conv2d_fwd / lb_lora_conv2d_fwd_ps pick for a forward (direction) conv
+ * of this shape on the current device (1: none), as lb_lora_linear_fwd_split_k. */
+int lb_lora_conv2d_fwd_split_k(int n_img, int H, int Wd, int Cin, int Cout, int kh, int kw, int r_pad);
+
+/* lb_lora_conv2d_fwd (forward direction) with per-sample coefficients (see lb_lora_linear_fwd_ps):
+ * pixel row m = (img*H + h)*W + w takes coef row ((m / rows_per_sample) % samples); rows_per_sample
+ * = H*W makes the sample the image. No T_out / T_in, dropout or input-gradient form. */
+int lb_lora_conv2d_fwd_ps(const void* X, const void* W, const float* bias, const void* down,
+                          const float* up, long long up_rs, long long up_cs, const float* coef,
+                          int coef_ld, int rows_per_sample, int samples, void* Y, int n_img, int H,
+                          int Wd, int Cin, int Cout, int kh, int kw, int pad_h, int pad_w, int r,
+                          int r_pad, int in_dtype, int out_dtype, void* stream);
 
 /* Frozen conv-weight preparation: src [Cout,Cin,kh,kw] (LB_F32/LB_BF16/LB_F16) ->
  *   dst16  [Cout, kh*kw*Cin]  (tap-major K; forward operand)              and/or

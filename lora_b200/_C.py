@@ -127,6 +127,14 @@ def _load():
         "lb_lora_up_dropout": ([vp, i32, vp, vp, ll, ll, vp, f32, f32, vp, i32, i32, i32, i32, vp], i32),
         "lb_lora_dropout_dt": ([vp, i32, vp, ll, ll, f32, vp, vp, i32, i32, i32, i32, vp], i32),
         "lb_lora_wgrad_masked": ([vp, vp, vp, f32, vp, ll, ll, i32, i32, i32, i32, f32, vp, i32, vp], i32),
+        "lb_lora_linear_fwd_ps": ([vp, vp, vp, vp, vp, ll, ll, vp, i32, i32, i32, vp,
+                                   i32, i32, i32, i32, i32, i32, i32, vp], i32),
+        "lb_lora_linear_fwd_grouped_ps": ([i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                           i32, i32, vp], i32),
+        "lb_lora_linear_fwd_split_k": ([i32, i32, i32, i32], i32),
+        "lb_lora_conv2d_fwd_split_k": ([i32, i32, i32, i32, i32, i32, i32, i32], i32),
+        "lb_lora_conv2d_fwd_ps": ([vp, vp, vp, vp, vp, ll, ll, vp, i32, i32, i32, vp,
+                                   i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp], i32),
     }
     for name, s in sig.items():
         if s is None or not hasattr(lib, name):
@@ -167,7 +175,9 @@ EXPORTED = [n for n in ("lb_abi_version", "lb_lora_linear_fwd", "lb_lora_wgrad",
                         "lb_optim_step_fused", "lb_step_prologue", "lb_step_prologue_v", "lb_masked_mse_fwd_bwd",
                         "lb_pixels_ingest", "lb_step_prologue_posterior", "lb_sample_step", "lb_pixels_emit",
                         "lb_sample_step_ch", "lb_sample_step_ms", "lb_sample_step_rescale", "lb_sample_init", "lb_pixels_ingest_inpaint",
-                        "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight")]
+                        "lb_optim_step_dp", "lb_ipc_export", "lb_ipc_open", "lb_lora_wgrad_batch", "lb_tiled_weight_elems", "lb_tile_weight",
+                        "lb_lora_linear_fwd_ps", "lb_lora_linear_fwd_grouped_ps", "lb_lora_conv2d_fwd_ps",
+                        "lb_lora_linear_fwd_split_k", "lb_lora_conv2d_fwd_split_k")]
 
 
 def check(status: int, what: str):

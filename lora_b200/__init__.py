@@ -6,6 +6,7 @@ from .lora import (_find_children, _find_modules, _find_modules_v2, _text_lora_p
 
 from .modules import get_fp32_mode, set_fp32_mode  # noqa: F401,E402
 from .grouping import get_grouping, link_sites, set_grouping  # noqa: F401,E402
+from .per_sample import per_sample_lora  # noqa: F401,E402
 # lora_diffusion/__init__.py:5 re-exports lora_manager's names at package level
 from .join import DummySafeTensorObject, LoRAManager, lora_join  # noqa: F401,E402
 

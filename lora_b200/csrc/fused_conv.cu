@@ -90,6 +90,21 @@ static int launch_conv_wide(const void* X, const void* W, const void* Dn, void* 
 #undef LB_CONVW
 }
 
+// Pixel rectangle of a CTA (TH x TW = 128 rows) and the rectangles per image.
+static void conv_tiling(int H, int Wd, int& TH, int& TW, int& tiles_h, int& tiles_w) {
+  TW = Wd >= 16 ? 16 : 8;
+  TH = BLOCK_M / TW;
+  tiles_h = (H + TH - 1) / TH;
+  tiles_w = (Wd + TW - 1) / TW;
+}
+
+// The L2 split-K factor of a rank-pad-16 conv launch (1: none); g = T groups (1 forward, taps for dX).
+static int conv_l2_split(int n_img, int tiles_h, int tiles_w, int taps, int Cin, int Cout, int g) {
+  const int cblocks = (Cin + BLOCK_K - 1) / BLOCK_K;
+  return plan_conv_split(static_cast<long long>(n_img) * tiles_h * tiles_w, taps * cblocks, Cout, g,
+                         sm_count()).split;
+}
+
 }  // namespace lb
 
 static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
@@ -98,7 +113,8 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
                                   void* Y, float* T_out, const float* T_in, int n_img, int H, int Wd, int Cin,
                                   int Cout, int kh, int kw, int pad_h, int pad_w, int r, int r_pad,
                                   int per_tap_T, int in_dtype, int out_dtype, float drop_p,
-                                  const void* seed_dev, void* stream) {
+                                  const void* seed_dev, void* stream, const float* coef = nullptr,
+                                  int coef_ld = 0, int rows_per_sample = 1, int samples = 1) {
   using namespace lb;
   if (r_pad != 16 && r_pad != 32 && r_pad != 64) return LB_ERR_SHAPE;
   if (!(drop_p >= 0.f && drop_p < 1.f) || (drop_p > 0.f && (seed_dev == nullptr || T_in != nullptr || per_tap_T != 0)))
@@ -128,12 +144,12 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
   p.M = n_img * H * Wd; p.N = Cout; p.K = taps * Cin; p.r = r;
   p.fmt = (in_dtype == LB_BF16) ? 1 : 0;
   p.H = H; p.W = Wd; p.C = Cin; p.kh = kh; p.kw = kw; p.pad_h = pad_h; p.pad_w = pad_w;
-  p.TW = Wd >= 16 ? 16 : 8; p.TH = BLOCK_M / p.TW;
-  p.tiles_h = (H + p.TH - 1) / p.TH; p.tiles_w = (Wd + p.TW - 1) / p.TW;
+  conv_tiling(H, Wd, p.TH, p.TW, p.tiles_h, p.tiles_w);
   const bool groups = per_tap_T != 0 && taps > 1;
   p.down_per_tap = groups ? 0 : 1;
   p.drop_p = drop_p; p.drop_inv = 1.f / (1.f - drop_p);
   p.seed = reinterpret_cast<const unsigned long long*>(seed_dev);
+  p.coef = coef; p.coef_ld = coef_ld; p.rows_per_sample = rows_per_sample; p.samples = samples;
   p.t_group = groups ? pad_h * kw + pad_w : 0;   // the tap with zero shift
   const int down_cols = groups ? Cin : taps * Cin;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -152,9 +168,7 @@ static int conv2d_fwd_impl(const void* X, const void* W, const float* bias,
     return r_pad == 32 ? launch_conv_wide<32>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, drop_p > 0.f, groups, narrow)
                        : launch_conv_wide<64>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, drop_p > 0.f, groups, narrow);
 #define LB_CONV(BN, OT, GG) launch_conv<BN, 4, OT, GG>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
-  const int cblocks = (Cin + BLOCK_K - 1) / BLOCK_K;
-  const ConvPlan sp = plan_conv_split(static_cast<long long>(n_img) * p.tiles_h * p.tiles_w, taps * cblocks, Cout,
-                                      groups ? taps : 1, sm_count());
+  const ConvPlan sp = {0, conv_l2_split(n_img, p.tiles_h, p.tiles_w, taps, Cin, Cout, groups ? taps : 1)};
   if (drop_p > 0.f) {   // forward with dropout on the branch: masked in the drain (DROP kernels)
 #define LB_CONVD(BN, OT) launch_conv<BN, 4, OT, 1, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st)
 #define LB_CONVDS(BN, OT) launch_conv<BN, 4, OT, 1, true, true>(X, W, down16, Y, p, n_img, down_cols, out_dtype, st, sp.split)
@@ -208,4 +222,26 @@ extern "C" int lb_lora_conv2d_fwd_dropout(const void* X, const void* W, const fl
   return conv2d_fwd_impl(X, W, bias, down, up, up_rs, up_cs, 0, diag, scale, Y, T_out, nullptr, n_img, H,
                          Wd, Cin, Cout, kh, kw, pad_h, pad_w, r, r_pad, 0, in_dtype, out_dtype, drop_p, seed_dev,
                          stream);
+}
+
+extern "C" int lb_lora_conv2d_fwd_ps(const void* X, const void* W, const float* bias, const void* down,
+                                     const float* up, long long up_rs, long long up_cs, const float* coef,
+                                     int coef_ld, int rows_per_sample, int samples, void* Y, int n_img, int H,
+                                     int Wd, int Cin, int Cout, int kh, int kw, int pad_h, int pad_w, int r,
+                                     int r_pad, int in_dtype, int out_dtype, void* stream) {
+  if (coef == nullptr || coef_ld < r || rows_per_sample < 1 || samples < 1) return LB_ERR_SHAPE;
+  return conv2d_fwd_impl(X, W, bias, down, up, up_rs, up_cs, 0, nullptr, 1.f, Y, nullptr, nullptr, n_img, H, Wd,
+                         Cin, Cout, kh, kw, pad_h, pad_w, r, r_pad, 0, in_dtype, out_dtype, 0.f, nullptr, stream,
+                         coef, coef_ld, rows_per_sample, samples);
+}
+
+extern "C" int lb_lora_conv2d_fwd_split_k(int n_img, int H, int Wd, int Cin, int Cout, int kh, int kw, int r_pad) {
+  using namespace lb;
+  if (n_img <= 0 || H <= 0 || Wd <= 0 || Cin <= 0 || Cout <= 0 || kh <= 0 || kw <= 0 ||
+      (r_pad != 16 && r_pad != 32 && r_pad != 64))
+    return LB_ERR_SHAPE;
+  if (r_pad != R_PAD) return 1;
+  int TH, TW, tiles_h, tiles_w;
+  conv_tiling(H, Wd, TH, TW, tiles_h, tiles_w);
+  return conv_l2_split(n_img, tiles_h, tiles_w, kh * kw, Cin, Cout, 1);
 }

@@ -92,6 +92,11 @@ struct FusedParams {
   float* ws;
   unsigned int* counters;
   unsigned long long* dbg;  // profiling only: 16 x %globaltimer stamps written by CTA (0,0), or null
+  // per-sample coefficients (forward, no DROP / TAPLOOP): when set, output row m scales rank column j
+  // by coef[((m / rows_per_sample) % samples) * coef_ld + j] instead of scale * diag[j] (rows past M:
+  // row 0). `% samples` maps both halves of a [uncond B ; cond B] guidance batch to the same image.
+  const float* coef;
+  int coef_ld, rows_per_sample, samples;
 };
 
 // B-operand tile of the frozen weight: rows [n0, n0 + BLOCK_N) x K block kb (global index, conv: tap-major).
@@ -459,19 +464,30 @@ __device__ __forceinline__ void fused_tile(const CUtensorMap& tmX, const CUtenso
   if (ct < EPI_THREADS) {
     // ------------------------------------------------------------ epilogue part 1 (row per thread)
     // T is scaled 16 columns at a time: t[RP] and coef[RP] at once would not fit beside the accumulator
+    // per-sample coefficients: forward forms only (one T group, no dropout); the others keep the
+    // scalar coefficients, loaded before the row index as they always were
+    constexpr bool PS = G == 1 && !DROP;
+    const float* crow = nullptr;   // this row's coefficient row, or null: scale * diag
     float coef[16];
     auto load_coef = [&](const int j0) {
 #pragma unroll
       for (int j = 0; j < 16; ++j)
-        coef[j] = (j0 + j < p.r) ? p.scale * (p.diag ? __ldg(p.diag + j0 + j) : 1.f) : 0.f;
+        coef[j] = (j0 + j < p.r) ? ((PS && crow != nullptr) ? __ldg(crow + j0 + j)
+                                                            : p.scale * (p.diag ? __ldg(p.diag + j0 + j) : 1.f))
+                                 : 0.f;
     };
-    if constexpr (RP == R_PAD) load_coef(0);
+    if constexpr (RP == R_PAD && !PS) load_coef(0);
     if constexpr (CONV) {
       const int hh = h0 + row / p.TW, ww = w0 + row % p.TW;
       if (hh < p.H && ww < p.W) grow = (static_cast<long long>(img) * p.H + hh) * p.W + ww;
     } else {
       if (m0 + row < p.M) grow = m0 + row;
     }
+    if constexpr (PS) {   // grow < M fits an int; rows past M take row 0
+      if (p.coef != nullptr)
+        crow = p.coef + ((grow < 0 ? 0 : static_cast<int>(grow)) / p.rows_per_sample % p.samples) * p.coef_ld;
+    }
+    if constexpr (RP == R_PAD && PS) load_coef(0);
     auto tap_touched = [&](int g) {   // did this CTA's K range feed tap g's T columns?
       return !SPLITK || G == 1 || (kb_begin < (g + 1) * cblocks && kb_end > g * cblocks);
     };

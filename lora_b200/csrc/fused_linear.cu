@@ -130,6 +130,13 @@ static int launch_linear_wide(const void* X, const void* W, const void* Dn, void
 static int g_linear_mode = 0;
 static unsigned long long* g_dbg = nullptr;  // profiling: device buffer of 16 timestamps
 
+// The L2 split-K factor lb_lora_linear_fwd's auto schedule picks for a dropout-free forward (1: none;
+// only rank pad 16 has split plans). Those plans reduce their partials in arrival order.
+static int auto_l2_split(int M, int K, int N, int r_pad) {
+  if (r_pad != R_PAD || (g_linear_mode & 3) != 0) return 1;
+  return plan_split(M, K, N, sm_count()).split;
+}
+
 }  // namespace lb
 
 // Tuning knob (benchmarks / profiling only): force the tile schedule of lb_lora_linear_fwd.
@@ -161,7 +168,8 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
                                   long long up_cs, const float* diag, float scale, void* Y,
                                   float* T_out, const float* T_in, int M, int K, int N, int r, int r_pad,
                                   int in_dtype, int out_dtype, float drop_p, const void* seed_dev,
-                                  void* stream) {
+                                  void* stream, const float* coef = nullptr, int coef_ld = 0,
+                                  int rows_per_sample = 1, int samples = 1) {
   using namespace lb;
   const int w_tiled = (in_dtype & LB_W_TILED) ? 1 : 0;
   in_dtype &= ~LB_W_TILED;
@@ -186,6 +194,7 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
   p.fmt = (in_dtype == LB_BF16) ? 1 : 0; p.t_group = 0; p.dbg = g_dbg; p.w_tiled = w_tiled;
   p.drop_p = drop_p; p.drop_inv = 1.f / (1.f - drop_p);
   p.seed = reinterpret_cast<const unsigned long long*>(seed_dev);
+  p.coef = coef; p.coef_ld = coef_ld; p.rows_per_sample = rows_per_sample; p.samples = samples;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (r_pad > R_PAD) {
     const int bn_choice = (g_linear_mode >> 2) & 3;
@@ -213,12 +222,12 @@ static int linear_fwd_impl(const void* X, const void* W, const float* bias,
                : launch_linear<128, 4, uint16_t, 1, true>(X, W, down16, Y, p, out_dtype, st);
   }
 
-  if ((g_linear_mode & 3) == 0) {
-    const SplitPlan sp = plan_split(M, K, N, sm_count());
-    if (sp.split > 1) {
+  {
+    const int l2 = auto_l2_split(M, K, N, r_pad);
+    if (l2 > 1) {
       if (out_dtype == LB_F32)
-        return launch_linear<64, 5, float, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split);
-      return launch_linear<64, 6, uint16_t, 1, false, true>(X, W, down16, Y, p, out_dtype, st, sp.split);
+        return launch_linear<64, 5, float, 1, false, true>(X, W, down16, Y, p, out_dtype, st, l2);
+      return launch_linear<64, 6, uint16_t, 1, false, true>(X, W, down16, Y, p, out_dtype, st, l2);
     }
   }
   const int sched = g_linear_mode & 3, bn_choice = (g_linear_mode >> 2) & 3, split_choice = g_linear_mode >> 4;
@@ -304,13 +313,34 @@ extern "C" int lb_lora_linear_fwd_dropout(const void* X, const void* W, const fl
                          in_dtype, out_dtype, drop_p, seed_dev, stream);
 }
 
-extern "C" int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W,
-                                          const float* const* bias, const void* const* down16,
-                                          const float* const* up, const long long* up_rs,
-                                          const long long* up_cs, const float* const* diag,
-                                          const float* scale, void* const* Y, float* const* T_out,
-                                          const int* M, const int* K, const int* N, const int* r,
-                                          int in_dtype, int out_dtype, void* stream) {
+extern "C" int lb_lora_linear_fwd_split_k(int M, int K, int N, int r_pad) {
+  if (M <= 0 || K <= 0 || N <= 0 || (r_pad != 16 && r_pad != 32 && r_pad != 64)) return LB_ERR_SHAPE;
+  return lb::auto_l2_split(M, K, N, r_pad);
+}
+
+// Per-sample coefficient table [samples, coef_ld] fp32 (lb_lora_*_fwd_ps): valid shape?
+static bool coef_ok(const float* coef, int coef_ld, int rows_per_sample, int samples, int r) {
+  return coef != nullptr && coef_ld >= r && rows_per_sample >= 1 && samples >= 1;
+}
+
+extern "C" int lb_lora_linear_fwd_ps(const void* X, const void* W, const float* bias, const void* down,
+                                     const float* up, long long up_rs, long long up_cs, const float* coef,
+                                     int coef_ld, int rows_per_sample, int samples, void* Y, int M, int K,
+                                     int N, int r, int r_pad, int in_dtype, int out_dtype, void* stream) {
+  if (!coef_ok(coef, coef_ld, rows_per_sample, samples, r)) return LB_ERR_SHAPE;
+  return linear_fwd_impl(X, W, bias, down, up, up_rs, up_cs, nullptr, 1.f, Y, nullptr, nullptr, M, K, N, r,
+                         r_pad, in_dtype, out_dtype, 0.f, nullptr, stream, coef, coef_ld, rows_per_sample, samples);
+}
+
+static int linear_fwd_grouped_impl(int n, const void* const* X, const void* const* W,
+                                   const float* const* bias, const void* const* down16,
+                                   const float* const* up, const long long* up_rs,
+                                   const long long* up_cs, const float* const* diag,
+                                   const float* scale, void* const* Y, float* const* T_out,
+                                   const int* M, const int* K, const int* N, const int* r,
+                                   int in_dtype, int out_dtype, void* stream,
+                                   const float* const* coef = nullptr, const int* coef_ld = nullptr,
+                                   const int* rows_per_sample = nullptr, const int* samples = nullptr) {
   using namespace lb;
   const int w_tiled = (in_dtype & LB_W_TILED) ? 1 : 0;
   in_dtype &= ~LB_W_TILED;
@@ -331,8 +361,12 @@ extern "C" int lb_lora_linear_fwd_grouped(int n, const void* const* X, const voi
     FusedParams p = {};
     p.bias = bias ? bias[i] : nullptr; p.up = up[i]; p.up_rs = up_rs[i]; p.up_cs = up_cs[i]; p.up_gs = 0;
     p.diag = diag ? diag[i] : nullptr; p.t_out = T_out ? T_out[i] : nullptr; p.t_in = nullptr;
-    p.scale = scale[i]; p.M = M[i]; p.N = N[i]; p.K = K[i]; p.r = r[i];
+    p.scale = scale ? scale[i] : 1.f; p.M = M[i]; p.N = N[i]; p.K = K[i]; p.r = r[i];
     p.fmt = (in_dtype == LB_BF16) ? 1 : 0; p.t_group = 0; p.dbg = nullptr; p.w_tiled = w_tiled;
+    if (coef != nullptr) {
+      if (!coef_ok(coef[i], coef_ld[i], rows_per_sample[i], samples[i], r[i])) return LB_ERR_SHAPE;
+      p.coef = coef[i]; p.coef_ld = coef_ld[i]; p.rows_per_sample = rows_per_sample[i]; p.samples = samples[i];
+    }
     a.p[i] = p;
     tiles128 += static_cast<long long>((M[i] + 127) / 128) * ((N[i] + 127) / 128);
     tiles64 += static_cast<long long>((M[i] + 127) / 128) * ((N[i] + 63) / 64);
@@ -348,4 +382,28 @@ extern "C" int lb_lora_linear_fwd_grouped(int n, const void* const* X, const voi
                    : launch_grouped<64, 7, uint16_t, 1>(a, X, W, down16, Y, out_dtype, st);
   return crowded ? launch_grouped<128, 2, uint16_t, 2, true>(a, X, W, down16, Y, out_dtype, st)
                  : launch_grouped<128, 4, uint16_t, 1>(a, X, W, down16, Y, out_dtype, st);
+}
+
+extern "C" int lb_lora_linear_fwd_grouped(int n, const void* const* X, const void* const* W,
+                                          const float* const* bias, const void* const* down16,
+                                          const float* const* up, const long long* up_rs,
+                                          const long long* up_cs, const float* const* diag,
+                                          const float* scale, void* const* Y, float* const* T_out,
+                                          const int* M, const int* K, const int* N, const int* r,
+                                          int in_dtype, int out_dtype, void* stream) {
+  return linear_fwd_grouped_impl(n, X, W, bias, down16, up, up_rs, up_cs, diag, scale, Y, T_out, M, K, N, r,
+                                 in_dtype, out_dtype, stream);
+}
+
+extern "C" int lb_lora_linear_fwd_grouped_ps(int n, const void* const* X, const void* const* W,
+                                             const float* const* bias, const void* const* down16,
+                                             const float* const* up, const long long* up_rs,
+                                             const long long* up_cs, const float* const* coef,
+                                             const int* coef_ld, const int* rows_per_sample, const int* samples,
+                                             void* const* Y, const int* M, const int* K, const int* N,
+                                             const int* r, int in_dtype, int out_dtype, void* stream) {
+  if (coef == nullptr || coef_ld == nullptr || rows_per_sample == nullptr || samples == nullptr)
+    return LB_ERR_SHAPE;
+  return linear_fwd_grouped_impl(n, X, W, bias, down16, up, up_rs, up_cs, nullptr, nullptr, Y, nullptr, M, K, N,
+                                 r, in_dtype, out_dtype, stream, coef, coef_ld, rows_per_sample, samples);
 }

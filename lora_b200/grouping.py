@@ -19,7 +19,7 @@ from typing import List, Optional
 
 import torch
 
-from . import ops
+from . import ops, per_sample
 from .modules import (_SiteState, _active_dropout, _compute_dtype, _dx_dtype, _factor_grads, _fp32_master,
                       _grad_targets, _out_dtype, _rows, _split_mode)
 
@@ -98,17 +98,25 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
         K = x.shape[-1]
         x2d = _rows(x, K, cdt)
         need_bwd = any(ctx.needs_input_grad)
+        # per-image coefficients (per_sample.py): every member is bound, one table per problem. The table
+        # replaces scale and selector, so neither is read: a graph captured here holds no copy of a
+        # selector weight that set_lora_diag may free (per-sample graphs outlive selector changes)
+        bound = members[0]._lb.ps is not None
         probs, meta = [], []
         for i, m in enumerate(members):
             A, B = factors[2 * i], factors[2 * i + 1]
             st: _SiteState = m._lb
             w16, _ = st.frozen(m.linear.weight, cdt, need_t=False)
-            diag = m._selector_diag()
-            scale = float(m.scale)
+            diag = None if bound else m._selector_diag()
+            scale = 1.0 if bound else float(m.scale)
             probs.append((x2d, w16, st.bias32(m.linear.bias), st.down16(A, cdt), _fp32_master(B), m.r, 1,
                           diag, scale, m.r))
             meta.append((diag, scale))
-        ys, Ts = ops.fused_linear_grouped(probs, odt, need_bwd)
+        if not bound:
+            ys, Ts = ops.fused_linear_grouped(probs, odt, need_bwd)
+        else:
+            ys, Ts = ops.fused_linear_grouped(probs, odt, False,
+                                              coef_rows=[per_sample.coef_rows(m, x, K) for m in members])
         ctx.members, ctx.meta, ctx.cdt = members, meta, cdt
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         ctx.save_for_backward(x2d, *[t for t in Ts if t is not None], *factors)
@@ -171,11 +179,12 @@ class _GroupedLoraLinearFn(torch.autograd.Function):
 def _site_sig(m):
     """Everything of a site that the parked output depends on besides the input: if any of it is
     edited between the family's launch and the sibling's own call (an external `.weight = ...`,
-    an in-place update, tune_lora_scale, set_lora_diag), the parked result is stale."""
+    an in-place update, tune_lora_scale, set_lora_diag, another per-sample table), the parked result is
+    stale."""
     from .modules import _key as mkey
     sel = m.selector
     return (mkey(m.linear.weight), mkey(m.linear.bias), mkey(m.lora_down.weight), mkey(m.lora_up.weight),
-            float(m.scale), mkey(getattr(sel, "weight", None)), m.training, m.dropout.p)
+            float(m.scale), mkey(getattr(sel, "weight", None)), m.training, m.dropout.p, per_sample.ps_sig(m))
 
 
 def forward_maybe_grouped(site, x):
@@ -213,7 +222,8 @@ def forward_maybe_grouped(site, x):
     fam = st.groups[id(site)]
     if fam is None:
         return None
-    members = tuple(m for m in fam if _plain(m, x) and m.r <= 16)
+    bound = site._lb.ps is not None      # per-sample members launch together, apart from unbound ones
+    members = tuple(m for m in fam if _plain(m, x) and m.r <= 16 and (m._lb.ps is not None) == bound)
     if len(members) < 2 or not any(m is site for m in members):
         return None
     factors = []

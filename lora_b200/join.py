@@ -119,6 +119,17 @@ class LoRAManager:
                                            torch.as_tensor(self.ranklist))
         set_lora_diag(self.pipe.unet, per_rank)
 
+    def diag_rows(self, per_image_scales) -> torch.Tensor:
+        """The selector diagonals `tune()` would set, one row per image: per_image_scales is B lists of
+        one strength per file; returns [B, total_rank] fp32, for `per_sample_lora(diag=...)` or the
+        samplers' `lora_diag={"unet": ...}` (every image of one batch with its own mix)."""
+        rows = []
+        for scales in per_image_scales:
+            assert len(scales) == len(self.ranklist), "Scale list should be the same length as ranklist"
+            rows.append(torch.repeat_interleave(torch.as_tensor(scales, dtype=torch.float32),
+                                                torch.as_tensor(self.ranklist)))
+        return torch.stack(rows)
+
     def prompt(self, prompt):
         if prompt is None:
             return prompt

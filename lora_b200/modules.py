@@ -124,6 +124,7 @@ class _SiteState:
         self.conv_tables = {}  # ops.conv_tap_table's tables: they follow the factor's shape, never its values
         self.grad_sink = None  # (gA view, gB view) when the arena owns the gradients
         self.parent = None     # weakref to the module this site was injected into (grouping.py)
+        self.ps = None         # (coefficient table [S, r] fp32, S) bound by per_sample.py, or None
 
     # caches and the parent back-reference are per-process runtime state: a copied / pickled module
     # starts with an empty one (copy.deepcopy(model), torch.save(model) keep working)
@@ -374,6 +375,9 @@ class LoraInjectedLinear(nn.Module):
 
     def forward(self, input):
         ops.wgrad_segment_boundary()
+        if self._lb.ps is not None:   # per-image coefficients (per_sample.py)
+            from .per_sample import linear_forward
+            return linear_forward(self, input)
         if self.r > ops.MAX_RANK:   # joined LoRAs above rank 64 (lora_manager.py:13-71): rank chunks of 64
             from .rank_chunks import lora_linear_chunked
             return lora_linear_chunked(self, input)
@@ -430,6 +434,9 @@ class LoraInjectedConv2d(nn.Module):
 
     def forward(self, input):
         ops.wgrad_segment_boundary()
+        if self._lb.ps is not None:   # per-image coefficients (per_sample.py)
+            from .per_sample import conv_forward
+            return conv_forward(self, input)
         from .conv_path import lora_conv2d
         return lora_conv2d(self, input)
 

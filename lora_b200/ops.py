@@ -190,22 +190,47 @@ def _w_arg(w16, K):
     return ptr(w16), w16.shape[0], 0
 
 
+def _coef_args(coef_rows, r: int):
+    """(table, ld, rows_per_sample, S) of a per-sample coefficient argument, checked."""
+    table, ld, rps, S = coef_rows
+    _req_cuda(table)
+    ld, rps, S = int(ld), int(rps), int(S)
+    assert table.dtype == torch.float32 and ld >= r and rps >= 1 and S >= 1
+    # row b of the table starts b * ld elements in: a 2-D table must have that row pitch
+    assert table.dim() in (1, 2) and table.stride(-1) == 1 and (table.dim() == 1 or table.stride(0) == ld)
+    assert table.numel() >= (S - 1) * ld + r
+    return table, ld, rps, S
+
+
 def fused_linear(x2d: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.Tensor],
                  down16: torch.Tensor, up: torch.Tensor, up_rs: int, up_cs: int,
                  diag: Optional[torch.Tensor], scale: float, r: int, out_dtype,
                  want_t: bool, t_in: Optional[torch.Tensor] = None, drop_p: float = 0.0,
-                 seed: Optional[torch.Tensor] = None
+                 seed: Optional[torch.Tensor] = None, coef_rows=None
                  ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """Y = x2d.w16^T + bias + ((x2d.down16^T) * scale*diag) . up^T ; returns (Y, T or None).
     down16: [RP, K] with RP = 16, 32 or 64 rows (the rank pad); T is [M, RP].
     t_in: use these rank-r activations [M,RP] instead of x2d.down16^T (dropout backward).
-    drop_p > 0 (+ seed: int64[1] on the device): nn.Dropout on the branch, masked in the drain."""
+    drop_p > 0 (+ seed: int64[1] on the device): nn.Dropout on the branch, masked in the drain.
+    coef_rows = (table fp32 [S, ld] on the device, ld, rows_per_sample, S): per-sample coefficients in
+    place of scale*diag (lb_lora_linear_fwd_ps; row m takes table row (m // rows_per_sample) % S).
+    Forward only: no T, t_in or dropout; diag and scale are ignored."""
     _req_cuda(x2d, down16, up)
     M, K = x2d.shape
     wp, N, wflag = _w_arg(w16, K)
     rp = down16.shape[0]
     assert down16.shape == (rp, K) and rp in (16, 32, 64)
     assert x2d.is_contiguous() and down16.is_contiguous()
+    if coef_rows is not None:
+        assert not want_t and t_in is None and drop_p == 0.0, "per-sample coefficients: forward only"
+        table, ld, rps, S = _coef_args(coef_rows, r)
+        y = torch.empty((M, N), device=x2d.device, dtype=out_dtype)
+        check(_C.lib.lb_lora_linear_fwd_ps(ptr(x2d), wp, ptr(bias), ptr(down16), ptr(up), up_rs, up_cs,
+                                           ptr(table), ld, rps, S, ptr(y), M, K, N, r, rp,
+                                           dtype_code(x2d.dtype) | wflag, dtype_code(out_dtype), stream_ptr()),
+              "lb_lora_linear_fwd_ps")
+        _count()
+        return y, None
     y = torch.empty((M, N), device=x2d.device, dtype=out_dtype)
     t = torch.empty((M, rp), device=x2d.device, dtype=torch.float32) if want_t else None
     assert t_in is None or t_in.shape == (M, rp)
@@ -299,10 +324,12 @@ def fused_conv2d(x_nhwc: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.T
                  up_gs: int, diag: Optional[torch.Tensor], scale: float, r: int, cout: int,
                  kh: int, kw: int, pad_h: int, pad_w: int, per_tap: bool, out_dtype,
                  want_t: bool, t_in: Optional[torch.Tensor] = None, drop_p: float = 0.0,
-                 seed: Optional[torch.Tensor] = None
+                 seed: Optional[torch.Tensor] = None, coef_rows=None
                  ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """x_nhwc: a [N,C,H,W] tensor in channels_last memory format (NHWC bytes). Returns
-    (Y as [N,cout,H,W] channels_last, T [N*H*W,RP] or None); RP = down16.shape[0] (16, 32 or 64)."""
+    (Y as [N,cout,H,W] channels_last, T [N*H*W,RP] or None); RP = down16.shape[0] (16, 32 or 64).
+    coef_rows: per-sample coefficients as in fused_linear, pixel rows (img*H + h)*W + w
+    (lb_lora_conv2d_fwd_ps; forward direction only: no T, t_in, dropout or per-tap form)."""
     _req_cuda(x_nhwc, w16, down16, up)
     n, cin, h, w = x_nhwc.shape
     rp = down16.shape[0]
@@ -312,7 +339,14 @@ def fused_conv2d(x_nhwc: torch.Tensor, w16: torch.Tensor, bias: Optional[torch.T
     t = torch.empty((n * h * w, rp), device=x_nhwc.device, dtype=torch.float32) if want_t else None
     import ctypes
     up_ptr = ctypes.c_void_p(up.data_ptr() + 4 * up_off)
-    if drop_p > 0.0:     # forward with nn.Dropout on the branch: masked in the drain, one launch
+    if coef_rows is not None:
+        assert not want_t and t_in is None and drop_p == 0.0 and not per_tap and up_gs == 0
+        table, ld, rps, S = _coef_args(coef_rows, r)
+        check(_C.lib.lb_lora_conv2d_fwd_ps(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs, up_cs,
+                                           ptr(table), ld, rps, S, ptr(y), n, h, w, cin, cout, kh, kw, pad_h, pad_w,
+                                           r, rp, dtype_code(x_nhwc.dtype), dtype_code(out_dtype), stream_ptr()),
+              "lb_lora_conv2d_fwd_ps")
+    elif drop_p > 0.0:     # forward with nn.Dropout on the branch: masked in the drain, one launch
         assert t_in is None and not per_tap and up_gs == 0 and seed is not None and seed.dtype == torch.int64
         check(_C.lib.lb_lora_conv2d_fwd_dropout(ptr(x_nhwc), ptr(w16), ptr(bias), ptr(down16), up_ptr, up_rs,
                                                 up_cs, ptr(diag), float(scale), ptr(y), ptr(t), n, h, w,
@@ -407,17 +441,20 @@ def merge_lora(W: torch.Tensor, up: torch.Tensor, down: torch.Tensor, alpha: flo
     return out
 
 
-def fused_linear_grouped(problems, out_dtype, want_t: bool):
+def fused_linear_grouped(problems, out_dtype, want_t: bool, coef_rows=None):
     """problems: list (<= 4) of (x2d, w16, bias32|None, down16, up32, up_rs, up_cs, diag|None, scale, r).
-    One launch; returns ([Y_i], [T_i or None])."""
+    One launch; returns ([Y_i], [T_i or None]). coef_rows: one (table, ld, rows_per_sample, S) per
+    problem, per-sample coefficients as in fused_linear (lb_lora_linear_fwd_grouped_ps; forward only)."""
     import ctypes
     n = len(problems)
     assert 1 <= n <= 4
+    assert coef_rows is None or (len(coef_rows) == n and not want_t)
     if any(p[3].shape[0] != R_PAD for p in problems):
         # the grouped kernel is built for rank pad 16 only (grouping.py groups only r <= 16 sites);
         # other callers with wider problems (bench.py's kernel sweep at --rank 32) get one launch each
-        outs = [fused_linear(x, w, b, d, up, rs, cs, diag, sc, r, out_dtype, want_t)
-                for (x, w, b, d, up, rs, cs, diag, sc, r) in problems]
+        outs = [fused_linear(x, w, b, d, up, rs, cs, diag, sc, r, out_dtype, want_t,
+                             coef_rows=None if coef_rows is None else coef_rows[i])
+                for i, (x, w, b, d, up, rs, cs, diag, sc, r) in enumerate(problems)]
         return [o[0] for o in outs], [o[1] for o in outs]
     VP, LL, I, F = ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int, ctypes.c_float
     ys, ts = [], []
@@ -445,6 +482,15 @@ def fused_linear_grouped(problems, out_dtype, want_t: bool):
     K = arr(I, [p[0].shape[1] for p in problems])
     N = arr(I, [p[1].shape[0] for p in problems])
     R = arr(I, [p[9] for p in problems])
+    if coef_rows is not None:
+        cargs = [_coef_args(c, p[9]) for c, p in zip(coef_rows, problems)]
+        check(_C.lib.lb_lora_linear_fwd_grouped_ps(
+            n, X, W, B, D, U, RS, CS, arr(VP, [c[0].data_ptr() for c in cargs]), arr(I, [c[1] for c in cargs]),
+            arr(I, [c[2] for c in cargs]), arr(I, [c[3] for c in cargs]), Y, M, K, N, R,
+            dtype_code(problems[0][0].dtype) | (LB_W_TILED if tiled else 0), dtype_code(out_dtype), stream_ptr()),
+            "lb_lora_linear_fwd_grouped_ps")
+        _count()
+        return ys, ts
     check(_C.lib.lb_lora_linear_fwd_grouped(n, X, W, B, D, U, RS, CS, DG, SC, Y, T, M, K, N, R,
                                             dtype_code(problems[0][0].dtype) | (LB_W_TILED if tiled else 0),
                                             dtype_code(out_dtype), stream_ptr()), "lb_lora_linear_fwd_grouped")

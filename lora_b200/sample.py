@@ -46,12 +46,21 @@ family: a capture of its own, while phi itself is a device scalar and changes pe
 The graphs are captured again only when something baked into a launch changes: a site's scale, a
 selector, the set of sites or their parameter storage, the grouping policy (`captures` counts them).
 
+Per-image LoRA coefficients: `sample(..., lora_scale={"unet": [..B], "text_encoder": 0.5},
+lora_diag={"unet": rows_BxR})` (model names as save_safeloras writes them; LoraXLSampler also takes
+"text_encoder_2") runs per-sample graphs, a capture key of their own: every sampled site reads its
+[B, r] coefficients (per_sample.py) from one static device table that the call rewrites before graph A,
+so they depend on the sites, ranks, factor storage and grouping only -- new values, tune_lora_scale,
+set_lora_diag and LoRAManager.tune between such calls cost no capture. `shared_noise=True` draws the
+noise as batch 1 from `seed` and copies it to every image (a strength sweep with one seed as one call).
+
 All noise (z_0 and each step's z_i) is one draw of [k + 1, B, C, h, w] from the sampler's own
 torch.Generator seeded by `seed`, then (img2img / inpaint) the posterior noise [B, C, h, w] of the one
 encoded image, in the VAE's dtype as DiagonalGaussianDistribution.sample draws it; the global CUDA RNG stream is never touched, so a training step's noise
 is the same with or without sampling in between. The models run in eval() under no_grad and get their
 train / eval modes back afterwards.
 """
+import contextlib
 from dataclasses import dataclass
 from typing import Optional
 
@@ -169,22 +178,27 @@ class LoraSampler:
         self._table_key = None
         self._graphs = {}             # (G, scheduler family[, "rescale"]) -> (A, B, C)
         self._fingerprint = None
+        self._ps_fingerprint = None   # the structural fingerprint the per-sample graphs were captured for
+        self._ps_buf = None           # per-sample graphs: the static coefficient table (per_sample.py layout)
         self._factor_bufs = []
         self._conv_tables = {}        # ops.conv_tap_table's row tables of the conv sites' down factors
         self.captures = 0
 
     # ------------------------------------------------------------------ what a capture bakes in
-    def _fingerprint_now(self):
-        """Everything of the models that a captured launch holds as a constant or an address."""
+    def _fingerprint_now(self, structural: bool = False):
+        """Everything of the models that a captured launch holds as a constant or an address. The
+        structural part (sites, ranks, factor storage, grouping) is all a per-sample graph depends on:
+        it reads scales and selectors from the static coefficient table."""
         from .grouping import get_grouping
         sig = []
         for m in _sites(*self._lora_models()):
             base = m.linear if hasattr(m, "linear") else m.conv
             sel = getattr(m.selector, "weight", None)
-            sig.append((id(m), float(m.scale), m.r, id(sel), None if sel is None else sel.data_ptr(),
-                        id(m.lora_down.weight), m.lora_down.weight.data_ptr(), m.lora_down.weight.dtype,
-                        id(m.lora_up.weight), m.lora_up.weight.data_ptr(), m.lora_up.weight.dtype,
-                        id(base.weight), base.weight.data_ptr()))
+            values = () if structural else (float(m.scale), id(sel), None if sel is None else sel.data_ptr())
+            sig.append((id(m), m.r) + values + (
+                id(m.lora_down.weight), m.lora_down.weight.data_ptr(), m.lora_down.weight.dtype,
+                id(m.lora_up.weight), m.lora_up.weight.data_ptr(), m.lora_up.weight.dtype,
+                id(base.weight), base.weight.data_ptr()))
         return get_grouping(), tuple(sig)
 
     def _collect_factor_buffers(self):
@@ -304,10 +318,15 @@ class LoraSampler:
         self.captures += 1
 
     def _graphs_for(self, key):
-        fp = self._fingerprint_now()
-        if fp != self._fingerprint:
-            self._graphs.clear()
-            self._fingerprint = fp
+        ps = "per_sample" in key
+        fp = self._fingerprint_now(structural=ps)
+        if fp != (self._ps_fingerprint if ps else self._fingerprint):
+            for k in [k for k in self._graphs if ("per_sample" in k) == ps]:
+                del self._graphs[k]
+            if ps:
+                self._ps_fingerprint = fp
+            else:
+                self._fingerprint = fp
         if key not in self._graphs:
             self._capture(key)
         return self._graphs[key]
@@ -390,13 +409,18 @@ class LoraSampler:
                num_inference_steps: Optional[int] = None, scheduler: Optional[str] = None,
                guidance_scale: Optional[float] = None, image: Optional[torch.Tensor] = None,
                mask_image: Optional[torch.Tensor] = None, strength: Optional[float] = None,
-               guidance_rescale: Optional[float] = None) -> torch.Tensor:
+               guidance_rescale: Optional[float] = None, lora_scale: Optional[dict] = None,
+               lora_diag: Optional[dict] = None, shared_noise: bool = False) -> torch.Tensor:
         """uint8 [B, 8h, 8w, 3] images (a view of `self.image`, overwritten by the next call) for the token
         ids [B, seq_len] of the prompts and of the negative prompts (the empty prompt's ids for plain
         classifier-free guidance; unused when guidance_scale <= 1). `self.latents` holds the final latents.
         img2img: image uint8 [B, 8h, 8w, 3], strength in (0, 1] (default cfg.strength); inpaint: image and
         mask_image uint8 [B, 8h, 8w] (0..255, >= 128 repainted). guidance_rescale: phi in [0, 1] (default
-        cfg.guidance_rescale), applied when guidance_scale > 1."""
+        cfg.guidance_rescale), applied when guidance_scale > 1.
+        lora_scale / lora_diag: per-image LoRA coefficients by model name ("unet", "text_encoder"; see
+        _per_sample_plan); shared_noise: every image gets the noise of a batch-1 call with this seed."""
+        plan = self._per_sample_plan(lora_scale, lora_diag)
+        self._check_shared_noise(shared_noise)
         n, sched, g, start = self._options(num_inference_steps, scheduler, guidance_scale, strength)
         phi = _check_phi(self.cfg.guidance_rescale if guidance_rescale is None else guidance_rescale)
         G = 2 if g > 1.0 else 1
@@ -413,15 +437,96 @@ class LoraSampler:
             if G == 2:
                 self.input_ids[:B].copy_(negative_input_ids)
 
-        return self._generate(n, sched, g, start, phi, seed, write_ids)
+        return self._generate(n, sched, g, start, phi, seed, write_ids, plan, shared_noise)
 
-    def _generate(self, n: int, sched: str, g: float, start: int, phi: float, seed: int, write_inputs):
+    # ------------------------------------------------------------------ per-image LoRA coefficients
+    def _model_names(self):
+        """The sampled models by their save_safeloras names."""
+        return {"unet": self.unet, "text_encoder": self.text_encoder}
+
+    def _per_sample_plan(self, lora_scale, lora_diag):
+        """None for a call without per-image coefficients; else {name: (scale [B] | None, diag [B, r] | None)},
+        validated (ValueError): known model names, models with LoRA sites, B values per scale, diag rows
+        [r] or [B, r] of the sites' one rank."""
+        if lora_scale is None and lora_diag is None:
+            return None
+        from . import per_sample
+        B = self.latents.shape[0]
+        names = self._model_names()
+        plan = {}
+        for what, arg in (("lora_scale", lora_scale), ("lora_diag", lora_diag)):
+            if arg is None:
+                continue
+            if not isinstance(arg, dict):
+                raise ValueError(f"{what} maps model names ({', '.join(names)}) to values, got {type(arg).__name__}")
+            for name in arg:
+                if name not in names:
+                    raise ValueError(f"{what}: unknown model {name!r}, one of {', '.join(names)}")
+        for name, model in names.items():
+            sc, dg = (lora_scale or {}).get(name), (lora_diag or {}).get(name)
+            if sc is None and dg is None:
+                continue
+            sites = per_sample.sites_of(model)
+            if not sites:
+                raise ValueError(f"{name} has no LoRA sites to scale per image")
+            try:
+                plan[name] = per_sample.check_args(sites, sc, dg, B)
+            except ValueError as e:
+                raise ValueError(f"{name}: {e}") from None
+        return plan
+
+    def _check_shared_noise(self, shared_noise: bool):
+        if shared_noise and self.cfg.external_noise:
+            raise ValueError("shared_noise draws the noise from the seed: not with SamplerConfig(external_noise=True)")
+
+    def _per_sample_tables(self, plan):
+        """Write the call's coefficients into the static table (allocated for these sites on first
+        use) and return (sites, per-site views): every sampled site is bound, those without
+        per-image values take their current scale and selector."""
+        from . import per_sample
+        B = self.latents.shape[0]
+        sites, parts = [], []
+        for name, model in self._model_names().items():
+            ms = per_sample.sites_of(model)
+            sc, dg = plan.get(name, (None, None))
+            sites += ms
+            sel = per_sample.selector_diags(ms) if dg is None else {}     # one read of the selectors
+            parts += [per_sample.site_rows(m, sc, dg, B, sel).reshape(-1) for m in ms]
+        flat = torch.cat(parts) if parts else torch.zeros(0)
+        if self._ps_buf is None or self._ps_buf.numel() != flat.numel():
+            self._ps_buf = torch.empty(flat.numel(), device=self.device, dtype=torch.float32)
+        self._ps_buf.copy_(flat)
+        return sites, per_sample.table_views(self._ps_buf, sites, B)
+
+    def _draw_noise(self, k: int, seed: int, shared: bool):
+        """z_0 and the steps' noise (and the posterior noise) from the sampler's generator; shared: drawn
+        once as batch 1, as a batch-1 call with this seed draws it, and copied to every image."""
+        self.generator.manual_seed(int(seed))
+        image_task = self.cfg.task != "txt2img"
+        if not shared:
+            self.noise[:k + 1].normal_(generator=self.generator)
+            if image_task:
+                self.posterior_noise.normal_(generator=self.generator)
+            return
+        one = torch.empty((k + 1, 1) + tuple(self.noise.shape[2:]), device=self.device, dtype=self.noise.dtype)
+        one.normal_(generator=self.generator)
+        self.noise[:k + 1].copy_(one.expand(-1, self.noise.shape[1], -1, -1, -1))
+        if image_task:
+            p1 = torch.empty((1,) + tuple(self.posterior_noise.shape[1:]), device=self.device,
+                             dtype=self.posterior_noise.dtype)
+            p1.normal_(generator=self.generator)
+            self.posterior_noise.copy_(p1.expand_as(self.posterior_noise))
+
+    def _generate(self, n: int, sched: str, g: float, start: int, phi: float, seed: int, write_inputs,
+                  plan=None, shared_noise: bool = False):
         """The call's tables, scalars, inputs (write_inputs()) and noise, then the graphs (or the eager
-        path): the part of sample() every sampler shares."""
+        path): the part of sample() every sampler shares. plan (per-image LoRA coefficients): the
+        per-sample graphs, with every sampled site bound to the static coefficient table."""
+        from . import per_sample
         k = n - start
         G = 2 if g > 1.0 else 1
         rescale = G == 2 and phi > 0.0
-        key = self._key(G, schedulers.family(sched), rescale)
+        key = self._key(G, schedulers.family(sched), rescale) + (("per_sample",) if plan is not None else ())
         saved = self._enter_eval()
         try:
             with torch.no_grad():
@@ -431,18 +536,20 @@ class LoraSampler:
                     self.guidance_rescale.fill_(phi)
                 write_inputs()
                 if not self.cfg.external_noise:
-                    self.generator.manual_seed(int(seed))
-                    self.noise[:k + 1].normal_(generator=self.generator)
-                    if self.cfg.task != "txt2img":
-                        self.posterior_noise.normal_(generator=self.generator)
-                if self.cfg.use_cuda_graph:
-                    ga, gb, gc = self._graphs_for(key)
-                    ga.replay()
-                    for _ in range(k):
-                        gb.replay()
-                    gc.replay()
-                else:
-                    self._run_eager(G, k, key[1], rescale)
+                    self._draw_noise(k, seed, shared_noise)
+                binding = contextlib.nullcontext()
+                if plan is not None:
+                    sites, views = self._per_sample_tables(plan)
+                    binding = per_sample.bound(sites, views, self.latents.shape[0])
+                with binding:
+                    if self.cfg.use_cuda_graph:
+                        ga, gb, gc = self._graphs_for(key)
+                        ga.replay()
+                        for _ in range(k):
+                            gb.replay()
+                        gc.replay()
+                    else:
+                        self._run_eager(G, k, key[1], rescale)
         finally:
             self._restore_modes(saved)
         return self.image
@@ -511,6 +618,9 @@ class LoraXLSampler(LoraSampler):
     def _lora_models(self):
         return (self.unet, self.text_encoder, self.text_encoder_2)
 
+    def _model_names(self):
+        return {"unet": self.unet, "text_encoder": self.text_encoder, "text_encoder_2": self.text_encoder_2}
+
     def _key(self, G: int, family: str, rescale: bool):
         zeros = G == 2 and self._zero_negatives
         return super()._key(G, family, rescale) + (("zero_negatives",) if zeros else ())
@@ -543,11 +653,16 @@ class LoraXLSampler(LoraSampler):
                seed: int = 0, original_size=None, crops_coords_top_left=(0, 0), target_size=None,
                guidance_rescale: Optional[float] = None, num_inference_steps: Optional[int] = None,
                scheduler: Optional[str] = None, guidance_scale: Optional[float] = None,
-               image: Optional[torch.Tensor] = None, strength: Optional[float] = None) -> torch.Tensor:
+               image: Optional[torch.Tensor] = None, strength: Optional[float] = None,
+               lora_scale: Optional[dict] = None, lora_diag: Optional[dict] = None,
+               shared_noise: bool = False) -> torch.Tensor:
         """uint8 [B, 8h, 8w, 3] images (a view of `self.image`) for the two tokenizers' ids [B, seq_len] of
         the prompts. The negative prompts' ids come as a pair or not at all (zeroed negatives).
         original_size and target_size default to (8h, 8w); with crops_coords_top_left they make each
-        sample's time ids. img2img: image uint8 [B, 8h, 8w, 3] and strength, as LoraSampler.sample."""
+        sample's time ids. img2img: image uint8 [B, 8h, 8w, 3] and strength, as LoraSampler.sample.
+        lora_scale / lora_diag / shared_noise as LoraSampler.sample, with "text_encoder_2" a model name too."""
+        plan = self._per_sample_plan(lora_scale, lora_diag)
+        self._check_shared_noise(shared_noise)
         n, sched, g, start = self._options(num_inference_steps, scheduler, guidance_scale, strength)
         phi = _check_phi(self.cfg.guidance_rescale if guidance_rescale is None else guidance_rescale)
         G = 2 if g > 1.0 else 1
@@ -576,4 +691,4 @@ class LoraXLSampler(LoraSampler):
                 self.input_ids_2[:B].copy_(negative_input_ids_2)
             self.time_ids.copy_(torch.tensor(sizes, dtype=torch.float32).expand(2 * B, 6))
 
-        return self._generate(n, sched, g, start, phi, seed, write_inputs)
+        return self._generate(n, sched, g, start, phi, seed, write_inputs, plan, shared_noise)
